@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- aggregate detection FPS on synthetic 640x480 streams (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W            our arm (B200, libwatsor_b200.so)
+    python bench.py --gpus N --steps K --warmup W            our arm (H100, libwatsor_b200.so)
     python bench.py --impl reference --gpus N --steps K ...  CPU arm: the reference path's CPU
                                                              restatement (oracle/), all host threads
 
@@ -17,7 +17,8 @@ confidence/area/mask-zone predicates -> Detection[100] per frame.
   value  device-timed throughput with frames already resident in HBM (ring of distinct frames per
          camera, larger than L2, so every step reads its input from HBM), exactly K steps
   e2e    same metric through the public detector API with HOST frames in pinned memory:
-         H2D of every frame and D2H of every Detection block inside the timed region
+         H2D of every frame and D2H of every Detection block inside the timed region, K steps
+         (--min-seconds S adds *_long records timed over at least S seconds)
   config.real_weights   the same two numbers on the only model with real weights (the reference's vendored
          3-class SSD-MobileNet-v1, watsor/test/model/cpu.pb), porch mask on camera 0
   e2e_worker   the same metric through the drop-in worker process (watsor_b200.detection.detector.ObjectDetector
@@ -28,6 +29,10 @@ Multi-GPU: one process per GPU (torchrun), cameras sharded, no data-path collect
 N>1 line adds a `scatter` record: the same steps with the NCCL frame scatter from rank 0 that BASELINE.json's
 north star names, through the library's own collective (wb_comm_init / wb_scatter_frames; --scatter-impl torch
 runs torch.distributed.scatter instead).
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller (rank 0): the
+Detection rows and filter verdicts of every camera as float64 .npy files, so that two builds can be compared output
+for output on identical inputs (the frames and the ring schedule depend only on the arguments).
 """
 import argparse
 import json
@@ -45,7 +50,7 @@ sys.path.insert(0, ROOT)
 METRIC = 'aggregate detection FPS on synthetic 640x480 streams'
 UNIT = 'frames/s'
 W, H = 640, 480
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024   # H100 SXM
 
 
 def parse_args():
@@ -60,7 +65,7 @@ def parse_args():
                         'backbone, 90-class heads; shapes: vendored 3-class SSD-MobileNet-v1 (real weights); '
                         'inception: SSD-Inception-v2, 90 classes, 1920x1080 frames (BASELINE configs[4]; use --cameras 2)')
     p.add_argument('--precision', default='tf32x3', choices=['fp32', 'tf32x3', 'bf16'],
-                   help='fp32: CUDA-core FFMA convs; tf32x3: fp32-faithful tcgen05 (3xTF32 split); bf16: tcgen05 bf16')
+                   help='fp32: CUDA-core FFMA convs; tf32x3: fp32-faithful wgmma (3xTF32 split); bf16: wgmma bf16')
     p.add_argument('--frames', default='artist', choices=['artist', 'random'])
     p.add_argument('--ingest', default='local', choices=['local', 'scatter'])
     p.add_argument('--inflight', type=int, default=6, help='batches kept in flight (library slots, max 6)')
@@ -73,8 +78,10 @@ def parse_args():
                         'torch.distributed.scatter')
     p.add_argument('--no-worker', action='store_true', help='skip the e2e_worker record')
     p.add_argument('--no-effects', action='store_true', help='skip the visual-effects record')
-    p.add_argument('--min-seconds', type=float, default=1.0,
-                   help='the *_long / e2e measurements run at least this long')
+    p.add_argument('--min-seconds', type=float, default=0.0,
+                   help='also time *_long records of at least this many seconds (default: every timed loop is K steps)')
+    p.add_argument('--dump-outputs', metavar='DIR', default=None,
+                   help='write the outputs of the last timed step as DIR/<name>.npy (float64)')
     return p.parse_args()
 
 
@@ -82,7 +89,7 @@ def parse_args():
 def load_model(kind):
     from watsor_b200.model import Model, synthetic_ssd_mobilenet_v1
     from tests.workload import v2_coco_model
-    blob = os.path.join(ROOT, 'models', '_ref', 'ssd_mobilenet_v1_shapes', 'b200.wb200')
+    from oracle.reference_build import MODEL_BLOB as blob
     if kind == 'shapes' and os.path.isfile(blob):
         return Model.load(blob), 'ssd_mobilenet_v1 300x300, 3 classes, real weights (watsor/test/model/cpu.pb)'
     if kind == 'shapes':
@@ -426,6 +433,14 @@ class Arm:
         self.torch.cuda.synchronize()
         return self.reduce_max(time.perf_counter() - t0)
 
+    def outputs_of_slot(self, s):
+        """What det.collect() handed back for slot `s`: per camera 100 Detection rows and their filter verdicts."""
+        rows = self.out_rows[s]
+        det = np.array([[(r.label, r.confidence, r.bounding_box.x_min, r.bounding_box.y_min, r.bounding_box.x_max,
+                          r.bounding_box.y_max) for r in cam] for cam in rows], dtype=np.float64)
+        zones = np.array([[list(r.zones) for r in cam] for cam in rows], dtype=np.float64)
+        return {'detections': det, 'zones': zones, 'verdicts': np.array(self.out_verd[s], dtype=np.float64)}
+
     def measure(self, want_long=True):
         """-> dict with value / e2e (+ *_long when the K-step region is shorter than --min-seconds)."""
         args, world, C = self.args, self.world, self.C
@@ -447,6 +462,7 @@ class Arm:
         self.run_device_steps(warm, 0)
         launches = self.det.engine.last_launch_count()
         dev_ms, t_wall = self.time_device(args.steps, args.warmup)
+        self.last_outputs = self.outputs_of_slot((args.steps - 1) % self.NS)
         out = {'value': world * C * args.steps / (dev_ms / 1e3), 'ms_per_step': dev_ms / args.steps,
                'launches_per_step': launches, 'wall_ms_per_step_device_loop': 1e3 * t_wall / args.steps,
                'prime_steps': self.prime_steps,
@@ -515,10 +531,7 @@ def main():
     import torch.distributed as dist
 
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py --impl b200 needs a B200; there is no CPU fallback')
-    # with several batches in flight the persistent GEMM should not pin every SM: leaving ~20 % of them to the
-    # other streams' kernels measured +4 % (148 -> 116 CTAs); single-stream users keep the default (all SMs)
-    os.environ.setdefault('WB_PERSIST_CTAS', '116')
+        raise SystemExit('bench.py --impl b200 needs an H100; there is no CPU fallback')
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group('nccl', device_id=torch.device('cuda', local_rank))
@@ -529,6 +542,10 @@ def main():
     if args.ingest == 'scatter' and world > 1:
         arm.enable_scatter()
     m = arm.measure()
+    if rank == 0 and args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in arm.last_outputs.items():
+            np.save(os.path.join(args.dump_outputs, name + '.npy'), a)
     scatter = None
     if world > 1 and args.ingest == 'local' and not args.no_scatter:
         scatter = arm.measure_scatter(m['ms_per_step'])
@@ -601,8 +618,7 @@ def main():
                 'camera_to_gpu': 'camera c -> rank c // %d (contiguous blocks; BASELINE.md suggests c mod G, '
                                  'equivalent for independent cameras)' % C,
                 'precision': args.precision, 'batches_in_flight': arm.NS,
-                'persistent_gemm_ctas': int(os.environ.get('WB_PERSIST_CTAS', '0')),
-                'l2': 'input ring of %d distinct frames per camera (%.0f MB per GPU) > 126 MB L2; no flush needed'
+                'l2': 'input ring of %d distinct frames per camera (%.0f MB per GPU) > 50 MB L2; no flush needed'
                       % (arm.ring, arm.ring * C * arm.frame_bytes / 1e6),
                 'detections_per_frame': m['detections_per_frame'],
                 'passed_filters_per_frame': m['passed_filters_per_frame'],
@@ -677,7 +693,7 @@ def measure_effects(args, local_rank, torch):
         wall = (time.perf_counter() - t0) / reps
         eng.close()
         alg = C * W * H * 11
-        peak = 6650.0
+        peak = 3350.0                   # H100 SXM data sheet, HBM3
         pk = os.path.join(ROOT, 'MEASURED_PEAKS.json')
         if os.path.isfile(pk):
             peak = json.load(open(pk)).get('hbm_gbs', peak)
@@ -747,27 +763,18 @@ def measure_roofline(det, model, dev_ring, C, cam_ids, precision):
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.isfile(p):
         peaks = json.load(open(p))
-    hbm = peaks.get('hbm_gbs', 6650.0)
-    tf = peaks.get('bf16_tflops_sustained', 1400.0)
-    src = 'measured (MEASURED_PEAKS.json)' if peaks else 'fallback (B200_PROFILING.md)'
+    hbm = peaks.get('hbm_gbs', 3350.0)
+    tf = peaks.get('bf16_tflops_sustained', 989.0)
+    src = ('measured (MEASURED_PEAKS.json)' if peaks else
+           'H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense BF16 at 700 W; not reached here)')
     if dom == 'gemm':
         ach = d['flops'] / (d['ms'] / 1e3) / 1e12
         roof = {'bound': 'tensor', 'achieved': ach, 'peak': tf, 'unit': 'TFLOP/s', 'frac': ach / tf}
     else:
         ach = d['bytes'] / (d['ms'] / 1e3) / 1e9
         roof = {'bound': 'hbm', 'achieved': ach, 'peak': hbm, 'unit': 'GB/s', 'frac': ach / hbm}
-    # DRAM bytes per launch of the dominant family from the committed ncu --set full capture of this model
-    # (profiles/r02_traffic.json: {model name: {precision: {family: {dram_bytes_per_launch}}}}), batch 8 only
-    traffic = None
-    prec_name = {0: 'fp32', 1: 'bf16', 2: 'tf32x3'}[precision]
-    tp = os.path.join(ROOT, 'profiles', 'r02_traffic.json')
-    if os.path.isfile(tp) and C == 8:
-        t = json.load(open(tp)).get(model.name, {}).get(prec_name, {}).get(dom)
-        if t:
-            traffic = t['dram_bytes_per_launch']
-    roof.update({'traffic': traffic, 'traffic_unit': 'bytes of DRAM read+write per launch (ncu capture in profiles/, batch 8)',
-                 'algorithmic_bytes_per_launch': d['bytes'] / max(1, d['launches']),
-                 'kernel': {'gemm': 'tcgen05 GEMM family: k_gemm_tc / k_gemm_tc_persist / fused kernels (1x1 convs, 3x3 extras, heads)',
+    roof.update({'algorithmic_bytes_per_launch': d['bytes'] / max(1, d['launches']),
+                 'kernel': {'gemm': 'wgmma GEMM family: k_gemm_tc / k_dwpw_tc_x3 (1x1 convs, 3x3 extras, heads)',
                             'dw': 'k_dw_strip', 'stem': 'k_stem', 'add': 'k_add',
                             'post': 'k_decode_scores+k_nms+k_merge_filter'}.get(dom, dom),
                  'peak_source': src, 'share_of_step': d['ms'] / total, 'launches_per_step': d['launches'],
@@ -779,8 +786,7 @@ def measure_roofline(det, model, dev_ring, C, cam_ids, precision):
                  'families_hbm_frac': {n: round(f['bytes'] / (f['ms'] / 1e3) / 1e9 / hbm, 4) for n, f in fam.items()
                                        if f['ms'] > 0},
                  'note': 'per-layer CUDA events, every layer launched 10x back to back (median of 5 runs); '
-                         'TF32X3 issues 3 TF32 MMAs per product, so its tensor ceiling is bf16 peak/6 (frac_of_mode_ceiling); '
-                         'traffic from ncu is in profiles/'})
+                         'TF32X3 issues 3 TF32 MMAs per product, so its tensor ceiling is bf16 peak/6 (frac_of_mode_ceiling)'})
     return roof, table
 
 

@@ -1,5 +1,5 @@
 /*
- * watsor_b200.h -- C-ABI of libwatsor_b200.so: the B200-native (sm_100a) detection hot path of
+ * watsor_b200.h -- C-ABI of libwatsor_b200.so: the H100-native (sm_90a) detection hot path of
  * asmirnou/watsor behind plain pointers and sizes.  No torch / CUDA types appear in any signature;
  * device pointers and streams travel as void* / integers.
  *
@@ -73,8 +73,8 @@ int wb_device_count(int* count);
 /* replaces TensorRTObjectDetector.__init__ / __enter__ (watsor/detection/tensorrt_gpu.py:23-57) and
  * TensorFlowObjectDetector.__init__ (tensorflow_cpu.py:13-25): builds the device-resident model from
  * a compiled model blob (watsor_b200/model.py writes it from frozen_inference_graph.pb / cpu.pb).
- * precision: 0 = fp32 storage, dense convs on CUDA cores (FFMA); 1 = bf16 storage, tcgen05 kind::f16 (fast mode, not
- * a parity mode); 2 = fp32 storage, dense convs as 3xTF32 tcgen05 MMAs with fp32 accumulation (fp32-faithful: the
+ * precision: 0 = fp32 storage, dense convs on CUDA cores (FFMA); 1 = bf16 storage, bf16 wgmma (fast mode, not
+ * a parity mode); 2 = fp32 storage, dense convs as 3xTF32 wgmma MMAs with fp32 accumulation (fp32-faithful: the
  * default of the Python host and what bench.py reports); 3 = single TF32 MMA (diagnostic). */
 int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_batch, int precision,
               wb_ctx** out);
@@ -123,7 +123,7 @@ int wb_detect(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_t* c
 /* asynchronous form of wb_detect over slots 0..5 (stream + arena + staging each): submit() enqueues H2D +
  * kernels + D2H on the slot's stream and returns; collect() waits and scatters results.  Lets host ingest of
  * batch k+1 overlap the kernels of batch k (the reference overlaps them with processes, detector.py:40-50),
- * and several batches in flight are what keeps a B200's SMs busy (DESIGN.md 4.5).  Thread-safe: a mutex in
+ * and several batches in flight are what keeps the GPU's SMs busy (DESIGN.md 4.5).  Thread-safe: a mutex in
  * the context serialises the calls that touch shared state. */
 int wb_submit(wb_ctx* ctx, int slot, int n, const uint8_t* const* frames, const int32_t* cam_ids,
               uint32_t flags);

@@ -6,7 +6,7 @@ reference`` legs may import it, and only as the checker or the reported CPU
 baseline.  ``watsor_b200`` never imports it; the product path fails loudly when
 the CUDA library is missing.
 
-What it restates (all citations into /root/reference, asmirnou/watsor @127f125):
+What it restates (all citations into upstream asmirnou/watsor @127f125):
 
 * watsor/detection/tensorflow_cpu.py:74-121 -- feed a uint8 HWC frame to the
   frozen TF Object-Detection graph, fetch detection_boxes/scores/classes, convert

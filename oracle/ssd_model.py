@@ -2,8 +2,8 @@
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).  Same arithmetic as
 oracle/ssd_graph.py (it inherits preprocess / decode / NMS / post-process from it); only
-the source of the layer list and constants differs.  This is the form that travels to the
-GPU box (no /root/reference there): tests/test_oracle_model.py checks here, where the
+the source of the layer list and constants differs.  This is the form the GPU tests use
+(they never read the GraphDef): tests/test_model.py checks, where the
 GraphDef is available, that both forms agree bit for bit on the vendored model, so a
 parity test against this class is a parity test against the GraphDef restatement.
 Synthetic-weight architectures (90-class heads) exist only in this form.

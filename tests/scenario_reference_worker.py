@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""The reference's only model test, restated with the reference's OWN stream runtime and the real B200 back-end
+"""The reference's only model test, restated with the reference's OWN stream runtime and the real H100 back-end
 (ref: watsor/test/test_detect.py:28-77): an Artist thread draws shapes into a shared `FrameBuffer`, the detector
 runs in a separate *process* under `spawn`, the DetectionSieve filters confidence >= 50 %, a ShapeCounter counts
 labelled detections and the test passes when 100 have been seen.
 
 Run as a script in a fresh interpreter (tests/test_gpu_worker.py does) with the reference package on PYTHONPATH
-(`baseline/_ref`, installed by __graft_entry__.build() with pip from /root/reference): the detector module must
+(oracle/_ref/site, copied by __graft_entry__.build() from an upstream checkout): the detector module must
 bind to `watsor.stream.*` at import time, here and in the spawned child.
 
 Everything from `watsor.*` below is the reference's code; `create_object_detectors`, `ObjectDetector`,
@@ -65,7 +65,7 @@ def main(width=100, height=100, wanted=100, wait_s=90.0):
                                                          {get_coco_class(3).label: {'confidence': 50}}]})])]
     sieve = DetectionSieve('sieve', stop, log_queue, sieve_queue, frame_buffer, filters, RateLimiter())
     counter = ShapeCounter(Thread, 'counter', stop, log_queue, subscriber_queue, frame_buffer, latch)
-    model_path = os.path.join(ROOT, 'models', '_ref', 'ssd_mobilenet_v1_shapes')
+    from oracle.reference_build import MODEL_DIR as model_path
     detectors = det_mod.create_object_detectors(Process, stop, log_queue, frame_queue, {artist.name: frame_buffer},
                                                 model_path)
     processes = [artist, sieve, counter] + detectors[:1]

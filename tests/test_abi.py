@@ -6,7 +6,8 @@ import re
 
 import pytest
 
-from tests.conftest import ROOT, has_gpu
+from tests.conftest import REF_DIR, ROOT, has_gpu
+from tests.reference_golden import upstream
 from watsor_b200 import _lib
 from watsor_b200.stream.share import BoundingBox, Detection, Frame, FrameBuffer, Header
 
@@ -22,22 +23,25 @@ def test_struct_layout_matches_reference_share_py():
             Header.detections.offset) == (0, 4, 8, 16, 24)
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='reference tree not present')
 def test_struct_layout_equals_reference_module():
-    import importlib.util
-    import sys
-    sys.path.insert(0, '/root/reference')
-    try:
-        spec = importlib.util.spec_from_file_location('ref_share', '/root/reference/watsor/stream/share.py')
-        ref = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(ref)
-    finally:
-        sys.path.remove('/root/reference')
+    def theirs():
+        import importlib.util
+        import sys
+        sys.path.insert(0, REF_DIR)
+        try:
+            spec = importlib.util.spec_from_file_location('ref_share', os.path.join(REF_DIR, 'watsor', 'stream', 'share.py'))
+            ref = importlib.util.module_from_spec(spec)
+            spec.loader.exec_module(ref)
+        finally:
+            sys.path.remove(REF_DIR)
+        return {name: {'size': ctypes.sizeof(getattr(ref, name)),
+                       'fields': [[f[0], getattr(getattr(ref, name), f[0]).offset] for f in getattr(ref, name)._fields_]}
+                for name in ('BoundingBox', 'Detection', 'Header')}
+    ref = upstream('share_layout', 'structs', theirs)
     for name in ('BoundingBox', 'Detection', 'Header'):
-        ours, theirs = globals()[name], getattr(ref, name)
-        assert ctypes.sizeof(ours) == ctypes.sizeof(theirs)
-        assert [(f[0], getattr(ours, f[0]).offset) for f in ours._fields_] == \
-               [(f[0], getattr(theirs, f[0]).offset) for f in theirs._fields_]
+        ours = globals()[name]
+        assert ctypes.sizeof(ours) == ref[name]['size']
+        assert [[f[0], getattr(ours, f[0]).offset] for f in ours._fields_] == ref[name]['fields']
 
 
 def test_frame_buffer_shared_memory_view():

@@ -22,7 +22,7 @@ def detector(shapes_model, request):
 
 
 def test_device_name(detector):
-    assert 'B200' in detector.device_name and len(detector.device_name.encode()) < 255
+    assert 'H100' in detector.device_name and len(detector.device_name.encode()) < 255
 
 
 def test_golden_cases_single_frame_protocol(detector, golden):

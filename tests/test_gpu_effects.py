@@ -137,18 +137,13 @@ def test_errors_are_loud(engine):
     assert np.array_equal(out, img)
 
 
-def test_equal_to_the_reference_classes_installed_under_baseline_ref(engine):
-    """The UNMODIFIED reference package (baseline/_ref, installed by __graft_entry__.build(), travels to the GPU box)
-    provides watsor.output.{blend,draw,copy}: run the reference's own effect chain on the CPU and the fused GPU effect
-    on the same frame and rows.  watsor.filter.mask imports shapely (absent): an empty stand-in satisfies the import."""
+def reference_chain(config, img, rows):
+    """SHA-256 of the reference's own effect chain (blend + draw with contours, or copy + draw) on `img`."""
+    import hashlib
     import sys
     import types
 
-    from tests.conftest import ROOT
-    from watsor_b200.output.effects import FusedEffects
-    ref_root = os.path.join(ROOT, 'baseline', '_ref')
-    if not os.path.isfile(os.path.join(ref_root, 'watsor', 'output', 'draw.py')):
-        pytest.skip('baseline/_ref not installed')
+    from tests.conftest import REF_DIR
     saved = {k: v for k, v in sys.modules.items() if k == 'shapely' or k.startswith('shapely.') or
              k == 'watsor' or k.startswith('watsor.')}
     for k in saved:
@@ -157,38 +152,52 @@ def test_equal_to_the_reference_classes_installed_under_baseline_ref(engine):
     geometry.Polygon = object
     shapely.geometry = geometry
     sys.modules['shapely'], sys.modules['shapely.geometry'] = shapely, geometry
-    sys.path.insert(0, ref_root)
+    sys.path.insert(0, REF_DIR)
     try:
         from watsor.output.blend import BlendEffect as RefBlend
         from watsor.output.copy import CopyImageEffect as RefCopy
         from watsor.output.draw import DrawEffect as RefDraw
         from watsor.output.draw import DrawEffectWithContours as RefDrawContours
         from watsor.stream.share import Detection as RefDetection
-        w, h = 640, 480
-        rng = np.random.default_rng(21)
-        with TemporaryDirectory() as tmp:
-            alpha = random_alpha(rng, w, h, 4)
-            path = os.path.join(tmp, 'mask.png')
-            assert cv2.imwrite(path, np.dstack([np.zeros((h, w, 3), np.uint8), alpha]))
-            for config in ({'mask': path, 'width': w, 'height': h}, {'width': w, 'height': h}):
-                img = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
-                rows = random_rows(rng, w, h, 20, n_zones=4 if 'mask' in config else 0)
-                theirs_hdr = types.SimpleNamespace(
-                    detections=(RefDetection * len(rows)).from_buffer_copy(bytes(rows)))
-                theirs = np.zeros_like(img)
-                if 'mask' in config:
-                    RefBlend(config).apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
-                    RefDrawContours(config).apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
-                else:
-                    RefCopy().apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
-                    RefDraw().apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
-                ours = np.zeros_like(img)
-                hdr = header_of(rows)
-                FusedEffects(config, engine).apply(img, ours, img.shape, hdr, hdr)
-                assert np.array_equal(theirs, ours), ('mask' in config, int((theirs != ours).sum()))
+        theirs_hdr = types.SimpleNamespace(detections=(RefDetection * len(rows)).from_buffer_copy(bytes(rows)))
+        theirs = np.zeros_like(img)
+        if 'mask' in config:
+            RefBlend(config).apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
+            RefDrawContours(config).apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
+        else:
+            RefCopy().apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
+            RefDraw().apply(img, theirs, img.shape, theirs_hdr, theirs_hdr)
+        return hashlib.sha256(theirs.tobytes()).hexdigest()
     finally:
-        sys.path.remove(ref_root)
+        sys.path.remove(REF_DIR)
         for k in [k for k in sys.modules if k == 'shapely' or k.startswith('shapely.') or k == 'watsor' or
                   k.startswith('watsor.')]:
             del sys.modules[k]
         sys.modules.update(saved)
+
+
+def test_equal_to_the_reference_classes_installed_under_baseline_ref(engine):
+    """The reference's own effect chain (watsor.output.{blend,draw,copy}, unmodified) on the CPU against the fused GPU
+    effect on the same frame and rows.  With an upstream checkout the chain runs live (its output must also equal the
+    SHA-256 digests stored in tests/golden/reference/gpu_effects.json); without one the stored digests stand in for it
+    (tests/reference_golden.py).  watsor.filter.mask imports shapely (absent): an empty stand-in satisfies the import."""
+    import hashlib
+
+    from tests.reference_golden import upstream
+    from watsor_b200.output.effects import FusedEffects
+
+    w, h = 640, 480
+    rng = np.random.default_rng(21)
+    with TemporaryDirectory() as tmp:
+        alpha = random_alpha(rng, w, h, 4)
+        path = os.path.join(tmp, 'mask.png')
+        assert cv2.imwrite(path, np.dstack([np.zeros((h, w, 3), np.uint8), alpha]))
+        for config in ({'mask': path, 'width': w, 'height': h}, {'width': w, 'height': h}):
+            img = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+            rows = random_rows(rng, w, h, 20, n_zones=4 if 'mask' in config else 0)
+            want = upstream('gpu_effects', 'mask' if 'mask' in config else 'plain',
+                            lambda: reference_chain(config, img, rows))
+            ours = np.zeros_like(img)
+            hdr = header_of(rows)
+            FusedEffects(config, engine).apply(img, ours, img.shape, hdr, hdr)
+            assert hashlib.sha256(ours.tobytes()).hexdigest() == want, 'mask' in config

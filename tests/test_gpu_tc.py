@@ -1,4 +1,4 @@
-"""The tcgen05 GEMM kernel (csrc/kernels_tc.cu) in isolation: one 1x1 convolution per precision mode
+"""The wgmma GEMM kernel (csrc/kernels_tc.cu) in isolation: one 1x1 convolution per precision mode
 against a float64 reference computed from the very activations the GPU produced."""
 import numpy as np
 import pytest
@@ -25,12 +25,12 @@ def tiny_model(K, N, hw, seed=0):
     return m, w1.reshape(K, N), sc, of
 
 
-# (K, N, hw, batch): K = 32 is a half-filled swizzle row in bf16, N = 48 / 96 are non-power-of-two
-# UMMA widths, M = 9 is a mostly out-of-bounds TMA box, 1024x1024 runs the full smem pipeline
+# (K, N, hw, batch): K = 32 is a half-filled swizzle row in bf16, N = 48 / 96 / 16 leave the last N tile ragged,
+# M = 9 is a mostly out-of-bounds TMA box, 1024x1024 runs the full smem pipeline and the cluster split-K
 CASES = [(512, 512, 19, 4), (32, 64, 32, 2), (1024, 1024, 10, 8), (256, 48, 3, 1), (64, 128, 20, 3),
          (128, 96, 7, 2), (16, 16, 5, 1),
-         # >= 148 output tiles: the persistent kernel (double-buffered TMEM, TMA-store epilogue); the last
-         # row tile is partial in each (M = 22500, 28125, 19200+) and 256 columns make two N tiles
+         # more output tiles than SMs; the last row tile is partial in each (M = 22500, 28125, 20172) and
+         # 256 columns make two N tiles
          (32, 64, 150, 1), (64, 128, 75, 5), (128, 256, 41, 12), (24, 128, 150, 2)]
 
 
@@ -52,27 +52,6 @@ def test_pointwise_gemm(precision, rel_tol, K, N, hw, n):
     ref = np.clip(ref * sc.astype(np.float64) + of.astype(np.float64), 0.0, 6.0)
     err = np.abs(y.reshape(-1, N) - ref).max()
     assert err <= rel_tol * max(1.0, np.abs(ref).max()) * (4 if precision == 1 else 1), (err, np.abs(ref).max())
-
-
-@pytest.mark.parametrize('K,N,hw,n', [(512, 512, 19, 4), (1024, 1024, 10, 8), (256, 48, 3, 1), (64, 128, 20, 3)])
-def test_tmem_staged_a_operand(monkeypatch, K, N, hw, n):
-    """The TMEM-staged A operand of k_gemm_tc<2, true> (default; WB_TMEM_A=0 = shared-memory hi / lo tiles): the converter warps tcgen05.st the hi / lo rows into
-    tensor memory and the MMAs take A from there.  Same bar as the shared-memory path; where both use one main
-    accumulator (chains <= 16 steps) the two must agree bit for bit."""
-    m, w1, sc, of = tiny_model(K, N, hw)
-    pre = np.random.default_rng(1).standard_normal((n, hw, hw, 3)).astype(np.float32)
-    out = {}
-    for ta in (False, True):
-        monkeypatch.setenv('WB_TMEM_A', '1' if ta else '0')
-        with Engine(m.to_blob(), device=0, max_batch=n, precision=2) as e:
-            _, _, a = e.backbone(pre, stop_layer=0, layer_shape=(hw, hw, K))
-            _, _, out[ta] = e.backbone(pre, stop_layer=1, layer_shape=(hw, hw, N))
-    ref = a.reshape(-1, K).astype(np.float64) @ w1.astype(np.float64)
-    ref = np.clip(ref * sc.astype(np.float64) + of.astype(np.float64), 0.0, 6.0)
-    err = np.abs(out[True].reshape(-1, N) - ref).max()
-    assert err <= 3e-6 * max(1.0, np.abs(ref).max()), (err, np.abs(ref).max())
-    if K <= 128:      # chains of <= 16 MMAs: one main accumulator on both paths
-        assert np.array_equal(out[True], out[False])
 
 
 def test_fused_depthwise_pointwise_equals_unfused(shapes_model):

@@ -199,34 +199,3 @@ def test_configs2_single_frame_equals_batch_rows(v2coco):
         a, b = rows_to_tuples(batch[3]), rows_to_tuples(single[0])
         same = sum(1 for x, y in zip(a, b) if x[0] == y[0] and x[2:] == y[2:])
         assert same >= 90 and max(abs(x[1] - y[1]) for x, y in zip(a, b)) < 1e-3
-
-
-def test_irb_block_kernel(v2coco, monkeypatch):
-    """WB_IRB=1: the inverted residual blocks 1..5 (expand -> depthwise -> projection [-> Add]) as ONE kernel
-    (k_irb_x3: expand on CUDA cores, depthwise producers, tcgen05 projection).  Same bar as the separate kernels:
-    heads against the float64 evaluation, rows against the oracle."""
-    from oracle.ssd_graph import to_detections
-    from oracle.ties import analyse, compare_with_ties
-    m, o32, o64, frames = v2coco
-    monkeypatch.setenv('WB_IRB', '1')
-    stats = {'strict_frames': 0, 'tie_frames': 0}
-    with B200ObjectDetector(None, device=0, max_batch=8, precision=2, model_blob=m.to_blob()) as det:
-        fused_launches = None
-        for c in range(8):
-            det.configure_camera(c, 640, 480, None)
-        rows = new_rows(8)
-        det.detect_batch([f['img'] for f in frames], list(range(8)), rows, fuse_filters=False)
-        fused_launches = det.engine.last_launch_count()
-        for i, fr in enumerate(frames):
-            _check_frame(rows_to_tuples(rows[i]), fr['img'], o32, o64, stats, to_detections, analyse, compare_with_ties,
-                         cached=fr)
-        genc, glg, _ = det.engine.backbone(frames[0]['pre'][None])
-        e64, l64 = frames[0]['heads64']
-        assert np.abs(genc[0] - e64).max() <= 5e-4 and np.abs(glg[0] - l64).max() <= 5e-4
-    monkeypatch.delenv('WB_IRB')
-    with B200ObjectDetector(None, device=0, max_batch=8, precision=2, model_blob=m.to_blob()) as det:
-        for c in range(8):
-            det.configure_camera(c, 640, 480, None)
-        det.detect_batch([f['img'] for f in frames], list(range(8)), new_rows(8), fuse_filters=False)
-        assert det.engine.last_launch_count() > fused_launches          # the block kernel really replaced launches
-    assert stats['strict_frames'] + stats['tie_frames'] == 8

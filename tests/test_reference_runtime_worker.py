@@ -7,11 +7,11 @@ import sys
 
 import pytest
 
-from tests.conftest import ROOT
+from tests.conftest import REF_DIR, REF_SITE, ROOT
 
 
 def reference_path():
-    for p in ('/root/reference', os.path.join(ROOT, 'baseline', '_ref')):
+    for p in (REF_DIR, REF_SITE):
         if os.path.isfile(os.path.join(p, 'watsor', 'stream', 'work.py')):
             return p
     return None

@@ -2,9 +2,11 @@
 TrackFilter (watsor/filter/track.py:29-149) and the sieve write-back (watsor/filter/sieve.py:21-52).
 
 Pinned by (a) the reference's known answers (watsor/test/test_filter.py:76-96), (b) the reference's TrackFilter
-itself, imported from /root/reference when present, (c) the oracle restatement, (d) the CPython interpreter for
+itself, imported from an upstream checkout when present, (c) the oracle restatement, (d) the CPython interpreter for
 the set iteration orders the reference leaks into its results.  No GPU involved."""
 import ctypes
+import hashlib
+import json
 import os
 import random
 import sys
@@ -16,7 +18,8 @@ from oracle.filters import Det, TrackOracle
 from watsor_b200 import _lib
 from watsor_b200.stream.share import MAX_DETECTIONS, BoundingBox, Detection
 
-REF = '/root/reference'
+from tests.conftest import REF_DIR as REF  # noqa: E402
+from tests.reference_golden import upstream  # noqa: E402
 
 
 class NativeTracker:
@@ -146,32 +149,43 @@ def test_native_tracker_equals_oracle(seed, sens, hist, per_label, labels, zone_
         assert [key(d) for d in got] == [d.key() for d in exp], f
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason='reference tree not present')
+def frame_digest(sa, keys):
+    return hashlib.sha256(json.dumps([sa, keys]).encode()).hexdigest()[:16]
+
+
 @pytest.mark.parametrize('seed,sens,hist,per_label,labels,zone_ids',
                          [(11, 1, 2, 3, 2, 3), (12, 5, 10, 10, 3, 12), (13, 2, 4, 14, 1, 9), (14, 3, 6, 7, 5, 5)])
 def test_native_tracker_equals_reference_trackfilter(seed, sens, hist, per_label, labels, zone_ids):
-    """The reference's own TrackFilter (watsor/filter/track.py), imported from the read-only tree."""
-    sys.path.insert(0, REF)
-    try:
-        from watsor.filter.track import TrackFilter as RefTrackFilter
-        from watsor.stream.share import BoundingBox as RefBox
-        from watsor.stream.share import Detection as RefDetection
-    finally:
-        sys.path.remove(REF)
+    """The reference's own TrackFilter (watsor/filter/track.py), from an upstream checkout or, without one, as the
+    per-frame digests of its output stored in tests/golden/reference/tracker.json."""
     rng = random.Random(seed)
     frames = random_frames(rng, 150, per_label, labels, zone_ids)
-    nat, ref = NativeTracker(sens, hist), RefTrackFilter(sensitivity=sens, history=hist)
+
+    def theirs():
+        sys.path.insert(0, REF)
+        try:
+            from watsor.filter.track import TrackFilter as RefTrackFilter
+            from watsor.stream.share import BoundingBox as RefBox
+            from watsor.stream.share import Detection as RefDetection
+        finally:
+            sys.path.remove(REF)
+        ref, out = RefTrackFilter(sensitivity=sens, history=hist), []
+        for dets in frames:
+            rdets = []
+            for l, c, b, z in dets:
+                d = RefDetection(label=l, confidence=c, bounding_box=RefBox(*b))
+                for i, zz in enumerate(z):
+                    d.zones[i] = zz
+                rdets.append(d)
+            exp, sa_r = ref(rdets)
+            out.append(frame_digest(sa_r, [key(d) for d in exp]))
+        return out
+    want = upstream('tracker', 'seed %d' % seed, theirs)
+    nat = NativeTracker(sens, hist)
+    assert len(want) == len(frames)
     for f, dets in enumerate(frames):
         got, sa = nat([mk(*d) for d in dets])
-        rdets = []
-        for l, c, b, z in dets:
-            d = RefDetection(label=l, confidence=c, bounding_box=RefBox(*b))
-            for i, zz in enumerate(z):
-                d.zones[i] = zz
-            rdets.append(d)
-        exp, sa_r = ref(rdets)
-        assert sa == sa_r, f
-        assert [key(d) for d in got] == [key(d) for d in exp], f
+        assert frame_digest(sa, [key(d) for d in got]) == want[f], f
 
 
 def test_sieve_rows_writes_back_and_zero_fills():

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""Generates tests/golden/* -- run HERE (needs /root/reference), outputs are committed.
+"""Generates tests/golden/* from an upstream watsor checkout (oracle/reference_build.py); outputs are committed.
 
 Inputs follow the reference's own frame generator
 (`watsor.test.detect_stream.Artist.draw_random_shapes`, detect_stream.py:42-70; restated in
 tests/artist.py because the original passes floats to random.randrange, which Python 3.12
 rejects) with `random.seed(1000*cam + frame)` (SURVEY.md 8d); expected outputs by the GraphDef-driven
 oracle (oracle/ssd_graph.py) on the reference's vendored model
-(/root/reference/watsor/test/model/cpu.pb).  NOT TensorFlow outputs: TensorFlow is not
+(watsor/test/model/cpu.pb).  NOT TensorFlow outputs: TensorFlow is not
 installed, see oracle/__init__.py ("parity unpinned" at the TF boundary).
 """
 import hashlib
@@ -20,7 +20,9 @@ from PIL import Image, ImageDraw
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = '/root/reference'
+from oracle.reference_build import reference_dir  # noqa: E402
+
+REF = reference_dir()
 sys.path.insert(0, REF)
 
 from tests.artist import draw_random_shapes  # noqa: E402  (restated recipe, see tests/artist.py)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Pin the oracle's conv arithmetic with an INDEPENDENT executor of the reference's own graph.
 
-    python tools/make_golden_cvdnn.py            (needs /root/reference; writes tests/golden/cvdnn_heads.npz)
+    python tools/make_golden_cvdnn.py            (needs an upstream checkout; writes tests/golden/cvdnn_heads.npz)
 
 TensorFlow -- the sole owner of the conv arithmetic in the reference (watsor/detection/tensorflow_cpu.py:104-121)
 -- cannot be installed here, and the reference's only model test asserts a detection count, not tensors
@@ -17,7 +17,7 @@ CPU kernels for TensorFlow GraphDefs.  This script
      Reshape + `concat` / `concat_1` nodes do) as golden vectors, labelled "OpenCV-dnn, not TensorFlow".
 
 tests/test_oracle_cvdnn.py asserts `oracle.raw_heads(pre)` equals these vectors to 1e-4 (CPU suite, reads only
-the committed .npz), and -- where /root/reference is present -- re-runs OpenCV live.  What this pins: 99 % of the
+the committed .npz), and -- where an upstream checkout is present -- re-runs OpenCV live.  What this pins: 99 % of the
 arithmetic (every convolution, batch norm, activation and bias of the backbone and heads; SAME padding, strides,
 layout).  What it does NOT pin: the legacy ResizeBilinear, the anchor generator, box decoding, sigmoid,
 NonMaxSuppressionV5 and the top-100 assembly -- those remain restated from the graph/TF kernel semantics
@@ -30,7 +30,9 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF_PB = '/root/reference/watsor/test/model/cpu.pb'
+from oracle.reference_build import reference_pb  # noqa: E402
+
+REF_PB = reference_pb()
 OUT = os.path.join(ROOT, 'tests', 'golden', 'cvdnn_heads.npz')
 CUT_INPUT = 'Preprocessor/sub'
 FRAMES = [(100, 100, 1, 0), (320, 240, 2, 1), (640, 480, 3, 2)]     # (w, h, cam, frame) of tests/artist.py

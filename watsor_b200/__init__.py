@@ -1,4 +1,4 @@
-"""watsor_b200 -- B200-native (sm_100a) implementation of watsor's per-frame detection
+"""watsor_b200 -- H100-native (sm_90a) implementation of watsor's per-frame detection
 hot path behind the reference's plugin surface:
 
     watsor_b200.detection   <-> watsor/detection/*   (Detector protocol, create_object_detectors)

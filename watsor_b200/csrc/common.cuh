@@ -1,4 +1,4 @@
-// common.cuh -- shared device-side types of libwatsor_b200 (sm_100a only).
+// common.cuh -- shared device-side types of libwatsor_b200 (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

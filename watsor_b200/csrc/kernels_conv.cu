@@ -4,7 +4,7 @@
 // `BoxPredictor_i/{BoxEncodingPredictor,ClassPredictor}` (Conv2D + BiasAdd, Reshape, concat) of the
 // frozen graph run by watsor/detection/tensorflow_cpu.py:114.  All tensors are NHWC, TF `SAME`
 // padding (asymmetric).  The 1x1 / KxK dense convolutions are one tiled SGEMM with an optional
-// im2col row gather; the bf16 tcgen05 path lives in kernels_tc.cu.
+// im2col row gather; the bf16 wgmma path lives in kernels_tc.cu.
 #include <algorithm>
 
 #include "common.cuh"
@@ -459,9 +459,15 @@ void launch_gemm_cc(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, 
   g.ncp1 = num_classes_p1;
   g.splits = 1;
   g.partial = partial;
-  // big tiles when they still fill the 148 SMs, small tiles otherwise
+  // big tiles when they still fill every SM, small tiles otherwise
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  }
   long big = (long)((g.M + 127) / 128) * ((g.N + 127) / 128);
-  if (big >= 148 && g.N >= 128) {
+  if (big >= sms && g.N >= 128) {
     dim3 grid((g.N + 127) / 128, (g.M + 127) / 128);
     k_gemm_cc<T, 128, 128, 8, 8><<<grid, 256, 0, lc.stream>>>(g);
     ++*lc.launch_counter;

@@ -4,18 +4,18 @@
 // Restates the layer pairs `Conv2d_i_depthwise` -> `Conv2d_i_pointwise` of the frozen graph
 // (watsor/detection/tensorflow_cpu.py:114 runs them inside sess.run).  fp32-faithful mode only (TF32X3).
 //
-// Persistent kernel, one CTA per SM, output tile = 8 x 16 pixels of one image x all N (<= 128) channels:
-//   warp 4      TMA producer: per 32-channel k-block a 4-D box {32 ch, halo_w, halo_h, 1 image} of the
+// Persistent kernel, one CTA per SM, output tile = 8 x 16 pixels of one image x all N (<= 64) channels:
+//   warp 16     TMA producer: per 32-channel k-block a 4-D box {32 ch, halo_w, halo_h, 1 image} of the
 //               depthwise INPUT (halo included; out-of-image coordinates are zero-filled by TMA = TF SAME
 //               padding) and the 1x1 weight tiles (hi, lo)
 //   warps 8..15 depthwise producers: thread = 4 adjacent pixels x 4 channels; a 3 x 6 window of the halo tile is
 //               read once from shared memory (8 lanes = the 8 channel quads of one pixel -> conflict-free
 //               128-byte rows, the 9 tap weights live in registers), BN + ReLU6, TF32 hi/lo split, written
-//               straight into the 128B-swizzled UMMA A tiles
-//   warp 5      tcgen05.mma issuer (3 TF32 MMAs per product), TMEM accumulator sets double-buffered
-//   warps 0..3  epilogue: tcgen05.ld -> BN + ReLU6 -> swizzled staging -> 4-D TMA store {32 ch, 16, 2, 1}
-// The depthwise accumulation order (ky, kx) and the GEMM's k order are those of the unfused kernels, so
-// the result is bit-identical to running k_dw_strip followed by k_gemm_tc_persist.
+//               straight into the 128B-swizzled wgmma A tiles
+//   warps 0..7  two consumer warpgroups (tile rows 0..63 / 64..127): wgmma (3 TF32 MMAs per product, accumulators in
+//               registers, k-block partial sums added with round-to-nearest), then BN + ReLU6 and the stores of their rows
+// The depthwise accumulation order (ky, kx) and the GEMM's MMA sequence (wg_mma_kblock) are those of the unfused
+// kernels, so the result is bit-identical to running k_dw_strip followed by k_gemm_tc.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -26,7 +26,6 @@
 namespace {
 
 constexpr int F_TH = 8, F_TW = 16;  // output tile (pixels) = 128 GEMM rows
-constexpr int F_STAGING_BYTES = 4 * 2 * 4096;
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
                                             int c3) {
@@ -36,11 +35,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map),
-               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
 
 struct FusedArgs {
   const float* dw_w;  // [9][C]
@@ -48,56 +42,48 @@ struct FusedArgs {
   const float* dw_offset;
   const float* scale;  // 1x1 layer, [n_pad]
   const float* offset;
+  float* out;  // [n_img][OH][OW][N]
   int dw_act, act;
   int C, S, pad_t, pad_l;
   int OH, OW, n_img;
-  int N, n_pad, block_n, k_blocks, n_main;
+  int N, n_pad, block_n, k_blocks;
   int tiles_x, tiles_y;
   int stages, halo_stages;
   int th_in, tw_in;
 };
 
-// Warp roles, by warpgroup (the epilogue warps must be warps 0..3 of a warpgroup: TMEM lane quarter = warp % 4):
-//   warps 0..3   epilogue
-//   warp  4      TMA producer, warp 5 MMA issuer, 6..7 idle (they wait at the final barrier)
-//   warps 8..15  depthwise producers (4 pixels x 1 channel quad per thread and k-block)
-// 16 producer warps with `setmaxnreg` 64/152 were measured too: slower (profiles/r01_pipeline_trace.md: the
-// long pole per tile is the epilogue / the MMAs, not the depthwise arithmetic).
+constexpr int F_CONSUMER_WARPS = 8;
 constexpr int F_PRODUCER_WARPS = 8;
-constexpr int F_FIRST_PRODUCER_THREAD = 256;
-constexpr int F_THREADS = F_FIRST_PRODUCER_THREAD + 32 * F_PRODUCER_WARPS;  // 512
+constexpr int F_FIRST_PRODUCER_THREAD = 32 * F_CONSUMER_WARPS;                   // 256
+constexpr int F_TMA_WARP = F_CONSUMER_WARPS + F_PRODUCER_WARPS;                  // 16
+constexpr int F_THREADS = F_FIRST_PRODUCER_THREAD + 32 * F_PRODUCER_WARPS + 32;  // 544
 
-template <int S>
+// barrier among the 128 threads of consumer warpgroup `wg` (hardware barriers 2 and 3)
+__device__ __forceinline__ void f_wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
+
+template <int S, int BN>
 __global__ void __launch_bounds__(F_THREADS, 1)
     k_dwpw_tc_x3(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_b,
-                 const __grid_constant__ CUtensorMap map_b_lo, const __grid_constant__ CUtensorMap map_out, FusedArgs g) {
+                 const __grid_constant__ CUtensorMap map_b_lo, FusedArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int halo_bytes = ((g.th_in * g.tw_in * ROW_BYTES + 1023) / 1024) * 1024;
-  const int b_tile_bytes = g.block_n * ROW_BYTES;
-  const int ab_bytes = 2 * A_TILE_BYTES + 2 * b_tile_bytes;
+  constexpr int B_TILE_BYTES = BN * ROW_BYTES;
+  constexpr int AB_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
   uint8_t* halo0 = smem;
   uint8_t* ab0 = halo0 + (size_t)g.halo_stages * halo_bytes;
-  uint8_t* staging = ab0 + (size_t)g.stages * ab_bytes;
-  uint64_t* halo_full = reinterpret_cast<uint64_t*>(staging + F_STAGING_BYTES);
+  uint64_t* halo_full = reinterpret_cast<uint64_t*>(ab0 + (size_t)g.stages * AB_BYTES);
   uint64_t* halo_empty = halo_full + g.halo_stages;
   uint64_t* b_full = halo_empty + g.halo_stages;
   uint64_t* a_ready = b_full + g.stages;
   uint64_t* empty = a_ready + g.stages;
-  uint64_t* acc_full = empty + g.stages;  // [2]
-  uint64_t* acc_empty = acc_full + 2;     // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_dw = reinterpret_cast<float*>(reinterpret_cast<uintptr_t>(tmem_slot + 4) + 15 & ~(uintptr_t)15);  // [11][C]
+  float* s_dw = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(empty + g.stages) + 15) & ~(uintptr_t)15);  // [11][C]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_img = g.tiles_x * g.tiles_y;
   const int num_tiles = tiles_per_img * g.n_img;
-  const int n_acc = g.n_main + 1;
-  const int set_cols = n_acc * g.block_n;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < 2 * set_cols) tmem_cols <<= 1;
 
-  if (warp == 4 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int h = 0; h < g.halo_stages; ++h) {
       mbar_init(smem_u32(&halo_full[h]), 1);
       mbar_init(smem_u32(&halo_empty[h]), F_PRODUCER_WARPS);  // one arrive per depthwise producer warp
@@ -105,33 +91,24 @@ __global__ void __launch_bounds__(F_THREADS, 1)
     for (int s = 0; s < g.stages; ++s) {
       mbar_init(smem_u32(&b_full[s]), 1);
       mbar_init(smem_u32(&a_ready[s]), F_PRODUCER_WARPS);
-      mbar_init(smem_u32(&empty[s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&acc_full[b]), 1);
-      mbar_init(smem_u32(&acc_empty[b]), 4);
+      mbar_init(smem_u32(&empty[s]), 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(smem_u32(tmem_slot), tmem_cols);
   // depthwise taps + folded BN of every channel: loaded once per CTA, read by the producers every k-block
   for (int i = threadIdx.x; i < 9 * g.C; i += blockDim.x) s_dw[i] = g.dw_w[i];
   for (int i = threadIdx.x; i < g.C; i += blockDim.x) {
     s_dw[9 * g.C + i] = g.dw_scale[i];
     s_dw[10 * g.C + i] = g.dw_offset[i];
   }
-  float* s_pw = s_dw + 11 * g.C;  // [2][block_n]: folded BN of the pointwise output channels
-  for (int i = threadIdx.x; i < g.block_n; i += blockDim.x) {  // block_n may exceed n_pad (N = 16 / 24: one 32-wide tile)
+  float* s_pw = s_dw + 11 * g.C;  // [2][BN]: folded BN of the pointwise output channels
+  for (int i = threadIdx.x; i < BN; i += blockDim.x) {  // BN may exceed n_pad (N = 16 / 24: one 32-wide tile)
     s_pw[i] = i < g.n_pad ? g.scale[i] : 1.f;
-    s_pw[g.block_n + i] = i < g.n_pad ? g.offset[i] : 0.f;
+    s_pw[BN + i] = i < g.n_pad ? g.offset[i] : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (threadIdx.x == 0) WB_STAMP(9, 0);
 
-  if (warp == 4) {
+  if (warp == F_TMA_WARP) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one()) {
       int it = 0;
@@ -141,118 +118,65 @@ __global__ void __launch_bounds__(F_THREADS, 1)
         for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
           const int h = it % g.halo_stages, s = it % g.stages;
           mbar_wait(smem_u32(&halo_empty[h]), ((it / g.halo_stages) & 1) ^ 1);
-          WB_STAMP(0, it);
           const uint32_t hb = smem_u32(&halo_full[h]);
           mbar_expect_tx(hb, (uint32_t)(g.th_in * g.tw_in * ROW_BYTES));
           tma_load_4d(smem_u32(halo0 + (size_t)h * halo_bytes), &map_in, hb, kb * 32, ox0 * S - g.pad_l,
                       oy0 * S - g.pad_t, img);
           mbar_wait(smem_u32(&empty[s]), ((it / g.stages) & 1) ^ 1);
-          WB_STAMP(1, it);
           const uint32_t bb = smem_u32(&b_full[s]);
-          uint8_t* sb = ab0 + (size_t)s * ab_bytes + 2 * A_TILE_BYTES;
-          mbar_expect_tx(bb, 2 * b_tile_bytes);
+          uint8_t* sb = ab0 + (size_t)s * AB_BYTES + 2 * A_TILE_BYTES;
+          mbar_expect_tx(bb, 2 * B_TILE_BYTES);
           tma_load_2d(smem_u32(sb), &map_b, bb, kb * 32, 0);
-          tma_load_2d(smem_u32(sb + b_tile_bytes), &map_b_lo, bb, kb * 32, 0);
+          tma_load_2d(smem_u32(sb + B_TILE_BYTES), &map_b_lo, bb, kb * 32, 0);
         }
       }
     }
-  } else if (warp == 5) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = make_idesc(true, BLOCK_M, g.block_n);
-    int it = 0, j = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-      const int buf = j & 1;
-      mbar_wait(smem_u32(&acc_empty[buf]), ((j >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t acc0 = tmem_base + (uint32_t)(buf * set_cols);
+  } else if (warp < F_CONSUMER_WARPS) {
+    // ------------------------------------------------------------------ consumer warpgroups
+    const int wg = warp >> 2;
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // tile row of accumulators 0, 1 (+8: 2, 3)
+    const int col = 2 * (lane & 3);
+    int it = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      const int img = t / tiles_per_img, r = t - img * tiles_per_img;
+      const int oy0 = (r / g.tiles_x) * F_TH, ox0 = (r % g.tiles_x) * F_TW;
+      float acc[BN / 2], part[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
         const int s = it % g.stages;
         const uint32_t ph = (it / g.stages) & 1;
         mbar_wait(smem_u32(&a_ready[s]), ph);
         mbar_wait(smem_u32(&b_full[s]), ph);
-        tc_fence_after();
-        if (elect_one()) {
-          WB_STAMP(5, it);
-          uint8_t* st = ab0 + (size_t)s * ab_bytes;
-          const uint32_t a_hi = smem_u32(st), a_lo = a_hi + A_TILE_BYTES;
-          const uint32_t b_hi = a_lo + A_TILE_BYTES, b_lo = b_hi + b_tile_bytes;
+        const uint32_t a_hi = smem_u32(ab0 + (size_t)s * AB_BYTES) + (uint32_t)(wg * 64 * ROW_BYTES);
+        const uint32_t a_lo = a_hi + A_TILE_BYTES;
+        const uint32_t b_hi = smem_u32(ab0 + (size_t)s * AB_BYTES) + 2 * A_TILE_BYTES, b_lo = b_hi + B_TILE_BYTES;
+        wg_x3_kblock_sum<BN>(acc, part, a_hi, a_lo, b_hi, b_lo);
+        f_wg_bar_sync(wg);  // every warp of the warpgroup has seen its MMAs complete: the stage may be refilled
+        if ((threadIdx.x & 127) == 0) mbar_arrive(smem_u32(&empty[s]));
+      }
+      // folded BN + ReLU6 of this thread's two rows, 8-byte stores (a lane quad covers 32 contiguous bytes)
 #pragma unroll
-          for (int k = 0; k < ROW_BYTES / UMMA_K_BYTES; ++k) {
-            const uint32_t koff = k * UMMA_K_BYTES;
-            const int step = kb * (ROW_BYTES / UMMA_K_BYTES) + k;
-            const uint32_t d_main = acc0 + (uint32_t)((step % g.n_main) * g.block_n);
-            const uint32_t d_corr = acc0 + (uint32_t)(g.n_main * g.block_n);
-            umma<true>(d_main, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), idesc, step >= g.n_main);
-            umma<true>(d_corr, make_sw128_desc(a_lo + koff), make_sw128_desc(b_hi + koff), idesc, step != 0);
-            umma<true>(d_corr, make_sw128_desc(a_hi + koff), make_sw128_desc(b_lo + koff), idesc, 1u);
+      for (int h = 0; h < 2; ++h) {
+        const int rr = row + 8 * h;
+        const int oy = oy0 + rr / F_TW, ox = ox0 + rr % F_TW;
+        if (oy >= g.OH || ox >= g.OW) continue;
+        float* op = g.out + (((size_t)img * g.OH + oy) * g.OW + ox) * g.N;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + col;
+          if (c >= g.N) break;
+          float y0 = affine_rn(acc[4 * j + 2 * h], s_pw[c], s_pw[BN + c]);
+          float y1 = affine_rn(acc[4 * j + 2 * h + 1], s_pw[c + 1], s_pw[BN + c + 1]);
+          if (g.act == WB_ACT_RELU6) {
+            y0 = relu6f(y0);
+            y1 = relu6f(y1);
           }
-          umma_commit(smem_u32(&empty[s]));
-          if (kb == g.k_blocks - 1) umma_commit(smem_u32(&acc_full[buf]));
-          WB_STAMP(6, it);
+          *reinterpret_cast<float2*>(op + c) = make_float2(y0, y1);
         }
-        __syncwarp();
       }
     }
-  } else if (warp < 4) {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;
-    uint8_t* my_stage = staging + (size_t)q * 2 * 4096;
-    const int used = min(g.n_main, g.k_blocks * (ROW_BYTES / UMMA_K_BYTES));
-    int j = 0, chunk_no = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-      const int buf = j & 1;
-      const int img = t / tiles_per_img, r = t - img * tiles_per_img;
-      const int oy0 = (r / g.tiles_x) * F_TH, ox0 = (r % g.tiles_x) * F_TW;
-      mbar_wait(smem_u32(&acc_full[buf]), (j >> 1) & 1);
-      tc_fence_after();
-      if (threadIdx.x == 0) WB_STAMP(7, j);
-      const uint32_t acc0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * set_cols);
-      for (int c0 = 0; c0 < g.block_n; c0 += 32, ++chunk_no) {
-        float y[32];
-        {
-          uint32_t v[32];
-          load_acc32<true>(acc0 + (uint32_t)c0, g.block_n, g.n_main, used, v);
-#pragma unroll
-          for (int i4 = 0; i4 < 8; ++i4) {
-            const int nn = c0 + i4 * 4;
-            const float4 sc = lds128(smem_u32(s_pw + nn)), of = lds128(smem_u32(s_pw + g.block_n + nn));
-            const float scs[4] = {sc.x, sc.y, sc.z, sc.w}, ofs[4] = {of.x, of.y, of.z, of.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float x = affine_rn(__uint_as_float(v[i4 * 4 + e]), scs[e], ofs[e]);
-              y[i4 * 4 + e] = g.act == WB_ACT_RELU6 ? relu6f(x) : x;
-            }
-          }
-        }
-        if (chunk_no >= 2) {
-          if (lane == 0) bulk_wait_read<1>();
-          __syncwarp();
-        }
-        const uint32_t sb = smem_u32(my_stage + (size_t)(chunk_no & 1) * 4096 + (size_t)lane * 128);
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          uint4 pk;
-          pk.x = __float_as_uint(y[c * 4 + 0]);
-          pk.y = __float_as_uint(y[c * 4 + 1]);
-          pk.z = __float_as_uint(y[c * 4 + 2]);
-          pk.w = __float_as_uint(y[c * 4 + 3]);
-          sts128(sb + (uint32_t)((c ^ (lane & 7)) << 4), pk);
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (elect_one()) {
-          // rows q*32 .. q*32+31 of the tile = spatial rows 2q, 2q+1 (16 pixels each)
-          tma_store_4d(&map_out, smem_u32(my_stage + (size_t)(chunk_no & 1) * 4096), c0, ox0, oy0 + 2 * q, img);
-          bulk_commit();
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (threadIdx.x == 0) WB_STAMP(8, j);
-      if (lane == 0) mbar_arrive(smem_u32(&acc_empty[buf]));
-    }
-    if (lane == 0) bulk_wait_read<0>();
-  } else if (warp >= 8) {
+  } else {
     // ------------------------------------------------------------------ depthwise producers
     const int pt = threadIdx.x - F_FIRST_PRODUCER_THREAD;
     const int q = pt & 7, slot = pt >> 3;  // channel quad of the k-block, pixel slot
@@ -267,11 +191,9 @@ __global__ void __launch_bounds__(F_THREADS, 1)
         const float4 sc = lds128(smem_u32(s_dw + 9 * g.C + cch));
         const float4 of = lds128(smem_u32(s_dw + 10 * g.C + cch));
         mbar_wait(smem_u32(&halo_full[h]), (it / g.halo_stages) & 1);
-        if (pt == 0) WB_STAMP(2, it);
         mbar_wait(smem_u32(&empty[s]), ((it / g.stages) & 1) ^ 1);  // A tiles of this stage are free again
-        if (pt == 0) WB_STAMP(3, it);
         const uint32_t hal = smem_u32(halo0 + (size_t)h * halo_bytes);
-        const uint32_t a_hi = smem_u32(ab0 + (size_t)s * ab_bytes);
+        const uint32_t a_hi = smem_u32(ab0 + (size_t)s * AB_BYTES);
         const uint32_t a_lo = a_hi + A_TILE_BYTES;
         // One thread = 4 horizontally adjacent output pixels of one channel quad: a 3 x 6 input window is read
         // once (18 LDS.128 instead of 36) and every input feeds up to three outputs.  Per output the taps
@@ -321,7 +243,6 @@ __global__ void __launch_bounds__(F_THREADS, 1)
         }
         fence_proxy_async();
         __syncwarp();
-        if (pt == 0) WB_STAMP(4, it);
         if (lane == 0) {
           mbar_arrive(smem_u32(&a_ready[s]));
           mbar_arrive(smem_u32(&halo_empty[h]));
@@ -329,37 +250,29 @@ __global__ void __launch_bounds__(F_THREADS, 1)
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
 }
 
 struct FusedPlan {
-  int block_n, n_main, stages, halo_stages, th_in, tw_in, tiles_x, tiles_y;
+  int block_n, stages, halo_stages, th_in, tw_in, tiles_x, tiles_y;
   size_t smem;
 };
 
 bool make_plan(const wb_layer& dw, const wb_layer& pw, FusedPlan* p) {
-  p->block_n = ((int)pw.n_pad + 31) / 32 * 32;  // weight rows / output columns beyond N: zero-filled / clipped by TMA
-  p->n_main = 1;
+  p->block_n = pw.n_pad <= 32 ? 32 : 64;  // the GEMM's N tile (weight rows beyond N: zero-filled)
   p->th_in = (F_TH - 1) * dw.stride + 3;
   p->tw_in = (F_TW - 1) * dw.stride + 3;
   p->tiles_x = (dw.out_w + F_TW - 1) / F_TW;
   p->tiles_y = (dw.out_h + F_TH - 1) / F_TH;
   const size_t halo = ((size_t)p->th_in * p->tw_in * ROW_BYTES + 1023) / 1024 * 1024;
   const size_t ab = 2 * A_TILE_BYTES + 2 * (size_t)p->block_n * ROW_BYTES;
-  const size_t budget = 224 * 1024 - F_STAGING_BYTES - 44 * (size_t)dw.out_c;
+  const size_t budget = 224 * 1024 - 44 * (size_t)dw.out_c;
   // prefer two A/B stages, then as many halo buffers as fit (at least two)
   for (int st = 2; st >= 1; --st)
     for (int hs = 3; hs >= 2; --hs) {
       if (hs * halo + st * ab <= budget) {
         p->stages = st;
         p->halo_stages = hs;
-        p->smem = hs * halo + st * ab + F_STAGING_BYTES + 1024 + 8 * (2 * hs + 3 * st + 4) + 64 + 44 * (size_t)dw.out_c + 8 * (size_t)pw.out_c;
+        p->smem = hs * halo + st * ab + 1024 + 8 * (2 * hs + 3 * st) + 16 + 44 * (size_t)dw.out_c + 8 * (size_t)p->block_n;
         return true;
       }
     }
@@ -367,542 +280,15 @@ bool make_plan(const wb_layer& dw, const wb_layer& pw, FusedPlan* p) {
 }
 
 
-// ===================================================================================================
-// MobileNet-v2 inverted residual block as ONE kernel (`expanded_conv_k/{expand,depthwise,project}` [+ `add`] of the
-// TF-slim graph a SSD-MobileNet-v2 frozen_inference_graph.pb holds; ref: watsor/detection/tensorflow_cpu.py:114 runs
-// them inside sess.run):
-//     1x1 expand (C_in <= 32 -> C, BN, ReLU6)  ->  depthwise 3x3 stride 1 (BN, ReLU6)  ->  1x1 linear projection
-//     (C -> N <= 128, BN)  [-> + shortcut]
-// The 6x expanded tensor and the depthwise output never leave the SM; both 1x1 convolutions run on tcgen05.
-//
-// Persistent kernel, output tile = 8 x 16 pixels (one 128-row UMMA tile of the projection).  Per tile:
-//   warp 4        TMA: the INPUT halo tile (10 x 18 pixels x 32 channels, out-of-image pixels and channels >= C_in
-//                 zero-filled) lands 128B-swizzled = it IS the K-major A operand of the expand GEMM (180 rows, two
-//                 UMMA M tiles); per 32-channel block kb of the expanded tensor: the expand weight tiles (hi, lo)
-//                 and the projection weight tiles (hi, lo)
-//   warps 14..17  (a) once per tile: the TF32 `lo` copy of the input tile; (b) per kb, "mid-epilogue": expand
-//                 accumulators TMEM -> registers -> BN + ReLU6, zero outside the image (= the depthwise conv's SAME
-//                 padding) -> depthwise halo chunk [pixels][32 ch] in shared memory (XOR-swizzled 16-byte chunks)
-//   warps 6..13   depthwise producers: 3x3 window from the halo chunk, BN + ReLU6, TF32 hi/lo split, written straight
-//                 into the 128B-swizzled UMMA A tiles of the projection (same arithmetic as k_dwpw_tc_x3)
-//   warp 5        tcgen05.mma issuer for BOTH GEMMs (3 TF32 MMAs per product): expand(kb + 1) is issued before
-//                 projection(kb), so the tensor core works on the next chunk while the depthwise warps are busy
-//   warps 0..3    epilogue: tcgen05.ld -> BN (+ shortcut read from the block input) -> swizzled staging -> TMA store
-// Stride-2 blocks are not fused: their 17 x 33 input halo needs 5 M tiles (hi + lo = 160 KB) beside a 72 KB halo chunk.
-struct IrbArgs {
-  const float* e_scale;  // expand layer: folded BN [C]
-  const float* e_offset;
-  const float* dw_w;  // [9][C]
-  const float* dw_scale;
-  const float* dw_offset;
-  const float* scale;  // projection, [n_pad]
-  const float* offset;
-  const float* residual;  // block input [n][IH][IW][C_in] when the bottleneck Add is fused (C_in == N), else NULL
-  int e_act, dw_act, act;
-  int Cin, C, Cr;  // Cr = C rounded up to 32
-  int IH, IW, pad_t, pad_l, OH, OW, n_img;
-  int N, n_pad, block_n, k_blocks, n_main;
-  int tiles_x, tiles_y, stages, halo_stages, th_in, tw_in, m_tiles, e_ksteps;
-};
-
-constexpr int IRB_XE_WARPS = 4;
-constexpr int IRB_FIRST_DW_THREAD = 192;                                          // warps 6..13
-constexpr int IRB_FIRST_XE_THREAD = IRB_FIRST_DW_THREAD + 32 * F_PRODUCER_WARPS;  // warps 14..17
-constexpr int IRB_THREADS = IRB_FIRST_XE_THREAD + 32 * IRB_XE_WARPS;              // 576
-constexpr int IRB_WE_STAGES = 2;
-constexpr int IRB_WE_BYTES = 2 * 32 * ROW_BYTES;  // expand weight tiles of one chunk: 32 channels x 32 k, hi + lo
-
-template <int S>
-__global__ void __launch_bounds__(IRB_THREADS, 1)
-    k_irb_x3(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_we,
-             const __grid_constant__ CUtensorMap map_we_lo, const __grid_constant__ CUtensorMap map_b,
-             const __grid_constant__ CUtensorMap map_b_lo, const __grid_constant__ CUtensorMap map_out, IrbArgs g) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int P = g.th_in * g.tw_in;  // halo pixels = rows of the expand GEMM
-  const int ain_bytes = g.m_tiles * A_TILE_BYTES;
-  const int halo_bytes = ((P * ROW_BYTES + 1023) / 1024) * 1024;
-  const int b_tile_bytes = g.block_n * ROW_BYTES;
-  const int ab_bytes = 2 * A_TILE_BYTES + 2 * b_tile_bytes;
-  uint8_t* ain_hi = smem;
-  uint8_t* ain_lo = ain_hi + ain_bytes;
-  uint8_t* we0 = ain_lo + ain_bytes;
-  uint8_t* halo0 = we0 + IRB_WE_STAGES * IRB_WE_BYTES;
-  uint8_t* ab0 = halo0 + (size_t)g.halo_stages * halo_bytes;
-  uint8_t* staging = ab0 + (size_t)g.stages * ab_bytes;
-  uint64_t* in_full = reinterpret_cast<uint64_t*>(staging + F_STAGING_BYTES);
-  uint64_t* in_ready = in_full + 1;
-  uint64_t* in_empty = in_ready + 1;
-  uint64_t* we_full = in_empty + 1;            // [2]
-  uint64_t* we_empty = we_full + IRB_WE_STAGES;  // [2]
-  uint64_t* eacc_full = we_empty + IRB_WE_STAGES;
-  uint64_t* eacc_empty = eacc_full + 1;
-  uint64_t* halo_full = eacc_empty + 1;
-  uint64_t* halo_empty = halo_full + g.halo_stages;
-  uint64_t* b_full = halo_empty + g.halo_stages;
-  uint64_t* a_ready = b_full + g.stages;
-  uint64_t* empty = a_ready + g.stages;
-  uint64_t* acc_full = empty + g.stages;  // [2]
-  uint64_t* acc_empty = acc_full + 2;     // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_dw = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 15) & ~(uintptr_t)15);  // [11][Cr]
-  float* s_pw = s_dw + 11 * g.Cr;     // [2][block_n]
-  float* s_e = s_pw + 2 * g.block_n;  // [2][Cr]: folded BN of the expand layer
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_per_img = g.tiles_x * g.tiles_y;
-  const int num_tiles = tiles_per_img * g.n_img;
-  const int n_acc = g.n_main + 1;
-  const int set_cols = n_acc * g.block_n;
-  const int e_cols = g.m_tiles * 64;  // per M tile: 32 main + 32 correction columns
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < e_cols + 2 * set_cols) tmem_cols <<= 1;
-
-  if (warp == 4 && lane == 0) {
-    mbar_init(smem_u32(in_full), 1);
-    mbar_init(smem_u32(in_ready), IRB_XE_WARPS);
-    mbar_init(smem_u32(in_empty), 1);
-    for (int i = 0; i < IRB_WE_STAGES; ++i) {
-      mbar_init(smem_u32(&we_full[i]), 1);
-      mbar_init(smem_u32(&we_empty[i]), 1);
-    }
-    mbar_init(smem_u32(eacc_full), 1);
-    mbar_init(smem_u32(eacc_empty), IRB_XE_WARPS);
-    for (int h = 0; h < g.halo_stages; ++h) {
-      mbar_init(smem_u32(&halo_full[h]), IRB_XE_WARPS);
-      mbar_init(smem_u32(&halo_empty[h]), F_PRODUCER_WARPS);
-    }
-    for (int s = 0; s < g.stages; ++s) {
-      mbar_init(smem_u32(&b_full[s]), 1);
-      mbar_init(smem_u32(&a_ready[s]), F_PRODUCER_WARPS);
-      mbar_init(smem_u32(&empty[s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&acc_full[b]), 1);
-      mbar_init(smem_u32(&acc_empty[b]), 4);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 5) tmem_alloc(smem_u32(tmem_slot), tmem_cols);
-  // per-channel tables; channels C .. Cr-1 (the ragged last 32-block, e.g. C = 144) are zero: they expand to 0
-  // (zero-filled weight rows), convolve to 0 and meet zero-filled projection weights
-  for (int i = threadIdx.x; i < 11 * g.Cr; i += blockDim.x) {
-    const int k = i / g.Cr, c = i - k * g.Cr;
-    float v = 0.f;
-    if (c < g.C) v = k < 9 ? g.dw_w[k * g.C + c] : (k == 9 ? g.dw_scale[c] : g.dw_offset[c]);
-    s_dw[i] = v;
-  }
-  for (int i = threadIdx.x; i < g.block_n; i += blockDim.x) {
-    s_pw[i] = i < g.n_pad ? g.scale[i] : 1.f;
-    s_pw[g.block_n + i] = i < g.n_pad ? g.offset[i] : 0.f;
-  }
-  for (int i = threadIdx.x; i < g.Cr; i += blockDim.x) {
-    s_e[i] = i < g.C ? g.e_scale[i] : 0.f;
-    s_e[g.Cr + i] = i < g.C ? g.e_offset[i] : 0.f;
-  }
-  // rows P .. m_tiles*128-1 of the input operand are never written by TMA: zero them once so that the (unused) MMA
-  // rows stay finite
-  for (int i = threadIdx.x * 16; i < 2 * ain_bytes; i += blockDim.x * 16)
-    if ((i % ain_bytes) >= P * ROW_BYTES) sts128(smem_u32(ain_hi) + (uint32_t)i, make_uint4(0u, 0u, 0u, 0u));
-  fence_proxy_async();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t e_col0 = (uint32_t)(2 * set_cols);  // expand accumulators behind the two projection sets
-  if (threadIdx.x == 0) WB_STAMP(9, 0);
-
-  if (warp == 4) {
-    // ------------------------------------------------------------------ TMA producer
-    if (elect_one()) {
-      int it = 0, j = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-        const int img = t / tiles_per_img, r = t - img * tiles_per_img;
-        const int oy0 = (r / g.tiles_x) * F_TH, ox0 = (r % g.tiles_x) * F_TW;
-        mbar_wait(smem_u32(in_empty), (j & 1) ^ 1);  // the previous tile's expand MMAs have read the operand
-        WB_STAMP(0, j);
-        mbar_expect_tx(smem_u32(in_full), (uint32_t)(P * ROW_BYTES));
-        tma_load_4d(smem_u32(ain_hi), &map_in, smem_u32(in_full), 0, ox0 * S - g.pad_l, oy0 * S - g.pad_t, img);
-        // expand weights run one chunk ahead of the projection weights: the wait for a free A/B stage (= projection
-        // MMAs of an earlier chunk complete) must not hold back the expand GEMM of the next chunk
-        auto load_we = [&](int kb, int itw) {
-          const int ws = itw % IRB_WE_STAGES;
-          mbar_wait(smem_u32(&we_empty[ws]), ((itw / IRB_WE_STAGES) & 1) ^ 1);
-          const uint32_t wb = smem_u32(&we_full[ws]);
-          mbar_expect_tx(wb, IRB_WE_BYTES);
-          tma_load_2d(smem_u32(we0 + (size_t)ws * IRB_WE_BYTES), &map_we, wb, 0, kb * 32);
-          tma_load_2d(smem_u32(we0 + (size_t)ws * IRB_WE_BYTES + 32 * ROW_BYTES), &map_we_lo, wb, 0, kb * 32);
-        };
-        load_we(0, it);
-        for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
-          const int s = it % g.stages;
-          if (kb + 1 < g.k_blocks) load_we(kb + 1, it + 1);
-          mbar_wait(smem_u32(&empty[s]), ((it / g.stages) & 1) ^ 1);
-          const uint32_t bb = smem_u32(&b_full[s]);
-          uint8_t* sb = ab0 + (size_t)s * ab_bytes + 2 * A_TILE_BYTES;
-          mbar_expect_tx(bb, 2 * b_tile_bytes);
-          tma_load_2d(smem_u32(sb), &map_b, bb, kb * 32, 0);
-          tma_load_2d(smem_u32(sb + b_tile_bytes), &map_b_lo, bb, kb * 32, 0);
-        }
-      }
-    }
-  } else if (warp == 5) {
-    // ------------------------------------------------------------------ MMA issuer (expand and projection)
-    const uint32_t idesc = make_idesc(true, BLOCK_M, g.block_n);
-    const uint32_t idesc_e = make_idesc(true, BLOCK_M, 32);
-    int it_e = 0, it_p = 0, j = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-      const int buf = j & 1;
-      const uint32_t acc0 = tmem_base + (uint32_t)(buf * set_cols);
-      mbar_wait(smem_u32(in_ready), j & 1);  // hi tile landed, lo tile written
-      for (int step = 0; step <= g.k_blocks; ++step) {
-        if (step < g.k_blocks) {
-          const int ws = it_e % IRB_WE_STAGES;
-          mbar_wait(smem_u32(&we_full[ws]), (it_e / IRB_WE_STAGES) & 1);
-          mbar_wait(smem_u32(eacc_empty), (it_e & 1) ^ 1);  // the mid-epilogue has drained the previous chunk
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t w_hi = smem_u32(we0 + (size_t)ws * IRB_WE_BYTES), w_lo = w_hi + 32 * ROW_BYTES;
-            for (int mt = 0; mt < g.m_tiles; ++mt) {
-              const uint32_t a_hi = smem_u32(ain_hi) + (uint32_t)(mt * A_TILE_BYTES), a_lo = a_hi + (uint32_t)ain_bytes;
-              const uint32_t d_main = tmem_base + e_col0 + (uint32_t)(mt * 64), d_corr = d_main + 32u;
-              for (int k = 0; k < g.e_ksteps; ++k) {
-                const uint32_t koff = k * UMMA_K_BYTES;
-                umma<true>(d_main, make_sw128_desc(a_hi + koff), make_sw128_desc(w_hi + koff), idesc_e, k != 0);
-                umma<true>(d_corr, make_sw128_desc(a_lo + koff), make_sw128_desc(w_hi + koff), idesc_e, k != 0);
-                umma<true>(d_corr, make_sw128_desc(a_hi + koff), make_sw128_desc(w_lo + koff), idesc_e, 1u);
-              }
-            }
-            umma_commit(smem_u32(&we_empty[ws]));
-            umma_commit(smem_u32(eacc_full));
-            if (step == g.k_blocks - 1) umma_commit(smem_u32(in_empty));
-            WB_STAMP(2, it_e);
-          }
-          __syncwarp();
-          ++it_e;
-        }
-        if (step >= 1) {
-          const int kb = step - 1;
-          const int s = it_p % g.stages;
-          const uint32_t ph = (it_p / g.stages) & 1;
-          if (kb == 0) {
-            mbar_wait(smem_u32(&acc_empty[buf]), ((j >> 1) & 1) ^ 1);
-          }
-          mbar_wait(smem_u32(&a_ready[s]), ph);
-          mbar_wait(smem_u32(&b_full[s]), ph);
-          tc_fence_after();
-          if (elect_one()) {
-            uint8_t* st = ab0 + (size_t)s * ab_bytes;
-            const uint32_t a_hi = smem_u32(st), a_lo = a_hi + A_TILE_BYTES;
-            const uint32_t b_hi = a_lo + A_TILE_BYTES, b_lo = b_hi + b_tile_bytes;
-#pragma unroll
-            for (int k = 0; k < ROW_BYTES / UMMA_K_BYTES; ++k) {
-              const uint32_t koff = k * UMMA_K_BYTES;
-              const int stp = kb * (ROW_BYTES / UMMA_K_BYTES) + k;
-              const uint32_t d_main = acc0 + (uint32_t)((stp % g.n_main) * g.block_n);
-              const uint32_t d_corr = acc0 + (uint32_t)(g.n_main * g.block_n);
-              umma<true>(d_main, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), idesc, stp >= g.n_main);
-              umma<true>(d_corr, make_sw128_desc(a_lo + koff), make_sw128_desc(b_hi + koff), idesc, stp != 0);
-              umma<true>(d_corr, make_sw128_desc(a_hi + koff), make_sw128_desc(b_lo + koff), idesc, 1u);
-            }
-            umma_commit(smem_u32(&empty[s]));
-            if (kb == g.k_blocks - 1) umma_commit(smem_u32(&acc_full[buf]));
-            WB_STAMP(6, it_p);
-          }
-          __syncwarp();
-          ++it_p;
-        }
-      }
-    }
-  } else if (warp < 4) {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;
-    uint8_t* my_stage = staging + (size_t)q * 2 * 4096;
-    const int used = min(g.n_main, g.k_blocks * (ROW_BYTES / UMMA_K_BYTES));
-    int j = 0, chunk_no = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-      const int buf = j & 1;
-      const int img = t / tiles_per_img, r = t - img * tiles_per_img;
-      const int oy0 = (r / g.tiles_x) * F_TH, ox0 = (r % g.tiles_x) * F_TW;
-      mbar_wait(smem_u32(&acc_full[buf]), (j >> 1) & 1);
-      tc_fence_after();
-      if (threadIdx.x == 0) WB_STAMP(7, j);
-      const uint32_t acc0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * set_cols);
-      // this thread's output pixel (row q*32 + lane of the tile = spatial row 2q + lane/16, column lane%16)
-      const int oy = oy0 + 2 * q + (lane >> 4), ox = ox0 + (lane & 15);
-      const bool px_ok = oy < g.OH && ox < g.OW;
-      for (int c0 = 0; c0 < g.block_n; c0 += 32, ++chunk_no) {
-        float y[32];
-        {
-          uint32_t v[32];
-          load_acc32<true>(acc0 + (uint32_t)c0, g.block_n, g.n_main, used, v);
-#pragma unroll
-          for (int i4 = 0; i4 < 8; ++i4) {
-            const int nn = c0 + i4 * 4;
-            const float4 sc = lds128(smem_u32(s_pw + nn)), of = lds128(smem_u32(s_pw + g.block_n + nn));
-            const float scs[4] = {sc.x, sc.y, sc.z, sc.w}, ofs[4] = {of.x, of.y, of.z, of.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float x = affine_rn(__uint_as_float(v[i4 * 4 + e]), scs[e], ofs[e]);
-              y[i4 * 4 + e] = g.act == WB_ACT_RELU6 ? relu6f(x) : x;
-            }
-          }
-        }
-        if (g.residual != nullptr && px_ok) {
-          // bottleneck `Add`: shortcut = the block input at the same pixel (stride 1, C_in == N)
-          const float* rs = g.residual + (((size_t)img * g.IH + oy) * g.IW + ox) * g.Cin + c0;
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            if (c0 + i < g.N) {
-              const float4 rr = *reinterpret_cast<const float4*>(rs + i);
-              y[i + 0] = __fadd_rn(y[i + 0], rr.x);
-              y[i + 1] = __fadd_rn(y[i + 1], rr.y);
-              y[i + 2] = __fadd_rn(y[i + 2], rr.z);
-              y[i + 3] = __fadd_rn(y[i + 3], rr.w);
-            }
-        }
-        if (chunk_no >= 2) {
-          if (lane == 0) bulk_wait_read<1>();
-          __syncwarp();
-        }
-        const uint32_t sb = smem_u32(my_stage + (size_t)(chunk_no & 1) * 4096 + (size_t)lane * 128);
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          uint4 pk;
-          pk.x = __float_as_uint(y[c * 4 + 0]);
-          pk.y = __float_as_uint(y[c * 4 + 1]);
-          pk.z = __float_as_uint(y[c * 4 + 2]);
-          pk.w = __float_as_uint(y[c * 4 + 3]);
-          sts128(sb + (uint32_t)((c ^ (lane & 7)) << 4), pk);
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (elect_one()) {
-          // columns >= N and pixels outside the map are clipped by the tensor map
-          tma_store_4d(&map_out, smem_u32(my_stage + (size_t)(chunk_no & 1) * 4096), c0, ox0, oy0 + 2 * q, img);
-          bulk_commit();
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (threadIdx.x == 0) WB_STAMP(8, j);
-      if (lane == 0) mbar_arrive(smem_u32(&acc_empty[buf]));
-    }
-    if (lane == 0) bulk_wait_read<0>();
-  } else if (warp >= 6 && warp < 14) {
-    // ------------------------------------------------------------------ depthwise producers
-    const int pt = threadIdx.x - IRB_FIRST_DW_THREAD;
-    const int q = pt & 7, slot = pt >> 3;  // channel quad of the k-block, pixel slot
-    constexpr int NCOL = 3 * S + 3;        // input columns feeding 4 adjacent outputs
-    const int TW_IN = g.tw_in;
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
-        const int h = it % g.halo_stages, s = it % g.stages;
-        const int cch = kb * 32 + q * 4;
-        float4 wr[9];
-#pragma unroll
-        for (int k = 0; k < 9; ++k) wr[k] = lds128_ro(smem_u32(s_dw + k * g.Cr + cch));
-        const float4 sc = lds128_ro(smem_u32(s_dw + 9 * g.Cr + cch));
-        const float4 of = lds128_ro(smem_u32(s_dw + 10 * g.Cr + cch));
-        mbar_wait(smem_u32(&halo_full[h]), (it / g.halo_stages) & 1);
-        mbar_wait(smem_u32(&empty[s]), ((it / g.stages) & 1) ^ 1);  // A tiles of this stage are free again
-        if (pt == 0) WB_STAMP(4, it);
-        const uint32_t hal = smem_u32(halo0 + (size_t)h * halo_bytes);
-        const uint32_t a_hi = smem_u32(ab0 + (size_t)s * ab_bytes);
-        const uint32_t a_lo = a_hi + A_TILE_BYTES;
-        const int ty = slot >> 2, x0 = (slot & 3) * 4;
-        const int p00 = (ty * S) * TW_IN + x0 * S;  // halo pixel of the window's top-left corner
-        float4 acc[4];
-#pragma unroll
-        for (int o = 0; o < 4; ++o) acc[o] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-          for (int c = 0; c < NCOL; ++c) {
-            const int hp = p00 + ky * TW_IN + c;  // halo rows are 128 B, 16-byte chunks XOR-swizzled by pixel % 8
-            const float4 x = lds128(hal + (uint32_t)(hp * 128 + ((q ^ (hp & 7)) << 4)));
-#pragma unroll
-            for (int kx = 0; kx < 3; ++kx) {
-              // output o reads input column o*S + kx; accumulation order (ky, kx) as in k_dw_strip
-              if ((c - kx) >= 0 && (c - kx) % S == 0 && (c - kx) / S < 4) {
-                const int o = (c - kx) / S;
-                const float4 ww = wr[ky * 3 + kx];
-                acc[o].x = fmaf(x.x, ww.x, acc[o].x);
-                acc[o].y = fmaf(x.y, ww.y, acc[o].y);
-                acc[o].z = fmaf(x.z, ww.z, acc[o].z);
-                acc[o].w = fmaf(x.w, ww.w, acc[o].w);
-              }
-            }
-          }
-#pragma unroll
-        for (int o = 0; o < 4; ++o) {
-          const int r = ty * F_TW + x0 + o;
-          float v[4] = {affine_rn(acc[o].x, sc.x, of.x), affine_rn(acc[o].y, sc.y, of.y),
-                        affine_rn(acc[o].z, sc.z, of.z), affine_rn(acc[o].w, sc.w, of.w)};
-          uint4 hi, lo;
-          uint32_t* hp = &hi.x;
-          uint32_t* lp = &lo.x;
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float a = g.dw_act == WB_ACT_RELU6 ? relu6f(v[e]) : v[e];
-            const uint32_t hb = __float_as_uint(a) & 0xFFFFE000u;
-            hp[e] = hb;
-            lp[e] = __float_as_uint(__fsub_rn(a, __uint_as_float(hb))) & 0xFFFFE000u;
-          }
-          const uint32_t off = (uint32_t)r * 128u + (uint32_t)((q ^ (r & 7)) << 4);  // 128B swizzle
-          sts128(a_hi + off, hi);
-          sts128(a_lo + off, lo);
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (pt == 0) WB_STAMP(5, it);
-        if (lane == 0) {
-          mbar_arrive(smem_u32(&a_ready[s]));
-          mbar_arrive(smem_u32(&halo_empty[h]));
-        }
-      }
-    }
-  } else if (warp >= 14) {
-    // ------------------------------------------------------------------ input lo-converters + mid-epilogue
-    const int xt = threadIdx.x - IRB_FIRST_XE_THREAD;  // 0..127
-    const int q = warp & 3;                            // TMEM lane quarter of this warp
-    int it = 0, j = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-      const int img_r = t % tiles_per_img;
-      const int iy0 = (img_r / g.tiles_x) * F_TH * S - g.pad_t, ix0 = (img_r % g.tiles_x) * F_TW * S - g.pad_l;
-      // (a) TF32 split of the input tile: hi stays as loaded (the tensor core truncates), lo = (x - hi) truncated
-      mbar_wait(smem_u32(in_full), j & 1);
-      if (xt == 0) WB_STAMP(1, j);
-      {
-        const uint32_t a = smem_u32(ain_hi), lo = smem_u32(ain_lo);
-        for (int i = xt; i < P * (ROW_BYTES / 16); i += 32 * IRB_XE_WARPS) {
-          const uint4 x = lds128u(a + i * 16);
-          uint4 l;
-          l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(x.x & 0xFFFFE000u))) & 0xFFFFE000u;
-          l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(x.y & 0xFFFFE000u))) & 0xFFFFE000u;
-          l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(x.z & 0xFFFFE000u))) & 0xFFFFE000u;
-          l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(x.w & 0xFFFFE000u))) & 0xFFFFE000u;
-          sts128(lo + i * 16, l);
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(in_ready));
-      }
-      // (b) per 32-channel chunk: expand accumulators -> BN + ReLU6 -> depthwise halo chunk
-      for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
-        const int h = it % g.halo_stages;
-        mbar_wait(smem_u32(eacc_full), it & 1);
-        mbar_wait(smem_u32(&halo_empty[h]), ((it / g.halo_stages) & 1) ^ 1);
-        tc_fence_after();
-        if (xt == 0) WB_STAMP(10, it);
-        const uint32_t hal = smem_u32(halo0 + (size_t)h * halo_bytes);
-        const int cch = kb * 32;
-        for (int mt = 0; mt < g.m_tiles; ++mt) {
-          if (mt * 128 + q * 32 >= P) break;  // warp-uniform: this lane quarter holds no halo pixel
-          const int p = mt * 128 + q * 32 + lane;
-          const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + e_col0 + (uint32_t)(mt * 64);
-          uint32_t vm[32], vc[32];
-          tmem_ld16(ta, vm);
-          tmem_ld16(ta + 16u, vm + 16);
-          tmem_ld16(ta + 32u, vc);
-          tmem_ld16(ta + 48u, vc + 16);
-          tmem_ld_wait();
-          const int ly = p / g.tw_in, lx = p - ly * g.tw_in;
-          const int iy = iy0 + ly, ix = ix0 + lx;
-          const bool inside = p < P && iy >= 0 && iy < g.IH && ix >= 0 && ix < g.IW;
-          if (p < P) {
-#pragma unroll
-            for (int k4 = 0; k4 < 8; ++k4) {
-              float4 y = make_float4(0.f, 0.f, 0.f, 0.f);  // outside the map: the depthwise conv's zero padding
-              if (inside) {
-                const float4 sc = lds128_ro(smem_u32(s_e + cch + k4 * 4)), of = lds128_ro(smem_u32(s_e + g.Cr + cch + k4 * 4));
-                const float a0 = __fadd_rn(__uint_as_float(vm[k4 * 4 + 0]), __uint_as_float(vc[k4 * 4 + 0]));
-                const float a1 = __fadd_rn(__uint_as_float(vm[k4 * 4 + 1]), __uint_as_float(vc[k4 * 4 + 1]));
-                const float a2 = __fadd_rn(__uint_as_float(vm[k4 * 4 + 2]), __uint_as_float(vc[k4 * 4 + 2]));
-                const float a3 = __fadd_rn(__uint_as_float(vm[k4 * 4 + 3]), __uint_as_float(vc[k4 * 4 + 3]));
-                y = make_float4(affine_rn(a0, sc.x, of.x), affine_rn(a1, sc.y, of.y), affine_rn(a2, sc.z, of.z),
-                                affine_rn(a3, sc.w, of.w));
-                if (g.e_act == WB_ACT_RELU6) y = make_float4(relu6f(y.x), relu6f(y.y), relu6f(y.z), relu6f(y.w));
-              }
-              sts128(hal + (uint32_t)(p * 128 + ((k4 ^ (p & 7)) << 4)),
-                     make_uint4(__float_as_uint(y.x), __float_as_uint(y.y), __float_as_uint(y.z), __float_as_uint(y.w)));
-            }
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (xt == 0) WB_STAMP(11, it);
-        if (lane == 0) {
-          mbar_arrive(smem_u32(eacc_empty));
-          mbar_arrive(smem_u32(&halo_full[h]));
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
-}
-
-// WB_IRB=1 switches the fused block kernel on.  It is parity-green (tests/test_gpu_v2.py::test_irb_block_kernel) but
-// off by default: with the expand on CUDA cores the block costs 95-115 us where the separate tensor-core expand,
-// depthwise and projection kernels cost 48-75 us (profiles/r02_pipeline_trace.md has the per-role timeline).
-bool irb_enabled() {
-  const char* e = getenv("WB_IRB");
-  return e != nullptr && e[0] == '1';
-}
-
-struct IrbPlan {
-  int block_n, n_main, stages, halo_stages, th_in, tw_in, tiles_x, tiles_y, Cr, k_blocks, m_tiles, e_ksteps;
-  size_t smem;
-};
-
-bool make_irb_plan(const wb_layer& ex, const wb_layer& dw, const wb_layer& pw, IrbPlan* p) {
-  if (dw.stride != 1) return false;  // the stride-2 input halo (561 rows, hi + lo) does not fit beside the halo chunk
-  p->block_n = ((int)pw.n_pad + 31) / 32 * 32;
-  p->Cr = ((int)dw.out_c + 31) / 32 * 32;
-  p->k_blocks = p->Cr / 32;
-  p->n_main = p->k_blocks * 4 <= 16 ? 1 : 2;  // longer accumulation chains rotate over two accumulators
-  p->th_in = (F_TH - 1) * dw.stride + 3;
-  p->tw_in = (F_TW - 1) * dw.stride + 3;
-  p->tiles_x = (dw.out_w + F_TW - 1) / F_TW;
-  p->tiles_y = (dw.out_h + F_TH - 1) / F_TH;
-  const size_t P = (size_t)p->th_in * p->tw_in;
-  p->m_tiles = (int)((P + BLOCK_M - 1) / BLOCK_M);
-  p->e_ksteps = ((int)ex.in_c + 7) / 8;
-  if (p->m_tiles * 64 + 2 * (p->n_main + 1) * p->block_n > 512) return false;  // tensor memory columns
-  const size_t ain = 2 * (size_t)p->m_tiles * A_TILE_BYTES;
-  const size_t halo = (P * ROW_BYTES + 1023) / 1024 * 1024;
-  const size_t ab = 2 * A_TILE_BYTES + 2 * (size_t)p->block_n * ROW_BYTES;
-  const size_t tables = 4 * ((size_t)11 * p->Cr + 2 * p->block_n + 2 * p->Cr) + 64;
-  const size_t fixed = ain + IRB_WE_STAGES * IRB_WE_BYTES + F_STAGING_BYTES + 1024 + 8 * 32 + tables;
-  const size_t budget = 227 * 1024;
-  const int opts[3][2] = {{2, 2}, {1, 2}, {1, 1}};  // {A/B stages, halo chunks}
-  for (auto& o : opts) {
-    const size_t need = o[1] * halo + o[0] * ab + fixed;
-    if (need <= budget) {
-      p->stages = o[0];
-      p->halo_stages = o[1];
-      p->smem = need;
-      return true;
-    }
-  }
-  return false;
-}
-
 }  // namespace
 
 bool fused_dwpw_supported(const TcWeights& tw, int pw_layer_index, const wb_layer& dw, const wb_layer& pw, int n) {
   if (tw.mode != TC_TF32X3 || getenv("WB_NO_FUSE") != nullptr) return false;
   if (dw.op != WB_OP_DW || pw.op != WB_OP_PW) return false;
   if (dw.kh != 3 || dw.kw != 3 || dw.stride != 1) return false;  // stride 2: the 17x33 halo does not fit beside the fp32 rings
-  if (dw.out_c % 32 != 0 || pw.in_c != dw.out_c || pw.n_pad > 128 || pw.out_c % 4 != 0) return false;
-  if (pw.in_c > 256) return false;  // one main accumulator: keep the accumulation chain short
+  // N <= 64: the running sum and the k-block partial (2 x N / 2 registers per consumer thread) fit beside the
+  // depthwise producers' registers
+  if (dw.out_c % 32 != 0 || pw.in_c != dw.out_c || pw.n_pad > 64 || pw.out_c % 4 != 0) return false;
   {  // the fused kernel reads the depthwise input while it writes the 1x1 output: they must not overlap
     const unsigned long long a0 = dw.in_off, a1 = a0 + (unsigned long long)dw.in_h * dw.in_w * dw.in_c;
     const unsigned long long b0 = pw.out_off, b1 = b0 + (unsigned long long)pw.out_h * pw.out_w * pw.out_c;
@@ -912,7 +298,10 @@ bool fused_dwpw_supported(const TcWeights& tw, int pw_layer_index, const wb_laye
   FusedPlan p;
   if (!make_plan(dw, pw, &p)) return false;
   // worth it only when there are enough tiles to keep every SM busy
-  return (long)p.tiles_x * p.tiles_y * n >= 148;
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return (long)p.tiles_x * p.tiles_y * n >= sms;
 }
 
 int fused_launch_dwpw(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_index, int n, const wb_layer& dw,
@@ -943,14 +332,14 @@ int fused_launch_dwpw(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_ind
   g.n_pad = pw.n_pad;
   g.block_n = p.block_n;
   g.k_blocks = (dw.out_c + 31) / 32;
-  g.n_main = p.n_main;
+  g.out = static_cast<float*>(out);
   g.tiles_x = p.tiles_x;
   g.tiles_y = p.tiles_y;
   g.stages = p.stages;
   g.halo_stages = p.halo_stages;
   g.th_in = p.th_in;
   g.tw_in = p.tw_in;
-  alignas(64) CUtensorMap map_in, map_out, map_b, map_b_lo;
+  alignas(64) CUtensorMap map_in, map_b, map_b_lo;
   {
     unsigned long long dims[4] = {(unsigned long long)dw.in_c, dw.in_w, dw.in_h, (unsigned long long)n};
     unsigned long long st[3] = {(unsigned long long)dw.in_c * 4, (unsigned long long)dw.in_w * dw.in_c * 4,
@@ -959,176 +348,36 @@ int fused_launch_dwpw(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_ind
     if (!tc_encode_map(&map_in, in, 4, 4, dims, st, box, false, err)) return 1;
   }
   {
-    unsigned long long dims[4] = {(unsigned long long)pw.out_c, pw.out_w, pw.out_h, (unsigned long long)n};
-    unsigned long long st[3] = {(unsigned long long)pw.out_c * 4, (unsigned long long)pw.out_w * pw.out_c * 4,
-                                (unsigned long long)pw.out_h * pw.out_w * pw.out_c * 4};
-    unsigned box[4] = {32, F_TW, 2, 1};
-    if (!tc_encode_map(&map_out, out, 4, 4, dims, st, box, true, err)) return 1;
-  }
-  {
     unsigned long long dims[2] = {(unsigned long long)w.k, (unsigned long long)w.n_pad};
     unsigned long long st[1] = {(unsigned long long)w.k * 4};
     unsigned box[2] = {32, (unsigned)p.block_n};
     if (!tc_encode_map(&map_b, w.w, 4, 2, dims, st, box, true, err)) return 1;
     if (!tc_encode_map(&map_b_lo, w.w_lo, 4, 2, dims, st, box, true, err)) return 1;
   }
-  static PerDeviceFlag attr_done;
-  if (!attr_done.get()) {
-    cudaError_t e = cudaFuncSetAttribute(k_dwpw_tc_x3<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) {
-      *err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e);
-      return 1;
-    }
-    attr_done.set();
-  }
+  static PerDeviceFlag attr_done[2];
   static int ctas = 0;
   if (ctas == 0) {
-    int dev = 0, sms = 148;
+    int dev = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const char* e = getenv("WB_PERSIST_CTAS");
-    ctas = e ? atoi(e) : sms;
-    if (ctas <= 0 || ctas > sms) ctas = sms;
-  }
-  const long tiles = (long)p.tiles_x * p.tiles_y * n;
-  k_dwpw_tc_x3<1><<<dim3((unsigned)std::min<long>(tiles, ctas)), F_THREADS, p.smem, lc.stream>>>(map_in, map_b, map_b_lo, map_out, g);
-  ++*lc.launch_counter;
-  return 0;
-}
-
-// expand (1x1, ReLU6) -> depthwise 3x3 -> linear 1x1 projection [-> Add]: can the three (four) layers run as k_irb_x3?
-bool fused_irb_supported(const TcWeights& tw, int pw_layer_index, const wb_layer& ex, const wb_layer& dw, const wb_layer& pw,
-                         const wb_layer* add, int n) {
-  if (pw_layer_index < 2 || !tw.layers[pw_layer_index - 2].ready) return false;  // expand weights (hi / lo, K-major)
-  if (tw.mode != TC_TF32X3 || getenv("WB_NO_FUSE") != nullptr || !irb_enabled()) return false;
-  if (ex.op != WB_OP_PW || dw.op != WB_OP_DW || pw.op != WB_OP_PW) return false;
-  if (dw.in_off != ex.out_off || pw.in_off != dw.out_off) return false;
-  if (ex.in_c > 32 || ex.in_c % 4 != 0 || (ex.in_c * 4) % 16 != 0) return false;  // CUDA-core expand: small K only
-  if (dw.kh != 3 || dw.kw != 3 || dw.stride != 1) return false;
-  if (dw.out_c % 16 != 0 || ex.out_c != dw.out_c || pw.in_c != dw.out_c || pw.n_pad > 128 || pw.out_c % 4 != 0) return false;
-  if (!tw.layers[pw_layer_index].ready) return false;
-  IrbPlan p;
-  if (!make_irb_plan(ex, dw, pw, &p)) return false;
-  const unsigned long long a0 = ex.in_off, a1 = a0 + (unsigned long long)ex.in_h * ex.in_w * ex.in_c;
-  const wb_layer& last = add ? *add : pw;
-  const unsigned long long b0 = last.out_off, b1 = b0 + (unsigned long long)last.out_h * last.out_w * last.out_c;
-  if (a0 < b1 && b0 < a1) return false;  // the kernel reads the block input while it writes the block output
-  if (add) {
-    if (add->op != WB_OP_ADD || dw.stride != 1 || ex.in_c != pw.out_c) return false;
-    const bool a_is_pw = add->in_off == pw.out_off, b_is_pw = add->in2_off == pw.out_off;
-    const uint32_t other = a_is_pw ? add->in2_off : add->in_off;
-    if (!(a_is_pw || b_is_pw) || other != ex.in_off) return false;
-  }
-  // worth it only when the tile list keeps most SMs busy
-  return (long)p.tiles_x * p.tiles_y * n >= 96;
-}
-
-int fused_launch_irb(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_index, int n, const wb_layer& ex,
-                     const wb_layer& dw, const wb_layer& pw, bool with_add, const void* in, const float* ex_w,
-                     const float* ex_scale, const float* ex_offset, const float* dw_w, const float* dw_scale,
-                     const float* dw_offset, const float* scale, const float* offset, void* out, std::string* err) {
-  (void)ex_w;
-  const TcLayerWeights& w = tw.layers[pw_layer_index];
-  const TcLayerWeights& we = tw.layers[pw_layer_index - 2];
-  IrbPlan p;
-  if (!make_irb_plan(ex, dw, pw, &p)) {
-    *err = "fused inverted residual block: no shared-memory plan";
-    return 1;
-  }
-  IrbArgs g;
-  g.e_scale = ex_scale;
-  g.e_offset = ex_offset;
-  g.dw_w = dw_w;
-  g.dw_scale = dw_scale;
-  g.dw_offset = dw_offset;
-  g.scale = scale;
-  g.offset = offset;
-  g.residual = with_add ? static_cast<const float*>(in) : nullptr;
-  g.e_act = ex.act;
-  g.dw_act = dw.act;
-  g.act = pw.act;
-  g.Cin = ex.in_c;
-  g.C = dw.out_c;
-  g.Cr = p.Cr;
-  g.IH = dw.in_h;
-  g.IW = dw.in_w;
-  g.pad_t = dw.pad_t;
-  g.pad_l = dw.pad_l;
-  g.OH = dw.out_h;
-  g.OW = dw.out_w;
-  g.n_img = n;
-  g.N = pw.out_c;
-  g.n_pad = pw.n_pad;
-  g.block_n = p.block_n;
-  g.k_blocks = p.k_blocks;
-  g.n_main = p.n_main;
-  g.tiles_x = p.tiles_x;
-  g.tiles_y = p.tiles_y;
-  g.stages = p.stages;
-  g.halo_stages = p.halo_stages;
-  g.th_in = p.th_in;
-  g.tw_in = p.tw_in;
-  g.m_tiles = p.m_tiles;
-  g.e_ksteps = p.e_ksteps;
-  alignas(64) CUtensorMap map_in, map_out, map_b, map_b_lo, map_we, map_we_lo;
-  {
-    // the input halo tile is the K-major A operand of the expand GEMM: 128-byte rows (32 channels, zero-filled beyond
-    // C_in), 128B swizzle, rows in (y, x) order of the halo
-    unsigned long long dims[4] = {(unsigned long long)ex.in_c, ex.in_w, ex.in_h, (unsigned long long)n};
-    unsigned long long st[3] = {(unsigned long long)ex.in_c * 4, (unsigned long long)ex.in_w * ex.in_c * 4,
-                                (unsigned long long)ex.in_h * ex.in_w * ex.in_c * 4};
-    unsigned box[4] = {32, (unsigned)p.tw_in, (unsigned)p.th_in, 1};
-    if (!tc_encode_map(&map_in, in, 4, 4, dims, st, box, true, err)) return 1;
-  }
-  {
-    unsigned long long dims[4] = {(unsigned long long)pw.out_c, pw.out_w, pw.out_h, (unsigned long long)n};
-    unsigned long long st[3] = {(unsigned long long)pw.out_c * 4, (unsigned long long)pw.out_w * pw.out_c * 4,
-                                (unsigned long long)pw.out_h * pw.out_w * pw.out_c * 4};
-    unsigned box[4] = {32, F_TW, 2, 1};
-    if (!tc_encode_map(&map_out, out, 4, 4, dims, st, box, true, err)) return 1;
-  }
-  {
-    unsigned long long dims[2] = {(unsigned long long)w.k, (unsigned long long)w.n_pad};
-    unsigned long long st[1] = {(unsigned long long)w.k * 4};
-    unsigned box[2] = {32, (unsigned)p.block_n};
-    if (!tc_encode_map(&map_b, w.w, 4, 2, dims, st, box, true, err)) return 1;
-    if (!tc_encode_map(&map_b_lo, w.w_lo, 4, 2, dims, st, box, true, err)) return 1;
-  }
-  {
-    // expand weights [n_pad = C (padded)][K = C_in] K-major: one tile = 32 expanded channels x 32 k (zero-filled)
-    unsigned long long dims[2] = {(unsigned long long)we.k, (unsigned long long)we.n_pad};
-    unsigned long long st[1] = {(unsigned long long)we.k * 4};
-    unsigned box[2] = {32, 32};
-    if (!tc_encode_map(&map_we, we.w, 4, 2, dims, st, box, true, err)) return 1;
-    if (!tc_encode_map(&map_we_lo, we.w_lo, 4, 2, dims, st, box, true, err)) return 1;
-  }
-  static PerDeviceFlag attr_done;
-  if (!attr_done.get()) {
-    cudaError_t e = cudaFuncSetAttribute(k_irb_x3<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) {
-      *err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e);
-      return 1;
-    }
-    attr_done.set();
-  }
-  static int ctas = 0;
-  if (ctas == 0) {
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const char* e = getenv("WB_PERSIST_CTAS");
-    ctas = e ? atoi(e) : sms;
-    if (ctas <= 0 || ctas > sms) ctas = sms;
+    cudaDeviceGetAttribute(&ctas, cudaDevAttrMultiProcessorCount, dev);
   }
   const long tiles = (long)p.tiles_x * p.tiles_y * n;
   const dim3 grid((unsigned)std::min<long>(tiles, ctas));
-  k_irb_x3<1><<<grid, IRB_THREADS, p.smem, lc.stream>>>(map_in, map_we, map_we_lo, map_b, map_b_lo, map_out, g);
+  auto launch = [&](auto kern, PerDeviceFlag& done) {
+    if (!done.get()) {
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+      if (e != cudaSuccess) return e;
+      done.set();
+    }
+    kern<<<grid, F_THREADS, p.smem, lc.stream>>>(map_in, map_b, map_b_lo, g);
+    return cudaGetLastError();
+  };
+  const cudaError_t e = p.block_n == 32 ? launch(k_dwpw_tc_x3<1, 32>, attr_done[0]) : launch(k_dwpw_tc_x3<1, 64>, attr_done[1]);
+  if (e != cudaSuccess) {
+    *err = std::string("fused depthwise+pointwise launch: ") + cudaGetErrorString(e);
+    return 1;
+  }
   ++*lc.launch_counter;
   return 0;
 }
 
-#ifdef WB_TRACE
-extern "C" int wb_trace_read_fused(long long* dst) {
-  return (int)cudaMemcpyFromSymbol(dst, wb_trace_buf, sizeof(wb_trace_buf));
-}
-#endif

@@ -443,7 +443,7 @@ int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_l
   FXCK(cudaSetDevice(device));
   cudaDeviceProp prop;
   FXCK(cudaGetDeviceProperties(&prop, device));
-  FXREQ(prop.major == 10, "libwatsor_b200 is built for sm_100a (B200) only");
+  FXREQ(prop.major == 9 && prop.minor == 0, "libwatsor_b200 is built for sm_90a (H100) only");
   std::unique_ptr<wb_fx> fx(new wb_fx());
   fx->device = device;
   FXCK(cudaStreamCreateWithFlags(&fx->stream, cudaStreamNonBlocking));

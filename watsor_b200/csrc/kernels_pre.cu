@@ -164,8 +164,8 @@ __device__ __forceinline__ void resized_pixel_staged(const FrameDesc& fd, const 
 // bytes per staged row for frames up to `max_src_w` wide resized to `in_w`, tile of `tile_w` resized columns; 0 = do
 // not stage (unknown width, or the rows would not fit)
 static int stage_pitch_for(int max_src_w, int in_w, int tile_w, int rows) {
-  // opt-in (WB_STAGE=1): measured slower than the direct path on B200 (profiles/r02_stem.md) -- the byte loads hit L1
-  // and the kernel is issue bound, not latency bound
+  // opt-in (WB_STAGE=1): the direct path reads the source bytes through L1 and is issue bound, not latency bound, so
+  // staging rows in shared memory is not the default
   const char* on = getenv("WB_STAGE");
   if (max_src_w <= 0 || on == nullptr || on[0] != '1' || getenv("WB_NO_STAGE")) return 0;
   const double scale = (double)max_src_w / in_w;

@@ -1,17 +1,18 @@
 // kernels_tc.cu -- tensor-core path for the dense 1x1 convolutions and heads (K4/K6):
-// TMA (cp.async.bulk.tensor) -> 128B-swizzled shared memory -> tcgen05.mma with the accumulator in
-// TMEM -> tcgen05.ld epilogue (folded BatchNorm / bias, ReLU6) -> global.  sm_100a only.
+// TMA (cp.async.bulk.tensor) -> 128B-swizzled shared memory -> wgmma with the fp32 accumulators in registers ->
+// staging tile -> epilogue (folded BatchNorm / bias, ReLU6) -> global.  sm_90a.
 //
-// Two operand modes share one warp-specialised kernel:
-//   TC_BF16    A, W in bf16 (kind::f16), bf16 activations out            -- "fast" mode
+// Three operand modes share one warp-specialised kernel:
+//   TC_BF16    A, W in bf16, bf16 activations out                        -- "fast" mode
+//   TC_TF32X1  A, W in fp32, one TF32 MMA per product                     -- diagnostic
 //   TC_TF32X3  A, W in fp32, every product formed as three TF32 MMAs
 //              (A_hi*W_hi + A_lo*W_hi + A_hi*W_lo, fp32 accumulate)      -- fp32-faithful "parity" mode
-// In TF32X3 the activation tile lands in shared memory as raw fp32; converter warps split it in place
-// into hi = a & 0xffffe000 and lo = (a - hi) & 0xffffe000 (both exactly representable in TF32, so
-// the tensor core's own input rounding never matters); the weights are split once on the host.
+// In TF32X3 the activation tile lands in shared memory as raw fp32; each consumer warpgroup splits its own 64 rows in
+// place into hi = a & 0xffffe000 and lo = (a - hi) & 0xffffe000 (both exactly representable in TF32); the weights
+// are split once on the host.
 //
-// Warp roles (192 + 128*X3 threads): warp 0 TMA producer, warp 1 TMEM owner + MMA issuer,
-// warps 2..5 epilogue (TMEM lane quarter = warp_idx % 4), warps 6..9 converters (TF32X3 only).
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups (rows 0..63 / 64..127 of the 128-row tile: split,
+// wgmma, epilogue), warp 8 = TMA producer.
 #include <cuda.h>
 
 #include <algorithm>
@@ -38,10 +39,8 @@ struct TcArgs {
   // KxK / strided convolutions: the A tile of k-block kb is the tap (kb / cpb) of the filter window, channel block
   // kb % cpb, fetched by a 4-D TMA box {32 ch, OW, OH, imgs} whose traversal strides are the conv stride
   int conv, cpb, conv_kw, conv_pad_t, conv_pad_l;
-  int ring_bytes;     // k_gemm_tc: bytes of the stage ring (re-used as the epilogue's staging tile)
+  int ring_bytes;     // bytes of the stage ring (re-used as the epilogue's staging tile)
   int rows_per_tile;  // GEMM rows one CTA produces (128, or imgs_per_tile*OH*OW for conv tiles)
-  int ta_stages;  // > 0: A operand staged in tensor memory (k_gemm_tc<2, true>), ring of 64-column hi/lo pairs
-  int n_main;  // TF32X3: the hi*hi products rotate over n_main TMEM accumulators (+1 for the corrections)
   int act, is_head, anchors_per_loc, row_off, n_box, num_anchors, ncp1, hw;
 };
 
@@ -53,8 +52,6 @@ __device__ __forceinline__ void tma_load_4d_tc(uint32_t dst, const CUtensorMap* 
       "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-// barrier among the four epilogue warps only (128 threads, hardware barrier 1)
-__device__ __forceinline__ void epilogue_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -133,289 +130,129 @@ __device__ __forceinline__ void copy_out_row(const TcArgs& g, const uint8_t* sme
   }
 }
 
-// MODE 0: bf16 operands; MODE 1: tf32 single product (diagnostic); MODE 2: tf32 x3 split
-// TA (TF32X3 only; default, WB_TMEM_A=0 disables): the converter warps write the hi / lo rows into tensor memory
-// (tcgen05.st) and the MMAs take A from there, so the shared-memory port carries neither the converter writes
-// nor the A operand reads (DESIGN.md section 8, item 1).
-// TWO: compiled for two co-resident CTAs per SM (<= 102 registers; the launcher keeps shared memory <= 110 KB and
-// tensor memory <= 256 columns).  The k-loop of one CTA then overlaps the prologue / epilogue of the other.
-template <int MODE, bool TA = false, bool TWO = false>
-__global__ void __launch_bounds__(MODE == 2 ? 320 : 192, TWO ? 2 : 1)
+constexpr int GEMM_THREADS = 288;
+constexpr int GEMM_PRODUCER_WARP = 8;
+
+// barrier among the 128 threads of consumer warpgroup `wg` (hardware barriers 2 and 3)
+__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
+
+// MODE 0: bf16 operands; MODE 1: tf32 single product (diagnostic); MODE 2: tf32 x3 split.  BN: N tile (32 / 64 / 128).
+template <int MODE, int BN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
     k_gemm_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
               const __grid_constant__ CUtensorMap map_b_lo, TcArgs g) {
   constexpr bool TF32 = MODE != 0;
   constexpr bool X3 = MODE == 2;
   constexpr int ELEM = TF32 ? 4 : 2;
   constexpr int K_PER_BLOCK = ROW_BYTES / ELEM;
+  constexpr int B_TILE_BYTES = BN * ROW_BYTES;
+  constexpr int SLOTS = X3 ? 2 : 1;  // raw / hi tile (+ lo tile)
+  constexpr int STAGE_BYTES = (A_TILE_BYTES + B_TILE_BYTES) * SLOTS;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int b_tile_bytes = g.block_n * ROW_BYTES;
-  static_assert(!TA || X3, "TMEM-staged A exists for the 3xTF32 mode only");
-  constexpr int A_SLOTS = TA ? 1 : (X3 ? 2 : 1);  // fp32 tile (+ lo tile when the split stays in smem)
-  const int stage_bytes = A_TILE_BYTES * A_SLOTS + b_tile_bytes * (X3 ? 2 : 1);
-  uint8_t* bar_base = smem + (size_t)g.ring_bytes;  // >= stages * stage_bytes (and >= the epilogue staging tile)
-  uint64_t* full = reinterpret_cast<uint64_t*>(bar_base);          // TMA landed
-  uint64_t* empty = full + g.stages;                               // MMAs done with the stage
-  uint64_t* conv = empty + g.stages;                               // converters done (X3)
-  uint64_t* acc_full = conv + g.stages;                            // accumulator complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-  uint64_t* ta_conv = acc_full + 2;   // [4] TA: hi/lo rows of a TMEM stage written
-  uint64_t* ta_empty = ta_conv + 4;   // [4] TA: MMAs done with a TMEM stage
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)g.ring_bytes);  // TMA landed
+  uint64_t* empty = full + g.stages;                                           // both warpgroups done with the stage
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) WB_STAMP(8, 0);  // kernel entry
-  if (threadIdx.x == 32) {  // descriptor fetch off the critical path of the first TMA load
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-    if (X3) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_lo) : "memory");
-  }
-  const int m0 = blockIdx.x * g.rows_per_tile, n0 = blockIdx.y * g.block_n;
+  const int m0 = blockIdx.x * g.rows_per_tile, n0 = blockIdx.y * BN;
   const int kb0 = blockIdx.z * g.kb_per;
   const int nkb = min(g.k_blocks, kb0 + g.kb_per) - kb0;  // k-blocks of this split (>= 1)
-  // TF32X3 keeps n_main + 1 accumulators (see the MMA issuer); columns must be a power of two >= 32
-  const int n_acc = X3 ? g.n_main + 1 : 1;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < g.block_n * n_acc + (TA ? g.ta_stages * 64 : 0)) tmem_cols <<= 1;
-  const uint32_t a_col0 = (uint32_t)(g.block_n * n_acc);  // TA: first column of the A ring
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < g.stages; ++s) {
       mbar_init(smem_u32(&full[s]), 1);
-      mbar_init(smem_u32(&empty[s]), 1);
-      mbar_init(smem_u32(&conv[s]), 4);  // one arrive per converter warp
+      mbar_init(smem_u32(&empty[s]), 2);  // one arrive per consumer warpgroup
     }
-    if (TA)
-      for (int s = 0; s < 4; ++s) {
-        mbar_init(smem_u32(&ta_conv[s]), 4);
-        mbar_init(smem_u32(&ta_empty[s]), 1);
-      }
-    mbar_init(smem_u32(acc_full), 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (threadIdx.x == 0) WB_STAMP(7, 0);
 
-  if (warp == 0) {
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+
+  if (warp == GEMM_PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one()) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
       for (int it = 0; it < nkb; ++it) {
         const int kb = kb0 + it;
         const int s = it % g.stages;
         const uint32_t ph = (it / g.stages) & 1;
         mbar_wait(smem_u32(&empty[s]), ph ^ 1);
-        WB_STAMP(0, it);
-        uint8_t* st = smem + (size_t)s * stage_bytes;
+        uint8_t* st = smem + (size_t)s * STAGE_BYTES;
         const uint32_t bar = smem_u32(&full[s]);
         if (g.conv) {
           // rows_per_tile = imgs * OH * OW rows arrive (the box never leaves the image range: whole images per tile);
           // taps that fall outside the input are zero-filled by TMA = TF SAME padding
-          mbar_expect_tx(bar, g.rows_per_tile * ROW_BYTES + b_tile_bytes * (X3 ? 2 : 1));
+          mbar_expect_tx(bar, g.rows_per_tile * ROW_BYTES + B_TILE_BYTES * SLOTS);
           const int tap = kb / g.cpb, cb = kb - tap * g.cpb;
           const int ky = tap / g.conv_kw, kx = tap - ky * g.conv_kw;
           tma_load_4d_tc(smem_u32(st), &map_a, bar, cb * K_PER_BLOCK, kx - g.conv_pad_l, ky - g.conv_pad_t, m0 / g.hw);
         } else {
-          mbar_expect_tx(bar, A_TILE_BYTES + b_tile_bytes * (X3 ? 2 : 1));
+          mbar_expect_tx(bar, A_TILE_BYTES + B_TILE_BYTES * SLOTS);
           tma_load_2d(smem_u32(st), &map_a, bar, kb * K_PER_BLOCK, m0);
         }
-        uint8_t* sb = st + A_TILE_BYTES * A_SLOTS;
+        uint8_t* sb = st + A_TILE_BYTES * SLOTS;
         tma_load_2d(smem_u32(sb), &map_b, bar, kb * K_PER_BLOCK, n0);
-        if (X3) tma_load_2d(smem_u32(sb + b_tile_bytes), &map_b_lo, bar, kb * K_PER_BLOCK, n0);
+        if (X3) tma_load_2d(smem_u32(sb + B_TILE_BYTES), &map_b_lo, bar, kb * K_PER_BLOCK, n0);
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = make_idesc(TF32, BLOCK_M, g.block_n);
+  } else {
+    // ------------------------------------------------------------------ consumer warpgroups
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    float part[X3 ? BN / 2 : 1];
     for (int it = 0; it < nkb; ++it) {
       const int s = it % g.stages;
-      const uint32_t ph = (it / g.stages) & 1;
-      const int ts = TA ? it % g.ta_stages : 0;
-      if (TA) {
-        mbar_wait(smem_u32(&full[s]), ph);  // B tiles (the converters waited on it too; this is the issuer's own acquire)
-        mbar_wait(smem_u32(&ta_conv[ts]), (it / g.ta_stages) & 1);
+      mbar_wait(smem_u32(&full[s]), (it / g.stages) & 1);
+      const uint32_t st = smem_u32(smem + (size_t)s * STAGE_BYTES);
+      const uint32_t a_hi = st + (uint32_t)(wg * 64 * ROW_BYTES), a_lo = a_hi + A_TILE_BYTES;
+      const uint32_t b_hi = st + (uint32_t)(A_TILE_BYTES * SLOTS), b_lo = b_hi + B_TILE_BYTES;
+      if (X3) {
+#pragma unroll
+        for (int i = t; i < 64 * ROW_BYTES / 16; i += 128) split_tf32(a_hi + (uint32_t)(i * 16), a_lo + (uint32_t)(i * 16));
+        fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
+        wg_bar_sync(wg);
+        wg_x3_kblock_sum<BN>(acc, part, a_hi, a_lo, b_hi, b_lo);
       } else {
-        mbar_wait(smem_u32(X3 ? &conv[s] : &full[s]), ph);
+        wgmma_fence();
+        wg_mma_kblock<TF32, false, BN>(acc, a_hi, a_lo, b_hi, b_lo, 1u);
+        wgmma_commit();
+        wgmma_wait_all();
       }
-      tc_fence_after();
-      if (elect_one()) {
-        WB_STAMP(3, it);
-        uint8_t* st = smem + (size_t)s * stage_bytes;
-        const uint32_t a_hi = smem_u32(st), a_lo = a_hi + A_TILE_BYTES;
-        const uint32_t b_hi = smem_u32(st + A_TILE_BYTES * A_SLOTS), b_lo = b_hi + b_tile_bytes;
-        const uint32_t ta_hi = tmem_base + a_col0 + (uint32_t)(ts * 64), ta_lo = ta_hi + 32u;
-        // The tensor core adds into the fp32 accumulator with truncation (round toward zero), a bias
-        // that grows with the length of the accumulation chain.  TF32X3 therefore rotates the dominant
-        // hi*hi products over n_main accumulators and keeps the two small correction products in a
-        // separate one; the epilogue adds the partial sums with round-to-nearest.
-#pragma unroll
-        for (int k = 0; k < ROW_BYTES / UMMA_K_BYTES; ++k) {
-          const uint32_t koff = k * UMMA_K_BYTES;
-          const int step = it * (ROW_BYTES / UMMA_K_BYTES) + k;
-          if (!X3) {
-            umma<TF32>(tmem_base, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), idesc, step != 0);
-          } else if (TA) {
-            const uint32_t d_main = tmem_base + (uint32_t)((step % g.n_main) * g.block_n);
-            const uint32_t d_corr = tmem_base + (uint32_t)(g.n_main * g.block_n);
-            const uint32_t kc = (uint32_t)(k * (UMMA_K_BYTES / 4));  // 8 TF32 columns per k-step
-            umma_tf32_ta(d_main, ta_hi + kc, make_sw128_desc(b_hi + koff), idesc, step >= g.n_main);
-            umma_tf32_ta(d_corr, ta_lo + kc, make_sw128_desc(b_hi + koff), idesc, step != 0);
-            umma_tf32_ta(d_corr, ta_hi + kc, make_sw128_desc(b_lo + koff), idesc, 1u);
-          } else {
-            const uint32_t d_main = tmem_base + (uint32_t)((step % g.n_main) * g.block_n);
-            const uint32_t d_corr = tmem_base + (uint32_t)(g.n_main * g.block_n);
-            umma<TF32>(d_main, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), idesc, step >= g.n_main);
-            umma<TF32>(d_corr, make_sw128_desc(a_lo + koff), make_sw128_desc(b_hi + koff), idesc, step != 0);
-            umma<TF32>(d_corr, make_sw128_desc(a_hi + koff), make_sw128_desc(b_lo + koff), idesc, 1u);
-          }
-        }
-        umma_commit(smem_u32(&empty[s]));
-        if (TA) umma_commit(smem_u32(&ta_empty[ts]));
-        if (it == nkb - 1) umma_commit(smem_u32(acc_full));
-        WB_STAMP(4, it);
-      }
-      __syncwarp();
-    }
-  } else if (X3 && warp >= 6) {
-    // ------------------------------------------------------------------ converters (A -> hi / lo)
-    const int t = threadIdx.x - 192;  // 0..127
-    if (TA) {
-      // thread = one row of the tile: TMEM lane quarter of this warp x lane
-      const int q = warp & 3, row = q * 32 + lane;
-      for (int it = 0; it < nkb; ++it) {
-        const int s = it % g.stages, ts = it % g.ta_stages;
-        mbar_wait(smem_u32(&full[s]), (it / g.stages) & 1);
-        mbar_wait(smem_u32(&ta_empty[ts]), ((it / g.ta_stages) & 1) ^ 1);
-        tc_fence_after();
-        if (t == 0) WB_STAMP(1, it);
-        const uint32_t a = smem_u32(smem + (size_t)s * stage_bytes) + (uint32_t)row * 128u;
-        uint32_t hi[32], lo[32];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const uint4 x = lds128u(a + (uint32_t)((c ^ (row & 7)) << 4));  // 128B swizzle: chunk ^= row % 8
-          const uint32_t xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const uint32_t h = xs[e] & 0xFFFFE000u;
-            hi[c * 4 + e] = h;
-            lo[c * 4 + e] = __float_as_uint(__fsub_rn(__uint_as_float(xs[e]), __uint_as_float(h))) & 0xFFFFE000u;
-          }
-        }
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + a_col0 + (uint32_t)(ts * 64);
-        tmem_st32(taddr, hi);
-        tmem_st32(taddr + 32u, lo);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (t == 0) WB_STAMP(2, it);
-        if (lane == 0) mbar_arrive(smem_u32(&ta_conv[ts]));
-      }
-    } else
-    for (int it = 0; it < nkb; ++it) {
-      const int s = it % g.stages;
-      const uint32_t ph = (it / g.stages) & 1;
-      mbar_wait(smem_u32(&full[s]), ph);
-      if (t == 0) WB_STAMP(1, it);
-      const uint32_t a = smem_u32(smem + (size_t)s * stage_bytes);
-      const uint32_t lo = a + A_TILE_BYTES;
-#pragma unroll 4
-      for (int i = t; i < A_TILE_BYTES / 16; i += 128) {
-        uint4 x = lds128u(a + i * 16), h, l;
-        h.x = x.x & 0xFFFFE000u;
-        h.y = x.y & 0xFFFFE000u;
-        h.z = x.z & 0xFFFFE000u;
-        h.w = x.w & 0xFFFFE000u;
-        l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x))) & 0xFFFFE000u;
-        l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y))) & 0xFFFFE000u;
-        l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z))) & 0xFFFFE000u;
-        l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w))) & 0xFFFFE000u;
-        // hi stays as loaded: the tensor core truncates fp32 inputs to tf32 exactly like the mask above
-        sts128(lo + i * 16, l);
-      }
-      fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      __syncwarp();
-      if (t == 0) WB_STAMP(2, it);
-      if (lane == 0) mbar_arrive(smem_u32(&conv[s]));
+      wg_bar_sync(wg);  // every warp of the warpgroup has seen its MMAs complete: the stage may be refilled
+      if (t == 0) mbar_arrive(smem_u32(&empty[s]));
     }
   }
 
   // ------------------------------------------------------------------ epilogue
-  // Every MMA has completed (acc_full), so the stage ring is dead: it becomes a [128][block_n + 4] fp32 staging tile
-  // (row pitch = 4 mod 16 words: the 8 lanes of a store phase hit 8 different bank groups).
-  // Phase 1 (warps 2.., thread = accumulator row): TMEM -> registers -> RAW accumulator sums -> staging.  A warp may
-  // read TMEM lane quarter warp % 4, so the four converter warps (idle by now) take every second 16-column chunk of
-  // "their" quarter: 8 warps instead of 4 on a phase that is bound by instruction latency, not bandwidth.
-  // Phase 2 (all warps, lanes along the columns): staging -> folded BN / bias, ReLU6, optional bottleneck shortcut ->
-  // 128-byte coalesced stores (dense [M][N], or the head scatter).
+  // Every MMA has completed, so the stage ring is dead: it becomes a [128][BN + 4] fp32 staging tile (row pitch = 4
+  // mod 16 words).  Phase 1 (consumer threads): raw accumulators -> staging.  Phase 2 (all warps, lanes along the
+  // columns): staging -> folded BN / bias, ReLU6, optional bottleneck shortcut -> coalesced stores (dense [M][N], or
+  // the head scatter into the concatenated box-encoding / class-logit tensors).
   // Split-K: the `splits` CTAs of an output tile form one thread-block cluster; after a cluster barrier CTA z
   // reduces rows z, z + splits, ... over all members' staging tiles through distributed shared memory, always in the
   // order z' = 0, 1, ... (deterministic), then runs the same phase 2 arithmetic.
-  const int pitch = g.block_n + 4;
-  if (warp >= 2) {
-    const int q = warp & 3;  // TMEM lane quarter this warp may read
-    const int row = q * 32 + lane;
-    const int part = warp >= 6 ? 1 : 0, parts = X3 ? 2 : 1;
-    mbar_wait(smem_u32(acc_full), 0);
-    tc_fence_after();
-    if (threadIdx.x == 64) WB_STAMP(5, 0);
-    const uint32_t stg_row = smem_u32(smem) + (uint32_t)(row * pitch * 4);
-    // 16 columns per step; the tcgen05.ld of the next step are issued before this one is processed, so the TMEM
-    // round trip overlaps the staging work
-    const int used = min(g.n_main, nkb * (ROW_BYTES / UMMA_K_BYTES));
-    const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16);
-    const int nch = g.block_n >> 4;
-    uint32_t bufs[TWO ? 1 : 2][4][16];  // [double buffer][main0, main1, main2, corr][16 columns]
-    auto issue = [&](int ch, int b) {
-      const uint32_t t = tbase + (uint32_t)(ch * 16);
-      tmem_ld16(t, bufs[b][0]);
-      if (X3) {
-        if (used > 1) tmem_ld16(t + (uint32_t)g.block_n, bufs[b][1]);
-        if (used > 2) tmem_ld16(t + (uint32_t)(2 * g.block_n), bufs[b][2]);
-        tmem_ld16(t + (uint32_t)(g.n_main * g.block_n), bufs[b][3]);
-      }
-    };
-    constexpr int NB = TWO ? 1 : 2;
-    if (!TWO && part < nch) issue(part, 0);
-#pragma unroll 1
-    for (int ch = part; ch < nch; ch += NB * parts) {
+  const int pitch = BN + 4;
+  __syncthreads();  // both warpgroups are past their last MMA: the ring may be overwritten
+  if (warp < GEMM_PRODUCER_WARP) {
+    const int row = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+    const uint32_t stg = smem_u32(smem) + (uint32_t)((row * pitch + 2 * (lane & 3)) * 4);
 #pragma unroll
-      for (int b = 0; b < NB; ++b) {
-        const int c = ch + b * parts;
-        if (c >= nch) break;
-        if (TWO) issue(c, 0);
-        tmem_ld_wait();
-        if (!TWO && c + parts < nch) issue(c + parts, b ^ 1);
-        const int c0 = c * 16;
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          float y4[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float a = __uint_as_float(bufs[b][0][j + e]);
-            if (X3) {  // fixed order ((main0 + main1) + main2) + corr, round to nearest
-              if (used > 1) a = __fadd_rn(a, __uint_as_float(bufs[b][1][j + e]));
-              if (used > 2) a = __fadd_rn(a, __uint_as_float(bufs[b][2][j + e]));
-              a = __fadd_rn(a, __uint_as_float(bufs[b][3][j + e]));
-            }
-            y4[e] = a;
-          }
-          sts128(stg_row + (uint32_t)((c0 + j) * 4),
-                 make_uint4(__float_as_uint(y4[0]), __float_as_uint(y4[1]), __float_as_uint(y4[2]), __float_as_uint(y4[3])));
-        }
-      }
+    for (int i = 0; i < BN / 2; i += 4) {
+      const uint32_t c = (uint32_t)((i >> 2) * 8 * 4);
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stg + c), "f"(acc[i]), "f"(acc[i + 1]) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stg + c + (uint32_t)(8 * pitch * 4)), "f"(acc[i + 2]), "f"(acc[i + 3])
+                   : "memory");
     }
-    tc_fence_before();
   }
-  __syncthreads();  // the staging tile is complete (and every TMEM read has retired)
-  if (threadIdx.x == 64) WB_STAMP(10, 0);
+  __syncthreads();  // the staging tile is complete
   const int n_warps = blockDim.x >> 5;
   const int rows = min(g.rows_per_tile, g.M - m0);
   if (g.splits > 1) {
     // all `splits` CTAs of this tile (one cluster) have staged their partial tiles
     cluster_sync_all();
-    if (threadIdx.x == 64) WB_STAMP(11, 0);
     const int z = (int)cluster_ctarank();
     for (int r = z + g.splits * warp; r < rows; r += n_warps * g.splits)
       copy_out_row<TF32>(g, smem, pitch, r, m0, n0, lane, g.splits, 1);
@@ -493,7 +330,7 @@ __global__ void __launch_bounds__(MODE == 2 ? 320 : 192, TWO ? 2 : 1)
       for (int u = 0; u < 4; ++u) {
         rr[u] = r_it;
         cc[u] = c_it * 4;
-        if (i0 + T * u < items) {
+        if (i0 + T * u < items && n0 + cc[u] < g.N) {
           y[u] = lds128(sbase + (uint32_t)((rr[u] * pitch + cc[u]) * 4));
           // folded BN / bias of these 4 columns (every row re-reads the same few lines: L1 hits)
           sc[u] = __ldg(reinterpret_cast<const float4*>(g.scale + n0 + cc[u]));
@@ -526,261 +363,8 @@ __global__ void __launch_bounds__(MODE == 2 ? 320 : 192, TWO ? 2 : 1)
       }
     }
   }
-  if (threadIdx.x == 64) WB_STAMP(6, 0);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
-  if (threadIdx.x == 0) WB_STAMP(9, 0);  // kernel exit
 }
 
-
-// ---------------------------------------------------------------------------------------------------
-// Persistent variant for layers with many output tiles (the 150x150 / 75x75 / 38x38 maps): one CTA per
-// SM walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...; the smem stage ring runs continuously
-// across tiles, the TMEM accumulators are double-buffered (the epilogue of tile j overlaps the TMA /
-// convert / MMA work of tile j+1) and the epilogue leaves through 128B-swizzled staging buffers and
-// TMA stores (cp.async.bulk.tensor ... global.shared::cta), i.e. fully coalesced 128-byte rows.
-constexpr int STAGING_BYTES = 4 * 2 * 4096;  // 4 epilogue warps x 2 buffers x (32 rows x 128 B); 3xTF32: 8 warps, twice that
-
-template <int MODE>
-__global__ void __launch_bounds__(MODE == 2 ? 448 : 192, 1)
-    k_gemm_tc_persist(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                      const __grid_constant__ CUtensorMap map_b_lo, const __grid_constant__ CUtensorMap map_out,
-                      TcArgs g) {
-  constexpr bool TF32 = MODE != 0;
-  constexpr bool X3 = MODE == 2;
-  constexpr int ELEM = TF32 ? 4 : 2;
-  constexpr int K_PER_BLOCK = ROW_BYTES / ELEM;
-  constexpr int CW = TF32 ? 32 : 64;  // output columns per 128-byte staging row
-  // 3xTF32: a second group of four epilogue warps (warps 10..13; TMEM lane quarter = warp % 4 as for warps 2..5) takes
-  // every second column chunk -- the epilogue is bound by instruction latency (one warp per scheduler), not bandwidth
-  constexpr int EPI_WARPS = X3 ? 8 : 4;
-  constexpr int STAGING = EPI_WARPS * 2 * 4096;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int b_tile_bytes = g.block_n * ROW_BYTES;
-  const int stage_bytes = A_TILE_BYTES * (X3 ? 2 : 1) + b_tile_bytes * (X3 ? 2 : 1);
-  uint8_t* staging = smem + (size_t)g.stages * stage_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(staging + STAGING);
-  uint64_t* empty = full + g.stages;
-  uint64_t* conv = empty + g.stages;
-  uint64_t* acc_full = conv + g.stages;  // [2]
-  uint64_t* acc_empty = acc_full + 2;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  // folded BN / bias of every output column, loaded once per CTA (the epilogue warps are latency bound: 64 global loads
-  // per 32-column chunk were most of their instruction stream)
-  float* s_so = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 15) & ~(uintptr_t)15);  // [2][n_pad]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tiles = (g.n_pad + g.block_n - 1) / g.block_n;  // the last N tile may be ragged (N = 144 = 128 + 16)
-  const int nt_cols = n_tiles * g.block_n;
-  const int num_tiles = ((g.M + BLOCK_M - 1) / BLOCK_M) * n_tiles;
-  const int n_acc = X3 ? g.n_main + 1 : 1;
-  const int set_cols = n_acc * g.block_n;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < 2 * set_cols) tmem_cols <<= 1;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < g.stages; ++s) {
-      mbar_init(smem_u32(&full[s]), 1);
-      mbar_init(smem_u32(&empty[s]), 1);
-      mbar_init(smem_u32(&conv[s]), 4);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&acc_full[b]), 1);
-      mbar_init(smem_u32(&acc_empty[b]), EPI_WARPS);  // one arrive per epilogue warp
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), tmem_cols);
-  for (int i = threadIdx.x; i < nt_cols; i += blockDim.x) {
-    s_so[i] = i < g.n_pad ? g.scale[i] : 1.f;
-    s_so[nt_cols + i] = i < g.n_pad ? g.offset[i] : 0.f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      int it = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int m0 = (t / n_tiles) * BLOCK_M, n0 = (t % n_tiles) * g.block_n;
-        for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
-          const int s = it % g.stages;
-          const uint32_t ph = (it / g.stages) & 1;
-          mbar_wait(smem_u32(&empty[s]), ph ^ 1);
-          uint8_t* st = smem + (size_t)s * stage_bytes;
-          const uint32_t bar = smem_u32(&full[s]);
-          mbar_expect_tx(bar, A_TILE_BYTES + b_tile_bytes * (X3 ? 2 : 1));
-          tma_load_2d(smem_u32(st), &map_a, bar, kb * K_PER_BLOCK, m0);
-          uint8_t* sb = st + A_TILE_BYTES * (X3 ? 2 : 1);
-          tma_load_2d(smem_u32(sb), &map_b, bar, kb * K_PER_BLOCK, n0);
-          if (X3) tma_load_2d(smem_u32(sb + b_tile_bytes), &map_b_lo, bar, kb * K_PER_BLOCK, n0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc = make_idesc(TF32, BLOCK_M, g.block_n);
-    int it = 0, j = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-      const int buf = j & 1;
-      mbar_wait(smem_u32(&acc_empty[buf]), ((j >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t acc0 = tmem_base + (uint32_t)(buf * set_cols);
-      for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
-        const int s = it % g.stages;
-        const uint32_t ph = (it / g.stages) & 1;
-        mbar_wait(smem_u32(X3 ? &conv[s] : &full[s]), ph);
-        tc_fence_after();
-        if (elect_one()) {
-          uint8_t* st = smem + (size_t)s * stage_bytes;
-          const uint32_t a_hi = smem_u32(st), a_lo = a_hi + A_TILE_BYTES;
-          const uint32_t b_hi = smem_u32(st + A_TILE_BYTES * (X3 ? 2 : 1)), b_lo = b_hi + b_tile_bytes;
-#pragma unroll
-          for (int k = 0; k < ROW_BYTES / UMMA_K_BYTES; ++k) {
-            const uint32_t koff = k * UMMA_K_BYTES;
-            const int step = kb * (ROW_BYTES / UMMA_K_BYTES) + k;
-            if (!X3) {
-              umma<TF32>(acc0, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), idesc, step != 0);
-            } else {
-              const uint32_t d_main = acc0 + (uint32_t)((step % g.n_main) * g.block_n);
-              const uint32_t d_corr = acc0 + (uint32_t)(g.n_main * g.block_n);
-              umma<TF32>(d_main, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), idesc, step >= g.n_main);
-              umma<TF32>(d_corr, make_sw128_desc(a_lo + koff), make_sw128_desc(b_hi + koff), idesc, step != 0);
-              umma<TF32>(d_corr, make_sw128_desc(a_hi + koff), make_sw128_desc(b_lo + koff), idesc, 1u);
-            }
-          }
-          umma_commit(smem_u32(&empty[s]));
-          if (kb == g.k_blocks - 1) umma_commit(smem_u32(&acc_full[buf]));
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 6 || warp >= 10) {
-    const int q = warp & 3;
-    const int grp = warp >= 10 ? 1 : 0;
-    uint8_t* my_stage = staging + (size_t)(grp * 4 + q) * 2 * 4096;
-    const int used = X3 ? min(g.n_main, g.k_blocks * (ROW_BYTES / UMMA_K_BYTES)) : 1;
-    int j = 0, chunk_no = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++j) {
-      const int buf = j & 1;
-      const int m0 = (t / n_tiles) * BLOCK_M, n0 = (t % n_tiles) * g.block_n;
-      mbar_wait(smem_u32(&acc_full[buf]), (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t acc0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * set_cols);
-      for (int c0 = 0, ci = 0; c0 < g.block_n; c0 += CW, ++ci) {
-        if (n0 + c0 >= g.N) break;  // ragged last N tile: these columns do not exist
-        if (EPI_WARPS == 8 && (ci & 1) != grp) continue;
-        float y[CW];
-#pragma unroll
-        for (int h = 0; h < CW / 32; ++h) {
-          uint32_t v[32];
-          load_acc32<X3>(acc0 + (uint32_t)(c0 + h * 32), g.block_n, g.n_main, used, v);
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            const int nn = n0 + c0 + h * 32 + i;
-            const float4 sc = lds128_ro(smem_u32(s_so + nn)), of = lds128_ro(smem_u32(s_so + nt_cols + nn));
-            const float scs[4] = {sc.x, sc.y, sc.z, sc.w}, ofs[4] = {of.x, of.y, of.z, of.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float x = affine_rn(__uint_as_float(v[i + e]), scs[e], ofs[e]);
-              y[h * 32 + i + e] = g.act == WB_ACT_RELU6 ? relu6f(x) : x;
-            }
-          }
-          if (TF32 && g.residual != nullptr && m0 + q * 32 + lane < g.M) {
-            // MobileNet-v2 bottleneck `Add` fused behind the linear projection: (conv*scale + offset) + shortcut
-            const float* rs = reinterpret_cast<const float*>(g.residual) + (size_t)(m0 + q * 32 + lane) * g.N + n0 + c0 + h * 32;
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-              const float4 rr = *reinterpret_cast<const float4*>(rs + i);
-              y[h * 32 + i + 0] = __fadd_rn(y[h * 32 + i + 0], rr.x);
-              y[h * 32 + i + 1] = __fadd_rn(y[h * 32 + i + 1], rr.y);
-              y[h * 32 + i + 2] = __fadd_rn(y[h * 32 + i + 2], rr.z);
-              y[h * 32 + i + 3] = __fadd_rn(y[h * 32 + i + 3], rr.w);
-            }
-          }
-        }
-        // staging buffer (chunk_no & 1) was last used two chunks ago: its TMA store must have read it
-        if (chunk_no >= 2) {
-          if (lane == 0) bulk_wait_read<1>();
-          __syncwarp();
-        }
-        const uint32_t sb = smem_u32(my_stage + (size_t)(chunk_no & 1) * 4096 + (size_t)lane * 128);
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          uint4 pk;
-          if (TF32) {
-            pk.x = __float_as_uint(y[c * 4 + 0]);
-            pk.y = __float_as_uint(y[c * 4 + 1]);
-            pk.z = __float_as_uint(y[c * 4 + 2]);
-            pk.w = __float_as_uint(y[c * 4 + 3]);
-          } else {
-            __nv_bfloat162 p0 = __floats2bfloat162_rn(y[c * 8 + 0], y[c * 8 + 1]), p1 = __floats2bfloat162_rn(y[c * 8 + 2], y[c * 8 + 3]);
-            __nv_bfloat162 p2 = __floats2bfloat162_rn(y[c * 8 + 4], y[c * 8 + 5]), p3 = __floats2bfloat162_rn(y[c * 8 + 6], y[c * 8 + 7]);
-            pk.x = *reinterpret_cast<uint32_t*>(&p0);
-            pk.y = *reinterpret_cast<uint32_t*>(&p1);
-            pk.z = *reinterpret_cast<uint32_t*>(&p2);
-            pk.w = *reinterpret_cast<uint32_t*>(&p3);
-          }
-          sts128(sb + (uint32_t)((c ^ (lane & 7)) << 4), pk);  // 128B swizzle: chunk ^= row % 8
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (elect_one()) {
-          tma_store_2d(&map_out, smem_u32(my_stage + (size_t)(chunk_no & 1) * 4096), n0 + c0, m0 + q * 32);
-          bulk_commit();
-        }
-        ++chunk_no;
-      }
-      // every TMEM read of this tile has completed: hand the accumulator set back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&acc_empty[buf]));
-    }
-    if (lane == 0) bulk_wait_read<0>();
-  } else if (X3) {
-    const int tt = threadIdx.x - 192;
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      for (int kb = 0; kb < g.k_blocks; ++kb, ++it) {
-        const int s = it % g.stages;
-        const uint32_t ph = (it / g.stages) & 1;
-        mbar_wait(smem_u32(&full[s]), ph);
-        const uint32_t a = smem_u32(smem + (size_t)s * stage_bytes);
-        const uint32_t lo = a + A_TILE_BYTES;
-#pragma unroll 4
-        for (int i = tt; i < A_TILE_BYTES / 16; i += 128) {
-          uint4 x = lds128u(a + i * 16), h, l;
-          h.x = x.x & 0xFFFFE000u;
-          h.y = x.y & 0xFFFFE000u;
-          h.z = x.z & 0xFFFFE000u;
-          h.w = x.w & 0xFFFFE000u;
-          l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x))) & 0xFFFFE000u;
-          l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y))) & 0xFFFFE000u;
-          l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z))) & 0xFFFFE000u;
-          l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w))) & 0xFFFFE000u;
-          // hi stays as loaded (the tensor core truncates fp32 inputs to tf32 itself)
-          sts128(lo + i * 16, l);
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&conv[s]));
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
-}
 
 // -------------------------------------------------------------------------------------- host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -816,27 +400,6 @@ bool make_map(CUtensorMap* map, const void* base, int elem_bytes, int rows, int 
   if (r != CUDA_SUCCESS) {
     *err = "cuTensorMapEncodeTiled failed with code " + std::to_string((int)r) + " (rows " + std::to_string(rows) +
            ", k " + std::to_string(k) + ", box_rows " + std::to_string(box_rows) + ")";
-    return false;
-  }
-  return true;
-}
-
-// output matrix [rows][n] (fp32 or bf16) -> tensor map with a (128 B x 32 rows) box, 128B swizzle
-bool make_out_map(CUtensorMap* map, void* base, int elem_bytes, int rows, int n, std::string* err) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) {
-    *err = "cuTensorMapEncodeTiled is not available from the driver";
-    return false;
-  }
-  cuuint64_t dims[2] = {(cuuint64_t)n, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)n * elem_bytes};
-  cuuint32_t box[2] = {(cuuint32_t)(ROW_BYTES / elem_bytes), 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims,
-                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    *err = "cuTensorMapEncodeTiled (output) failed with code " + std::to_string((int)r);
     return false;
   }
   return true;
@@ -880,32 +443,14 @@ int num_sms_hint() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
-int pick_block_n(int n_pad, int k_steps, int mode) {
-  if (n_pad <= 128) return n_pad;  // multiples of 16 up to 128: one N tile
-  // A tcgen05.mma of the TF32 kinds covers only K = 8 and costs ~100 cycles whatever its width (profiles/
-  // r02_pipeline_trace.md), so wide instructions are the cheap ones: short accumulation chains (one main + one correction
-  // accumulator: 2 x 256 columns of tensor memory) take the widest tile (multiple of 16, <= 256) that divides N.
-  // Measured (profiles/r02_final_summary.md): SM time of the 19x19 expansions -20 %, their latency +20 %, throughput with
-  // six batches in flight unchanged -> opt-in.
-  if (mode == TC_TF32X3 && k_steps <= 16 && getenv("WB_WIDE_N") != nullptr)
-    for (int bn = 256; bn > 128; bn -= 16)
-      if (n_pad % bn == 0) return bn;
-  int best = 16;
-  for (int bn = 128; bn >= 16; bn -= 16)
-    if (n_pad % bn == 0) {
-      best = bn;  // largest UMMA width (multiple of 16) that tiles N exactly
-      break;
-    }
-  // N = 144 (MobileNet-v2 24 -> 144 expansions) only tiles as 3 x 48: three CTAs per row block re-reading the A tile
-  // and running three prologues/epilogues.  One UMMA may be up to 256 columns wide: use a single N tile instead.
-  if (best < 64 && n_pad <= 256) return n_pad;
-  return best;
-}
+// N tile of the GEMM: the narrowest of the compiled wgmma widths (32 / 64 / 128) that covers N, else 128 with a ragged
+// last tile (TMA zero-fills the weight rows beyond n_pad; the epilogue skips the columns beyond N).
+int pick_block_n(int n_pad) { return n_pad <= 32 ? 32 : (n_pad <= 64 ? 64 : 128); }
 
 }  // namespace
 
@@ -929,7 +474,7 @@ int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb
     const float* src = host_data + tensors[L.w_tensor].offset;  // [K][NP]
     w.k = K;
     w.n_pad = NP;
-    w.block_n = pick_block_n(NP, (K + 7) / 8, mode);
+    w.block_n = pick_block_n(NP);
     const int elem = mode == TC_BF16 ? 2 : 4;
     const size_t bytes = (size_t)NP * K * elem;
     std::vector<uint8_t> hi(bytes), lo(mode == TC_TF32X3 ? bytes : 0);
@@ -1027,18 +572,16 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
   g.ncp1 = num_classes_p1;
   g.hw = L.out_h * L.out_w;
   const int x3 = mode == TC_TF32X3 ? 2 : 1;
-  g.n_main = 1;
-  g.ta_stages = 0;
-  int stage_bytes = A_TILE_BYTES * x3 + g.block_n * ROW_BYTES * x3;
+  const int stage_bytes = (A_TILE_BYTES + g.block_n * ROW_BYTES) * x3;
   dim3 grid((g.M + g.rows_per_tile - 1) / g.rows_per_tile, (g.n_pad + g.block_n - 1) / g.block_n);
-  // latency-bound shapes: split K so that about one wave of CTAs exists (deterministic two-pass reduce)
+  // latency-bound shapes: split K so that about one wave of CTAs exists (deterministic cluster reduce)
   g.splits = 1;
   g.kb_per = g.k_blocks;
   g.partial = partial;
   const long tiles = (long)grid.x * grid.y;
-  // A k-block costs ~850 cycles (profiles/r02_pipeline_trace.md) while the cluster barriers + DSMEM reduction of a split
-  // cost ~5-9 k cycles: splitting only pays for long accumulation chains, and every split keeps >= 8 k-blocks.
-  if (tiles < 74 && g.k_blocks >= 16 && getenv("WB_NO_SPLITK") == nullptr) {
+  // the cluster barriers + DSMEM reduction of a split cost several k-blocks' worth of time: splitting only pays for
+  // long accumulation chains, and every split keeps >= 8 k-blocks
+  if (tiles < num_sms_hint() / 2 && g.k_blocks >= 16 && getenv("WB_NO_SPLITK") == nullptr) {
     int want = std::max(1, (int)(num_sms_hint() / tiles));  // at most one wave: tiles * splits <= SMs (a second wave of a
                                                             // few CTAs doubles the kernel's duration)
     int splits = std::min(std::min(want, g.k_blocks / 8), 8);  // 8 = portable thread-block cluster size
@@ -1048,82 +591,13 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
       grid.z = g.splits;
     }
   }
-  // many-tile layers: persistent kernel (double-buffered TMEM, TMA-store epilogue)
-  const int cw = mode == TC_BF16 ? 64 : 32;
-  static int num_sms = 0;
-  if (num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (num_sms <= 0) num_sms = 148;
-  }
-  // N = 144 (one 144-wide UMMA tile: 2 x 2 x 144 TMEM columns do not fit twice) runs persistent as 128 + a ragged 16:
-  // the weight rows beyond N are zero-filled by TMA and the missing output columns are skipped / clipped.
-  if (mode == TC_TF32X3 && !g.is_head && !g.conv && g.block_n > 128 && g.block_n == g.n_pad && g.N % 4 == 0 &&
-      (long)grid.x * ((g.n_pad + 127) / 128) >= num_sms && getenv("WB_NO_RAGGED_N") == nullptr) {
-    g.block_n = 128;
-    grid.y = (g.n_pad + 127) / 128;
-    stage_bytes = A_TILE_BYTES * x3 + g.block_n * ROW_BYTES * x3;
-  }
-  const long ptiles = (long)grid.x * grid.y;
-  bool persist = !g.is_head && !g.conv && g.splits == 1 && ptiles >= num_sms && (g.N == g.n_pad || (g.N % 4 == 0 && mode != TC_BF16)) && g.block_n % cw == 0 &&
-                 (g.n_pad % g.block_n == 0 || mode == TC_TF32X3) && getenv("WB_NO_PERSIST") == nullptr;
-  if (persist && mode == TC_TF32X3) {
-    g.n_main = std::max(1, std::min(3, 512 / (2 * g.block_n) - 1));
-    if (g.k_blocks * (ROW_BYTES / UMMA_K_BYTES) <= 32) g.n_main = 1;  // short chains: no measurable bias
-    if (2 * (g.n_main + 1) * g.block_n > 512) persist = false;
-  }
-  if (persist && mode != TC_TF32X3 && 2 * g.block_n > 512) persist = false;
-  int stages;
-  if (persist) {
-    stages = (224 * 1024 - STAGING_BYTES * (mode == TC_TF32X3 ? 2 : 1) - 8 * (int)(grid.y * g.block_n)) / stage_bytes;
-    if (stages > 8) stages = 8;
-    if (stages < 2) persist = false;
-  }
-  if (!persist) {
-    if (mode == TC_TF32X3) {
-      g.n_main = std::max(1, std::min(3, 512 / g.block_n - 1));
-      // short accumulation chains (split-K tails, small K) carry no measurable truncation bias: one main
-      // accumulator halves the TMEM footprint, so two such CTAs can share an SM
-      if (g.kb_per * (ROW_BYTES / UMMA_K_BYTES) <= 16) g.n_main = 1;
-    }
-    const char* ta_env = getenv("WB_TMEM_A");
-    if (mode == TC_TF32X3 && !g.conv && !(ta_env != nullptr && ta_env[0] == '0')) {
-      // A operand of the 3xTF32 MMAs from tensor memory (default since round 2: +3.3 % on the v2 step; WB_TMEM_A=0
-      // switches back to the shared-memory hi / lo tiles)
-      // A ring in tensor memory; chains of <= 32 steps per main accumulator
-      const int steps = g.kb_per * (ROW_BYTES / UMMA_K_BYTES);
-      const int nm = steps <= 16 ? 1 : (steps <= 24 ? 2 : 3);  // chains > 24 MMAs rotate over 3 accumulators (layer-by-layer bar)
-      const int ta = std::min(4, (512 - (nm + 1) * g.block_n) / 64);
-      if (ta >= 2) {
-        g.n_main = nm;
-        g.ta_stages = ta;
-        stage_bytes = A_TILE_BYTES + 2 * g.block_n * ROW_BYTES;
-      }
-    }
-    stages = (200 * 1024) / stage_bytes;
-    if (stages > 6) stages = 6;
-    if (stages > g.kb_per) stages = g.kb_per;
-  }
-  // Two CTAs per SM for short, epilogue-dominated layers (WB_GEMM_2CTA=1): <= 2 k-blocks, the stage ring cut down so
-  // that ring + staging tile fit in ~110 KB, <= 256 TMEM columns.
-  bool two = false;
-  if (!persist && mode == TC_TF32X3 && g.ta_stages == 0 && g.splits == 1 && getenv("WB_GEMM_2CTA") != nullptr) {
-    const int staging = BLOCK_M * (g.block_n + 4) * 4;
-    int st2 = std::min(stages, std::max(1, (108 * 1024) / stage_bytes));
-    if (g.kb_per <= 4 && std::max(st2 * stage_bytes, staging) <= 108 * 1024 && (g.n_main + 1) * g.block_n <= 256) {
-      stages = st2;
-      two = true;
-    }
-  }
+  int stages = std::min(6, (200 * 1024) / stage_bytes);
+  if (stages > g.kb_per) stages = g.kb_per;
   if (stages < 1) stages = 1;
   g.stages = stages;
-  g.ring_bytes = stages * stage_bytes;
-  if (!persist) {
-    const int staging = BLOCK_M * (g.block_n + 4) * 4;  // epilogue staging tile re-uses the stage ring
-    g.ring_bytes = ((std::max(g.ring_bytes, staging) + 1023) / 1024) * 1024;
-  }
-  const size_t smem = (size_t)g.ring_bytes + (persist ? STAGING_BYTES * (mode == TC_TF32X3 ? 2 : 1) + 8 * (size_t)(grid.y * g.block_n) + 32 : 0) + 1024 /*align*/ + 8 * (3 * stages + 4) + 16 + 64 /*TA barriers*/;
+  const int staging = BLOCK_M * (g.block_n + 4) * 4;  // epilogue staging tile re-uses the stage ring
+  g.ring_bytes = ((std::max(stages * stage_bytes, staging) + 1023) / 1024) * 1024;
+  const size_t smem = (size_t)g.ring_bytes + 1024 /*align*/ + 16 * stages;
   alignas(64) CUtensorMap map_a;
   if (g.conv) {
     const int imgs = BLOCK_M / (int)(L.out_h * L.out_w);
@@ -1139,24 +613,18 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
     return 1;
   }
   CUtensorMap map_b, map_b_lo;
-  if (g.block_n == w.block_n) {
-    memcpy(&map_b, w.tmap_b, sizeof(map_b));
-    memcpy(&map_b_lo, w.tmap_b_lo, sizeof(map_b_lo));
-  } else {
-    if (!make_map(&map_b, w.w, elem, w.n_pad, w.k, g.block_n, err)) return 1;
-    if (mode == TC_TF32X3) {
-      if (!make_map(&map_b_lo, w.w_lo, elem, w.n_pad, w.k, g.block_n, err)) return 1;
-    } else {
-      map_b_lo = map_b;
-    }
-  }
-  static PerDeviceFlag attr_done[6];
-  cudaError_t e = cudaSuccess;
+  memcpy(&map_b, w.tmap_b, sizeof(map_b));
+  memcpy(&map_b_lo, w.tmap_b_lo, sizeof(map_b_lo));
   // split-K launches: the `splits` CTAs of a tile are one thread-block cluster (1, 1, splits)
-  auto launch = [&](auto kern, int threads) {
+  auto launch = [&](auto kern, PerDeviceFlag& attr_done) {
+    if (!attr_done.get()) {
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+      if (e != cudaSuccess) return e;
+      attr_done.set();
+    }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
-    cfg.blockDim = dim3(threads);
+    cfg.blockDim = dim3(GEMM_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = lc.stream;
     cudaLaunchAttribute at[1];
@@ -1168,60 +636,18 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
     cfg.numAttrs = g.splits > 1 ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, map_a, map_b, map_b_lo, g);
   };
-  if (persist) {
-    CUtensorMap map_out;
-    if (!make_out_map(&map_out, out, elem, g.M, g.N, err)) return 1;
-    const int idx = 3 + (mode == TC_BF16 ? 0 : (mode == TC_TF32X1 ? 1 : 2));
-    static int persist_ctas = 0;
-    if (persist_ctas == 0) {
-      const char* e = getenv("WB_PERSIST_CTAS");
-      persist_ctas = e ? atoi(e) : num_sms;
-      if (persist_ctas <= 0 || persist_ctas > num_sms) persist_ctas = num_sms;
-    }
-    dim3 pgrid((unsigned)std::min<long>(ptiles, persist_ctas));
-    if (mode == TC_BF16) {
-      if (!attr_done[idx].get()) e = cudaFuncSetAttribute(k_gemm_tc_persist<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      k_gemm_tc_persist<0><<<pgrid, 192, smem, lc.stream>>>(map_a, map_b, map_b_lo, map_out, g);
-    } else if (mode == TC_TF32X1) {
-      if (!attr_done[idx].get()) e = cudaFuncSetAttribute(k_gemm_tc_persist<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      k_gemm_tc_persist<1><<<pgrid, 192, smem, lc.stream>>>(map_a, map_b, map_b_lo, map_out, g);
-    } else {
-      if (!attr_done[idx].get()) e = cudaFuncSetAttribute(k_gemm_tc_persist<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      k_gemm_tc_persist<2><<<pgrid, 448, smem, lc.stream>>>(map_a, map_b, map_b_lo, map_out, g);
-    }
-    attr_done[idx].set();
-  } else if (mode == TC_BF16) {
-    if (!attr_done[0].get()) {
-      e = cudaFuncSetAttribute(k_gemm_tc<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-      attr_done[0].set();
-    }
-    if (e == cudaSuccess) e = launch(k_gemm_tc<0>, 192);
+  static PerDeviceFlag attr_done[3][3];
+  const int bi = g.block_n == 32 ? 0 : (g.block_n == 64 ? 1 : 2);
+  cudaError_t e;
+  if (mode == TC_BF16) {
+    e = bi == 0 ? launch(k_gemm_tc<0, 32>, attr_done[0][0])
+                : (bi == 1 ? launch(k_gemm_tc<0, 64>, attr_done[0][1]) : launch(k_gemm_tc<0, 128>, attr_done[0][2]));
   } else if (mode == TC_TF32X1) {
-    if (!attr_done[1].get()) {
-      e = cudaFuncSetAttribute(k_gemm_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-      attr_done[1].set();
-    }
-    if (e == cudaSuccess) e = launch(k_gemm_tc<1>, 192);
-  } else if (g.ta_stages > 0) {
-    static PerDeviceFlag ta_attr_done;
-    if (!ta_attr_done.get()) {
-      e = cudaFuncSetAttribute(k_gemm_tc<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-      ta_attr_done.set();
-    }
-    if (e == cudaSuccess) e = launch(k_gemm_tc<2, true>, 320);
-  } else if (two) {
-    static PerDeviceFlag two_attr_done;
-    if (!two_attr_done.get()) {
-      e = cudaFuncSetAttribute(k_gemm_tc<2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024);
-      two_attr_done.set();
-    }
-    if (e == cudaSuccess) e = launch(k_gemm_tc<2, false, true>, 320);
+    e = bi == 0 ? launch(k_gemm_tc<1, 32>, attr_done[1][0])
+                : (bi == 1 ? launch(k_gemm_tc<1, 64>, attr_done[1][1]) : launch(k_gemm_tc<1, 128>, attr_done[1][2]));
   } else {
-    if (!attr_done[2].get()) {
-      e = cudaFuncSetAttribute(k_gemm_tc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-      attr_done[2].set();
-    }
-    if (e == cudaSuccess) e = launch(k_gemm_tc<2>, 320);
+    e = bi == 0 ? launch(k_gemm_tc<2, 32>, attr_done[2][0])
+                : (bi == 1 ? launch(k_gemm_tc<2, 64>, attr_done[2][1]) : launch(k_gemm_tc<2, 128>, attr_done[2][2]));
   }
   if (e != cudaSuccess) {
     *err = std::string("tensor-core GEMM launch: ") + cudaGetErrorString(e);
@@ -1231,8 +657,3 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
   return 0;
 }
 
-#ifdef WB_TRACE
-extern "C" int wb_trace_read_gemm(long long* dst) {
-  return (int)cudaMemcpyFromSymbol(dst, wb_trace_buf, sizeof(wb_trace_buf));
-}
-#endif

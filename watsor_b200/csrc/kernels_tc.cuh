@@ -1,4 +1,4 @@
-// kernels_tc.cuh -- tensor-core (tcgen05 + TMA + TMEM) GEMM path for the dense 1x1 convolutions.
+// kernels_tc.cuh -- tensor-core (wgmma + TMA) GEMM path for the dense 1x1 convolutions.
 #pragma once
 #include <string>
 #include <vector>
@@ -40,12 +40,3 @@ bool fused_dwpw_supported(const TcWeights& tw, int pw_layer_index, const wb_laye
 int fused_launch_dwpw(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_index, int n, const wb_layer& dw,
                       const wb_layer& pw, const void* in, const float* dw_w, const float* dw_scale, const float* dw_offset,
                       const float* scale, const float* offset, void* out, std::string* err);
-
-// MobileNet-v2 inverted residual block (1x1 expand -> depthwise 3x3 -> linear 1x1 projection [-> Add]) as one kernel
-// (kernels_fused.cu: k_irb_x3); TF32X3 only.  `add` may be NULL.
-bool fused_irb_supported(const TcWeights& tw, int pw_layer_index, const wb_layer& ex, const wb_layer& dw, const wb_layer& pw,
-                         const wb_layer* add, int n);
-int fused_launch_irb(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_index, int n, const wb_layer& ex,
-                     const wb_layer& dw, const wb_layer& pw, bool with_add, const void* in, const float* ex_w,
-                     const float* ex_scale, const float* ex_offset, const float* dw_w, const float* dw_scale,
-                     const float* dw_offset, const float* scale, const float* offset, void* out, std::string* err);

@@ -1,6 +1,6 @@
-// tc_common.cuh -- inline PTX wrappers shared by the tcgen05 kernels (kernels_tc.cu, kernels_fused.cu):
-// mbarrier, TMA (cp.async.bulk.tensor load / store), TMEM allocation, tcgen05.mma / commit / ld, and the
-// shared-memory / instruction descriptors (bit layouts as in cute/arch/mma_sm100_desc.hpp).  sm_100a only.
+// tc_common.cuh -- inline PTX wrappers shared by the tensor-core kernels (kernels_tc.cu, kernels_fused.cu):
+// mbarrier, TMA (cp.async.bulk.tensor load / store), wgmma (warpgroup MMA with the accumulator in registers) and the
+// shared-memory matrix descriptor (bit layout as in cute/arch/mma_sm90_desc.hpp).  sm_90a.
 #pragma once
 #include <cuda.h>
 
@@ -35,8 +35,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
   asm volatile(
@@ -44,139 +42,19 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
 // One elected lane of a converged warp.  Unlike `lane == 0`, ptxas knows the guarded region runs in a single
-// thread, so the tcgen05.mma operands move to uniform registers without the per-instruction
-// ELECT / R2UR.BROADCAST / BRA.U.ANY uniformisation loop (measured: ~100 -> ~30 cycles per issued MMA).
+// thread, so the TMA operands move to uniform registers without a per-instruction uniformisation loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
   return pred != 0;
 }
 
-template <bool TF32>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (TF32)
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  else
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// A operand from tensor memory (lane = row of the 128-row tile, one TF32 per 32-bit column), B from shared memory.
-__device__ __forceinline__ void umma_tf32_ta(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 consecutive columns of this thread's TMEM lane (the mirror image of tmem_ld16's shape)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 16 accumulator columns of this thread's row, summed over the TF32X3 partial accumulators in the fixed
-// order ((main0 + main1) + main2) + corr.  All tcgen05.ld are issued before the single wait::ld, so the
-// TMEM round trips overlap instead of serialising.
-template <bool X3>
-__device__ __forceinline__ void load_acc16(uint32_t taddr, int block_n, int n_main, int used, uint32_t* v) {
-  if (!X3) {
-    tmem_ld16(taddr, v);
-    tmem_ld_wait();
-    return;
-  }
-  uint32_t u1[16], u2[16], uc[16];
-  tmem_ld16(taddr, v);
-  if (used > 1) tmem_ld16(taddr + (uint32_t)block_n, u1);
-  if (used > 2) tmem_ld16(taddr + (uint32_t)(2 * block_n), u2);
-  tmem_ld16(taddr + (uint32_t)(n_main * block_n), uc);
-  tmem_ld_wait();
-  if (used > 1) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__fadd_rn(__uint_as_float(v[i]), __uint_as_float(u1[i])));
-  }
-  if (used > 2) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__fadd_rn(__uint_as_float(v[i]), __uint_as_float(u2[i])));
-  }
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__fadd_rn(__uint_as_float(v[i]), __uint_as_float(uc[i])));
-}
-
-// 32 accumulator columns at once.  With a single main accumulator (or none to add) all four / two tcgen05.ld
-// go out before one wait::ld - the epilogue warps are latency bound (profiles/r01_pipeline_trace.md), and two
-// dependent ld -> wait round trips per 32 columns were a third of their time.  Same RN additions as load_acc16.
-template <bool X3>
-__device__ __forceinline__ void load_acc32(uint32_t taddr, int block_n, int n_main, int used, uint32_t* v) {
-  if (!X3) {
-    tmem_ld16(taddr, v);
-    tmem_ld16(taddr + 16u, v + 16);
-    tmem_ld_wait();
-    return;
-  }
-  if (used > 1) {
-    load_acc16<true>(taddr, block_n, n_main, used, v);
-    load_acc16<true>(taddr + 16u, block_n, n_main, used, v + 16);
-    return;
-  }
-  uint32_t uc[32];
-  tmem_ld16(taddr, v);
-  tmem_ld16(taddr + 16u, v + 16);
-  tmem_ld16(taddr + (uint32_t)(n_main * block_n), uc);
-  tmem_ld16(taddr + (uint32_t)(n_main * block_n) + 16u, uc + 16);
-  tmem_ld_wait();
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__fadd_rn(__uint_as_float(v[i]), __uint_as_float(uc[i])));
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout_type=2 (SW128) [61,64).
-// Rows are 128 B apart, 8-row swizzle atoms 1024 B apart (SBO).
 // Explicit shared-window accesses: the carve-up of the dynamic buffer goes through integer alignment, after
 // which nvcc no longer proves the address space and would emit generic LD.E/ST.E in the hottest loops.
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
-// Read-only tables (written once before the prologue __syncthreads, never again): NOT volatile, so the compiler may
-// hoist / pipeline these loads across the FFMA chains that consume them.  Never use for data guarded by an mbarrier.
-__device__ __forceinline__ float4 lds128_ro(uint32_t addr) {
-  float4 v;
-  asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
   return v;
 }
 __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
@@ -189,59 +67,139 @@ __device__ __forceinline__ uint4 lds128u(uint32_t addr) {
   return v;
 }
 
-// Pipeline tracing (diagnostic builds only: make EXTRA=-DWB_TRACE; see tools/trace_pipeline.py).  CTA 0 stamps
-// clock64() per role and iteration into a per-translation-unit buffer that wb_trace_read_*() copies out.
-#ifdef WB_TRACE
-#define WB_TRACE_SLOTS 12
-#define WB_TRACE_ITERS 64
-static __device__ long long wb_trace_buf[WB_TRACE_SLOTS * WB_TRACE_ITERS];
-#define WB_STAMP(kind, it)                                                                  \
-  do {                                                                                      \
-    if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (it) < WB_TRACE_ITERS)     \
-      wb_trace_buf[(kind) * WB_TRACE_ITERS + (it)] = clock64();                             \
-  } while (0)
-#else
-#define WB_STAMP(kind, it) \
-  do {                     \
-  } while (0)
-#endif
-
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (cute::GMMA::DescriptorSm90 bit layout):
+// start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major) | SBO>>4 [32,46) | layout_type=1 (SW128) [62,64).
+// Rows are 128 B apart, 8-row swizzle atoms 1024 B apart (SBO).  A k-step inside the 128-byte row advances the start
+// address by its byte offset; tiles start on 1024-byte boundaries, so the base offset field stays 0.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A/B format, K-major both, N>>3, M>>4
-__host__ __device__ inline uint32_t make_idesc(bool tf32, int m, int n) {
-  uint32_t d = 0;
-  d |= 1u << 4;                        // c_format = F32
-  d |= (tf32 ? 2u : 1u) << 7;          // a_format  (BF16 = 1, TF32 = 2)
-  d |= (tf32 ? 2u : 1u) << 10;         // b_format
-  d |= (uint32_t)(n >> 3) << 17;
-  d |= (uint32_t)(m >> 4) << 24;
-  return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x N] (+)= A[64 x K] * B[N x K]^T, both operands K-major in shared memory, fp32 accumulators in registers.
+// TF32: k = 8 per instruction; BF16: k = 16.  Either way one instruction covers 32 bytes of a 128-byte row.
+// Accumulator i of a thread holds row 16 * (warp % 4) + lane / 4 + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (lane % 4) + i % 2.
+// scale_d = 0 overwrites D instead of adding to it.
+template <bool TF32, int N> struct Wgmma;
+template <> struct Wgmma<true, 32> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<true, 64> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<true, 128> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<false, 32> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<false, 64> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<false, 128> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+
+// One 128-byte k-block (32 fp32 / 64 bf16 along K) of a warpgroup's 64 x N tile: four k-steps.  X3 (3xTF32) issues
+// the small correction products lo(A)*hi(B) and hi(A)*lo(B) of all four k-steps first and the hi(A)*hi(B) products
+// last: the tensor core's accumulation rounds toward zero, and this order leaves four such roundings at the magnitude
+// of the k-block's partial sum instead of twelve.  The GEMM and the fused depthwise kernel both issue their MMAs
+// through here, so equal inputs give bit-equal outputs.
+template <bool TF32, bool X3, int N>
+__device__ __forceinline__ void wg_mma_kblock(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                              uint32_t scale_first) {
+  if (X3) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t koff = (uint32_t)(k * 32);
+      Wgmma<TF32, N>::mma(d, make_sw128_desc(a_lo + koff), make_sw128_desc(b_hi + koff), k == 0 ? scale_first : 1u);
+      Wgmma<TF32, N>::mma(d, make_sw128_desc(a_hi + koff), make_sw128_desc(b_lo + koff), 1u);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t koff = (uint32_t)(k * 32);
+    Wgmma<TF32, N>::mma(d, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), (X3 || k > 0) ? 1u : scale_first);
+  }
+}
+
+// 3xTF32 k-block into the running sum: the k-block's partial sum lands in `part` (overwritten), then is added to
+// `acc` with round-to-nearest, so the tensor core's truncating accumulation never spans more than one k-block.
+template <int N>
+__device__ __forceinline__ void wg_x3_kblock_sum(float* acc, float* part, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+                                                 uint32_t b_lo) {
+  wgmma_fence();
+  wg_mma_kblock<true, true, N>(part, a_hi, a_lo, b_hi, b_lo, 0u);
+  wgmma_commit();
+  wgmma_wait_all();
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = __fadd_rn(acc[i], part[i]);
+}
+
+// Split one 16-byte chunk of fp32 in place into hi = a & 0xffffe000 (written back) and lo = (a - hi) & 0xffffe000:
+// both exactly representable in TF32, so the tensor core's own input conversion never matters.
+__device__ __forceinline__ void split_tf32(uint32_t hi_addr, uint32_t lo_addr) {
+  const uint4 x = lds128u(hi_addr);
+  uint4 h, l;
+  h.x = x.x & 0xFFFFE000u;
+  h.y = x.y & 0xFFFFE000u;
+  h.z = x.z & 0xFFFFE000u;
+  h.w = x.w & 0xFFFFE000u;
+  l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x))) & 0xFFFFE000u;
+  l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y))) & 0xFFFFE000u;
+  l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z))) & 0xFFFFE000u;
+  l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w))) & 0xFFFFE000u;
+  sts128(hi_addr, h);
+  sts128(lo_addr, l);
 }
 
 constexpr int BLOCK_M = 128;
 constexpr int ROW_BYTES = 128;                     // one swizzle row = 64 bf16 or 32 fp32 along K
 constexpr int A_TILE_BYTES = BLOCK_M * ROW_BYTES;  // 16 KB
-constexpr int UMMA_K_BYTES = 32;
-
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src),
-               "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
 
 
 }  // namespace

@@ -165,7 +165,7 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   REQUIRE(blob_bytes >= sizeof(wb_model_header), "model blob too small");
   REQUIRE(max_batch >= 1 && max_batch <= 4096, "max_batch out of range");
   REQUIRE(precision >= 0 && precision <= 3,
-          "precision must be 0 (fp32 CUDA cores), 1 (bf16 tcgen05), 2 (fp32 via 3xTF32 tcgen05) or 3 (1xTF32, diagnostic)");
+          "precision must be 0 (fp32 CUDA cores), 1 (bf16 wgmma), 2 (fp32 via 3xTF32 wgmma) or 3 (1xTF32, diagnostic)");
   CK(cudaSetDevice(device));
   struct CtxFree {
     void operator()(wb_ctx* p) const { wb_destroy(p); }
@@ -177,7 +177,7 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   c->precision = precision;
   if (const char* g = getenv("WB_NO_GRAPH")) c->use_graph = !(g[0] == '1');
   CK(cudaGetDeviceProperties(&c->prop, device));
-  REQUIRE(c->prop.major == 10, std::string("libwatsor_b200 is built for sm_100a only; device is ") +
+  REQUIRE(c->prop.major == 9 && c->prop.minor == 0, std::string("libwatsor_b200 is built for sm_90a only; device is ") +
                                    c->prop.name + " (sm_" + std::to_string(c->prop.major) +
                                    std::to_string(c->prop.minor) + ")");
   memcpy(&c->hdr, model_blob, sizeof(wb_model_header));
@@ -299,7 +299,7 @@ int wb_destroy(wb_ctx* c) {
 int wb_device_name(wb_ctx* c, char* buf, size_t n) {
   REQUIRE(c && buf && n > 0, "NULL argument");
   snprintf(buf, n, "%s (cuda:%d, sm_%d%d, %s)", c->prop.name, c->device, c->prop.major, c->prop.minor,
-           c->precision == 1 ? "bf16 tcgen05" : (c->precision == 2 ? "fp32 3xTF32 tcgen05" : (c->precision == 3 ? "tf32 tcgen05" : "fp32")));
+           c->precision == 1 ? "bf16 wgmma" : (c->precision == 2 ? "fp32 3xTF32 wgmma" : (c->precision == 3 ? "tf32 wgmma" : "fp32")));
   return 0;
 }
 
@@ -411,25 +411,6 @@ int wb_unregister_host(wb_ctx* c, void* ptr) {
 
 }  // extern "C"
 
-// Number of layers starting at `li` that run as one fused inverted-residual-block kernel (0 = none, 3 = expand +
-// depthwise + projection, 4 = ... + Add), all inside [li, end).
-static int irb_span(wb_ctx* c, int li, int end, int n) {
-  if (c->precision != 2 || li + 2 >= end) return 0;
-  const wb_layer& E = c->layers[li];
-  const wb_layer& D = c->layers[li + 1];
-  const wb_layer& P = c->layers[li + 2];
-  if (E.op != WB_OP_PW || E.act != WB_ACT_RELU6 || D.op != WB_OP_DW || P.op != WB_OP_PW || P.act != WB_ACT_NONE) return 0;
-  if (li + 3 < end && c->layers[li + 3].op == WB_OP_ADD &&
-      (c->layers[li + 3].in_off == P.out_off || c->layers[li + 3].in2_off == P.out_off) &&
-      fused_irb_supported(c->tc, li + 2, E, D, P, &c->layers[li + 3], n))
-    return 4;
-  // without the Add the projection output must not feed a later Add as a fused pair elsewhere: plain 3-layer block
-  if (li + 3 < (int)c->layers.size() && c->layers[li + 3].op == WB_OP_ADD &&
-      (c->layers[li + 3].in_off == P.out_off || c->layers[li + 3].in2_off == P.out_off))
-    return 0;  // a residual block whose Add is outside the requested range: run it unfused
-  return fused_irb_supported(c->tc, li + 2, E, D, P, nullptr, n) ? 3 : 0;
-}
-
 // ---------------------------------------------------------------------------------------------------
 // the layer program.  `pre` != NULL feeds an already pre-processed input (wb_backbone); otherwise the
 // fused stem samples the frames directly.  When `times` is given every launch is bracketed by events.
@@ -483,20 +464,6 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
       case WB_OP_PW:
       case WB_OP_CONV:
       case WB_OP_HEAD:
-        // MobileNet-v2 inverted residual block (expand -> depthwise -> projection [-> Add]) as one kernel
-        if (int span = irb_span(c, (int)li, (int)end, n)) {
-          const wb_layer& D = c->layers[li + 1];
-          const wb_layer& P = c->layers[li + 2];
-          const wb_layer& last = c->layers[li + span - 1];
-          std::string err;
-          if (fused_launch_irb(lc, c->tc, (int)li + 2, n, L, D, P, span == 4, static_cast<const void*>(in), w, sc, of,
-                               c->tensor(D.w_tensor), c->tensor(D.scale_tensor), c->tensor(D.offset_tensor),
-                               c->tensor(P.scale_tensor), c->tensor(P.offset_tensor),
-                               static_cast<void*>(arena + (size_t)last.out_off * n), &err))
-            return fail("block " + std::string(L.name) + ": " + err);
-          li += span - 1;
-          break;
-        }
         if (c->precision != 0 && tc_layer_supported(L)) {
           // MobileNet-v2 bottleneck: a linear projection followed by `Add(shortcut, projection)` runs as one kernel,
           // the shortcut is added in the GEMM epilogue (fp32 modes) and the Add layer is skipped
@@ -883,21 +850,6 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
     // a depthwise layer that the executor fuses into the following 1x1 conv is timed together with it:
     // the pair's time is reported on the 1x1 layer, the depthwise entry reads 0
     int last = li;
-    if (int span = irb_span(c, li, nl, n)) {
-      // a fused inverted residual block: the kernel's time is reported on the expand entry, the others read 0
-      for (int r = 0; r < REPS; ++r) {
-        int rc = run_layers<float>(c, s, st, n, nullptr, li, li + span - 1);
-        if (rc) return rc;
-      }
-      CK(cudaEventRecord(ev[li + 1], st));
-      kinds[li] = (int)c->layers[li].op;
-      for (int k = 1; k < span; ++k) {
-        CK(cudaEventRecord(ev[li + k + 1], st));
-        kinds[li + k] = (int)c->layers[li + k].op;
-      }
-      li += span - 1;
-      continue;
-    }
     if (c->precision == 2 && li + 1 < nl && c->layers[li].op == WB_OP_DW &&
         c->layers[li + 1].in_off == c->layers[li].out_off &&
         fused_dwpw_supported(c->tc, li + 1, c->layers[li], c->layers[li + 1], n))

@@ -1,4 +1,4 @@
-"""B200ObjectDetector -- the detector plugin for NVIDIA B200 (sm_100a).
+"""B200ObjectDetector -- the detector plugin for NVIDIA H100 (sm_90a).
 
 Implements the duck-typed Detector protocol every reference back-end provides
 (watsor/detection/tensorflow_cpu.py:8-92, tensorrt_gpu.py:15-91):
@@ -6,7 +6,7 @@ Implements the duck-typed Detector protocol every reference back-end provides
     __init__(model_path[, device]);  context manager;  `device_name`;
     detect(image_shape, image_np, detections) -> inference time in ms
 
-and adds the batched form the B200 needs to be busy: one call per tick for all cameras
+and adds the batched form the GPU needs to be busy: one call per tick for all cameras
 (`detect_batch`, `submit`/`collect`), with the confidence / area / mask-zone predicates of
 watsor/filter fused behind the NMS.  Model selection follows tensorflow_cpu.py:50-53:
 `frozen_inference_graph.pb`, else `cpu.pb`, in `model_path` (a pre-compiled `b200.wb200`

@@ -7,10 +7,10 @@ detector.py:111-112), back-end constructed inside the child so that CUDA state i
 
 Differences from watsor/detection/detector.py:102-112: the worker drains every payload that is
 already waiting (at most one per camera: `BalancedQueue` holds a 1-slot semaphore per camera,
-sync.py:156-166) and hands them to the B200 as ONE batch; the shared-memory frames are page-locked once
+sync.py:156-166) and hands them to the GPU as ONE batch; the shared-memory frames are page-locked once
 (`wb_register_host`) and the ticks are pipelined over up to four library slots (`submit` / `collect`,
 `WATSOR_B200_PIPELINE_DEPTH`): while the GPU runs ticks k-2 .. k the worker writes back tick k-3 and drains the
-queue for tick k+1 -- a B200 needs several 8-frame batches in flight to be busy.  A frame's latch still advances
+queue for tick k+1 -- the GPU needs several 8-frame batches in flight to be busy.  A frame's latch still advances
 exactly once, after its Detection rows are in its header (also when the back-end raises).
 """
 from collections import deque
@@ -37,7 +37,7 @@ def has_model(model_path):
 
 
 def create_object_detectors(delegate_class, stop_event, log_queue, frame_queue, frame_buffers, model_path, kwargs=None):
-    """One batched detector worker per visible B200 (detector.py:12-55).  There is deliberately no
+    """One batched detector worker per visible H100 (detector.py:12-55).  There is deliberately no
     CPU fallback here: without a GPU or a model the assertion below fires, as in the reference."""
     detectors = []
     kwargs = {} if kwargs is None else kwargs
@@ -48,7 +48,7 @@ def create_object_detectors(delegate_class, stop_event, log_queue, frame_queue, 
                                             kwargs={**kwargs, 'detector_class': clazz,
                                                     'detector_args': (model_path, device)}))
     assert len(detectors) > 0, "Failed to create an object detector. " \
-                               "Make sure a B200 is visible and model files are provided."
+                               "Make sure an H100 is visible and model files are provided."
     return detectors
 
 

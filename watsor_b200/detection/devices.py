@@ -1,4 +1,4 @@
-"""Device discovery for the B200 back-end: the counterpart of `cuda_gpus()` in
+"""Device discovery for the H100 back-end: the counterpart of `cuda_gpus()` in
 watsor/detection/devices.py:28-77, with the same precedence rules --
 `CUDA_DEVICE` > `~/.cuda_device` > every visible device, nothing at all when no device is visible
 (`CUDA_VISIBLE_DEVICES=""`: the CUDA runtime inside libwatsor_b200 honours it, so the count is 0).

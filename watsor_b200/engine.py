@@ -12,7 +12,7 @@ from . import _lib
 from ._lib import ClassFilter, check
 from .stream.share import MAX_DETECTIONS, Detection
 
-# 0: fp32 CUDA-core convs; 1: bf16 tcgen05; 2: fp32 storage, dense convs as 3xTF32 tcgen05 (fp32-faithful)
+# 0: fp32 CUDA-core convs; 1: bf16 wgmma; 2: fp32 storage, dense convs as 3xTF32 wgmma (fp32-faithful)
 PRECISION_FP32, PRECISION_BF16_TC, PRECISION_TF32X3 = 0, 1, 2
 
 
@@ -36,7 +36,7 @@ def _addr(obj):
 
 
 class Engine:
-    """One `wb_ctx`: a model resident on one B200 plus per-camera filter tables."""
+    """One `wb_ctx`: a model resident on one H100 plus per-camera filter tables."""
 
     def __init__(self, model_blob, device=0, max_batch=8, precision=PRECISION_FP32):
         self.lib = _lib.load()

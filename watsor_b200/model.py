@@ -1,4 +1,4 @@
-"""Model compiler: frozen TF Object-Detection SSD graph -> B200 layer program.
+"""Model compiler: frozen TF Object-Detection SSD graph -> H100 layer program.
 
 The reference loads `frozen_inference_graph.pb` / `cpu.pb` into a TF session
 (watsor/detection/tensorflow_cpu.py:50-62) or a UFF/ONNX file into TensorRT

@@ -4,7 +4,7 @@ Same class names, constructors and `apply(image_in, image_out, shape, header_in,
 reference, so `Watsor._create_effects` (watsor/main.py:302-312) can return them unchanged; every class is one call
 into `wb_fx_render` (include/watsor_b200.h).  `FusedEffects` does what the whole chain of main.py does for a camera
 -- copy or blend, then draw, then the zone outlines -- in ONE pass over the frame; `EffectsEngine.render` is the batched
-form for several cameras.  There is no CPU fallback: without the library and a B200 the constructors raise.
+form for several cameras.  There is no CPU fallback: without the library and an H100 the constructors raise.
 
 The output bytes are the reference's: BlendEffect's float32 arithmetic is restated (blend.py:15-32), cv2.rectangle at
 thickness 1 is the box outline, cv2.addWeighted is one float fused multiply-add rounded half to even, the label text
@@ -55,7 +55,7 @@ def contour_bits(alpha_channel):
 
 
 class EffectsEngine:
-    """One `wb_fx` context: font tables, label styles and per-camera rasters resident on one B200."""
+    """One `wb_fx` context: font tables, label styles and per-camera rasters resident on one H100."""
 
     def __init__(self, device=0, labels=None):
         self.lib = _lib.load()
@@ -151,7 +151,7 @@ def default_engine():
         from ..detection.devices import b200_gpus
         devices = [d for d, _ in b200_gpus()]
         if not devices:
-            raise _lib.WatsorB200Error('no B200 visible: the GPU visual effects have no CPU fallback')
+            raise _lib.WatsorB200Error('no H100 visible: the GPU visual effects have no CPU fallback')
         _ENGINE = EffectsEngine(devices[0])
     return _ENGINE
 
