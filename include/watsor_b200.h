@@ -107,7 +107,13 @@ int wb_register_host(wb_ctx* ctx, void* ptr, size_t bytes);
 int wb_unregister_host(wb_ctx* ctx, void* ptr);
 
 /* replaces ObjectDetector.detect (tensorflow_cpu.py:74-92 / tensorrt_gpu.py:65-91) for a batch:
- *   frames[i]   uint8 RGB24 HWC image of camera cam_ids[i] (share.py:68-73), host or device memory
+ *   frames[i]   frame of camera cam_ids[i], host or device memory, packed (no row padding):
+ *               uint8 RGB24 HWC [h][w][3] (share.py:68-73) by default; with WB_F_YUV420P or WB_F_NV12 a
+ *               4:2:0 frame [h*3/2][w]: the luma plane [h][w], then the chroma ([h/2][w/2] U, then [h/2][w/2] V
+ *               for yuv420p; [h/2][w/2] interleaved (U, V) pairs for NV12).  4:2:0 needs an even w and h; the
+ *               conversion to RGB (BT.601 limited range) is fused into the resize and equals cv2.cvtColor's
+ *               COLOR_YUV2RGB_I420 / COLOR_YUV2RGB_NV12 byte for byte, so the rows equal those of the RGB frame
+ *               cvtColor makes.  The format is one per batch.
  *   out[i]      Detection[100] block of that frame's header (share.py:27-32); all 100 rows written
  *   verdicts[i] optional uint32[100] filter verdicts (NULL to skip)
  *   flags       WB_F_* below
@@ -117,6 +123,8 @@ int wb_unregister_host(wb_ctx* ctx, void* ptr);
 #define WB_F_FRAMES_ON_DEVICE 1u /* frames[] are device pointers (no H2D)                        */
 #define WB_F_FUSE_FILTERS 2u     /* also write zones[] of rows that pass (state after track.py:26) */
 #define WB_F_OUT_ON_DEVICE 4u    /* out[]/verdicts[] are device pointers (no D2H)                 */
+#define WB_F_YUV420P 8u          /* frames[] are yuv420p (ffmpeg -pix_fmt yuv420p)                */
+#define WB_F_NV12 16u            /* frames[] are NV12 (NVDEC's output, packed); not with YUV420P   */
 int wb_detect(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_t* cam_ids,
               uint32_t flags, wb_detection* const* out, uint32_t* const* verdicts, float* gpu_ms);
 
@@ -182,6 +190,8 @@ typedef struct wb_fx_label {      /* drawing attributes of one label index (conf
 #define WB_FX_DRAW 2u      /* DrawEffect */
 #define WB_FX_CONTOURS 4u  /* ... WithContours */
 #define WB_FX_ON_DEVICE 8u /* images_in / images_out are device pointers */
+#define WB_FX_YUV420P 16u  /* images_in are yuv420p [h*3/2][w] (layouts as for wb_detect); images_out stay RGB24 */
+#define WB_FX_NV12 32u     /* images_in are NV12 [h*3/2][w]; not with WB_FX_YUV420P */
 /* labels[0] is also the style of unknown label indices (coco.py:124-131); digit_glyphs = glyph indices of '0'..'9','%';
  * alpha = opacity of the label box (coco.py:119) */
 int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_label* labels,
@@ -190,7 +200,9 @@ int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_l
  * uint32, bit z-1 set where cv2.drawContours(contours, z-1, thickness=1) paints, or NULL */
 int wb_fx_set_camera(wb_fx* fx, int cam_id, int width, int height, const uint8_t* alpha, const uint32_t* contour_bits);
 /* rows[i]: the 100 Detection rows of frame i (host memory: header.detections).  images: RGB24, host pointers unless
- * WB_FX_ON_DEVICE.  gpu_ms: kernels only. */
+ * WB_FX_ON_DEVICE.  With WB_FX_YUV420P / WB_FX_NV12 images_in are 4:2:0 (even width and height), converted as
+ * cv2.cvtColor does, and images_out[i] must not be images_in[i]; without effect flags the call is then a pure
+ * converter.  gpu_ms: kernels only. */
 int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* const* images_out, const int32_t* cam_ids,
                  const wb_detection* const* rows, uint32_t flags, float* gpu_ms);
 int wb_fx_destroy(wb_fx* fx);

@@ -6,14 +6,15 @@
 
 #include "../../include/watsor_b200.h"
 #include "model_format.h"
+#include "yuv420.cuh"
 
-// One frame of a batch: where its RGB24 pixels are and which camera it belongs to.
+// One frame of a batch: where its pixels are and which camera it belongs to.
 // Replaces the (image_shape, image_np) pair of ObjectDetector.detect (tensorflow_cpu.py:74).
 struct FrameDesc {
-  const uint8_t* ptr;  // device pointer, H*W*3 bytes, row-major RGB24 (share.py:68-73)
+  const uint8_t* ptr;  // device pointer, packed frame_bytes(fmt, w, h) bytes: RGB24 HWC (share.py:68-73) or 4:2:0
   int32_t w, h;
   int32_t cam;
-  int32_t _pad;
+  int32_t fmt;         // WB_FMT_* (yuv420.cuh)
 };
 
 // Per-camera filter state resident in HBM (ConfidenceFilter / AreaFilter / MaskFilter __init__).

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "../../include/watsor_b200.h"
+#include "yuv420.cuh"
 
 namespace {
 
@@ -74,9 +75,10 @@ struct FxCamera {
 };
 
 struct FxFrameDesc {
-  const uint8_t* in;
-  uint8_t* out;
+  const uint8_t* in;  // frame_bytes(fmt, w, h) bytes
+  uint8_t* out;       // RGB24
   FxCamera cam;
+  int32_t fmt;        // WB_FMT_* (yuv420.cuh)
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -216,17 +218,31 @@ __global__ void __launch_bounds__(256, 5)
   const size_t row = (size_t)(live ? y : 0) * W;
   const int npx = live ? min(4, W - xb) : 0;
   const size_t px0 = row + (live ? xb : 0);
-  const uint8_t* src = fd.in + px0 * 3;
+  const bool yuv = fd.fmt != WB_FMT_RGB24;
+  const uint8_t* src = fd.in + px0 * (yuv ? 1 : 3);  // RGB24 pixels, or the luma of a 4:2:0 frame
   uint8_t* dst = fd.out + px0 * 3;
   const bool blend = (flags & WB_FX_BLEND) && fd.cam.alpha != nullptr;
   const bool outline = (flags & WB_FX_CONTOURS) && fd.cam.contours != nullptr;
-  const bool vec = npx == 4 && ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 3) == 0;
+  const bool vec = npx == 4 && (((yuv ? 0 : reinterpret_cast<uintptr_t>(src)) | reinterpret_cast<uintptr_t>(dst)) & 3) == 0;
   // ---- loads first
-  uint32_t ws[3] = {0u, 0u, 0u};
+  uint32_t ws[3] = {0u, 0u, 0u};  // RGB24: the 12 bytes; 4:2:0: 4 Y bytes, then U and V of the 2 chroma samples
   uint8_t v[4][3];
   uint8_t al[4] = {255, 255, 255, 255};
   uint32_t cb[4] = {0u, 0u, 0u, 0u};
-  if (vec) {
+  if (yuv) {
+    // 4 pixels starting at a multiple of 4 in an even-width frame: exactly 2 chroma samples
+    const ChromaLayout cl = chroma_layout(fd.fmt, W, H);
+    const uint8_t* c = chroma_ptr(fd.in, W, H, cl, live ? xb : 0, live ? y : 0);
+#pragma unroll
+    for (int p = 0; p < 4; ++p)
+      if (p < npx) ws[0] |= (uint32_t)__ldg(src + p) << (8 * p);
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+      if (2 * q < npx) {
+        ws[1] |= (uint32_t)__ldg(c + q * cl.step) << (8 * q);
+        ws[2] |= (uint32_t)__ldg(c + q * cl.step + cl.v_off) << (8 * q);
+      }
+  } else if (vec) {
     const uint32_t* s32 = reinterpret_cast<const uint32_t*>(src);
     ws[0] = __ldg(s32);
     ws[1] = __ldg(s32 + 1);
@@ -297,7 +313,16 @@ __global__ void __launch_bounds__(256, 5)
     }
   }
   if (!live) return;
-  if (vec) {
+  if (yuv) {
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      uint32_t r, g, b;
+      yuv_to_rgb((ws[0] >> (8 * p)) & 255u, (ws[1] >> (8 * (p >> 1))) & 255u, (ws[2] >> (8 * (p >> 1))) & 255u, r, g, b);
+      v[p][0] = (uint8_t)r;
+      v[p][1] = (uint8_t)g;
+      v[p][2] = (uint8_t)b;
+    }
+  } else if (vec) {
 #pragma unroll
     for (int i = 0; i < 12; ++i) v[i / 3][i % 3] = (uint8_t)(ws[i >> 2] >> (8 * (i & 3)));
   }
@@ -520,12 +545,20 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   std::lock_guard<std::mutex> lock(fx->mu);
   FXCK(cudaSetDevice(fx->device));
   const bool on_device = (flags & WB_FX_ON_DEVICE) != 0;
+  FXREQ(!((flags & WB_FX_YUV420P) && (flags & WB_FX_NV12)), "WB_FX_YUV420P and WB_FX_NV12 are mutually exclusive");
+  const int fmt = (flags & WB_FX_YUV420P) ? WB_FMT_YUV420P : (flags & WB_FX_NV12) ? WB_FMT_NV12 : WB_FMT_RGB24;
   size_t total = 0;
   int max_w = 0, max_h = 0;
   for (int i = 0; i < n; ++i) {
     auto it = fx->cams.find(cam_ids[i]);
     FXREQ(it != fx->cams.end(), "cam_id " + std::to_string(cam_ids[i]) + " has not been configured with wb_fx_set_camera");
     FXREQ(images_in[i] && images_out[i] && rows[i], "NULL frame / rows pointer");
+    if (fmt != WB_FMT_RGB24) {
+      FXREQ(it->second.w % 2 == 0 && it->second.h % 2 == 0,
+            "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(it->second.w) + "x" +
+                std::to_string(it->second.h) + ": 4:2:0 frames need an even width and height");
+      FXREQ(images_in[i] != images_out[i], "4:2:0 input cannot be rendered in place: images_out must be another buffer");
+    }
     // labels are placed inside the frame only if it is high enough for one above/below/inside a box (draw.py:68-73);
     // lower frames would need OpenCV's re-capping of strokes cut by the bottom border, which the tables do not hold
     const int min_h = 2 * (fx->font.text_height + 2 * fx->font.margin + fx->font.baseline) + 1;
@@ -563,15 +596,16 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   size_t off = 0;
   for (int i = 0; i < n; ++i) {
     const FxCamera& cam = fx->cams[cam_ids[i]];
-    const size_t bytes = (size_t)cam.w * cam.h * 3;
+    const size_t bytes = (size_t)cam.w * cam.h * 3;  // staging slot: the RGB24 output, at least the input
     memcpy(fx->h_rows + (size_t)i * WB_MAX_DETECTIONS, rows[i], sizeof(wb_detection) * WB_MAX_DETECTIONS);
     FxFrameDesc d;
     d.cam = cam;
+    d.fmt = fmt;
     if (on_device) {
       d.in = images_in[i];
       d.out = images_out[i];
     } else {
-      FXCK(cudaMemcpyAsync(fx->d_in + off, images_in[i], bytes, cudaMemcpyHostToDevice, st));
+      FXCK(cudaMemcpyAsync(fx->d_in + off, images_in[i], frame_bytes(fmt, cam.w, cam.h), cudaMemcpyHostToDevice, st));
       d.in = fx->d_in + off;
       d.out = fx->d_out + off;
     }

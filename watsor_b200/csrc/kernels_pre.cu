@@ -34,41 +34,49 @@ __device__ __forceinline__ float lerp_px(float tl, float tr, float bl, float br,
   return __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), ly));
 }
 
-// one resized + normalised pixel (3 channels)
-__device__ __forceinline__ void resized_pixel(const uint8_t* __restrict__ img, int w, const AxisTap& ty,
-                                              const AxisTap& tx, float mul, float sub, float* out3) {
-  const uint8_t* r0 = img + (size_t)ty.lo * w * 3;
-  const uint8_t* r1 = img + (size_t)ty.hi * w * 3;
+// The 12 source bytes one resized pixel interpolates: channel c of tap k (tl, tr, bl, br) goes to raw[c * 4 + k].
+// For a 4:2:0 frame the slots hold Y, U, V of each tap, and resized_pixel_lerp converts them to the RGB24 bytes of
+// cv2.cvtColor first, so the interpolation sees the same bytes as for the converted RGB frame.
+__device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const AxisTap& ty, const AxisTap& tx,
+                                                   uint32_t (&raw)[12]) {
+  if (fd.fmt == WB_FMT_RGB24) {
+    const uint8_t* r0 = fd.ptr + (size_t)ty.lo * fd.w * 3;
+    const uint8_t* r1 = fd.ptr + (size_t)ty.hi * fd.w * 3;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    float tl = (float)__ldg(r0 + tx.lo * 3 + c), tr = (float)__ldg(r0 + tx.hi * 3 + c);
-    float bl = (float)__ldg(r1 + tx.lo * 3 + c), br = (float)__ldg(r1 + tx.hi * 3 + c);
-    float v = lerp_px(tl, tr, bl, br, tx.lerp, ty.lerp);
-    out3[c] = __fsub_rn(__fmul_rn(mul, v), sub);
+    for (int c = 0; c < 3; ++c) {
+      raw[c * 4 + 0] = __ldg(r0 + tx.lo * 3 + c);
+      raw[c * 4 + 1] = __ldg(r0 + tx.hi * 3 + c);
+      raw[c * 4 + 2] = __ldg(r1 + tx.lo * 3 + c);
+      raw[c * 4 + 3] = __ldg(r1 + tx.hi * 3 + c);
+    }
+  } else {
+    const ChromaLayout cl = chroma_layout(fd.fmt, fd.w, fd.h);
+    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.lo, ty.lo, raw[0], raw[4], raw[8]);
+    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.hi, ty.lo, raw[1], raw[5], raw[9]);
+    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.lo, ty.hi, raw[2], raw[6], raw[10]);
+    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.hi, ty.hi, raw[3], raw[7], raw[11]);
   }
 }
-
-// resized_pixel() in two halves, so that a thread can have the 12 byte loads of a second pixel in flight while it
-// lerps the first one (same operations in the same order: bit-identical)
-__device__ __forceinline__ void resized_pixel_load(const uint8_t* __restrict__ img, int w, const AxisTap& ty,
-                                                   const AxisTap& tx, uint32_t (&raw)[12]) {
-  const uint8_t* r0 = img + (size_t)ty.lo * w * 3;
-  const uint8_t* r1 = img + (size_t)ty.hi * w * 3;
+__device__ __forceinline__ void resized_pixel_lerp(uint32_t (&raw)[12], bool yuv, float lx, float ly, float mul,
+                                                   float sub, float* out3) {
+  if (yuv) {
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    raw[c * 4 + 0] = __ldg(r0 + tx.lo * 3 + c);
-    raw[c * 4 + 1] = __ldg(r0 + tx.hi * 3 + c);
-    raw[c * 4 + 2] = __ldg(r1 + tx.lo * 3 + c);
-    raw[c * 4 + 3] = __ldg(r1 + tx.hi * 3 + c);
+    for (int k = 0; k < 4; ++k) yuv_to_rgb(raw[k], raw[4 + k], raw[8 + k], raw[k], raw[4 + k], raw[8 + k]);
   }
-}
-__device__ __forceinline__ void resized_pixel_lerp(const uint32_t (&raw)[12], float lx, float ly, float mul, float sub,
-                                                   float* out3) {
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     float v = lerp_px((float)raw[c * 4 + 0], (float)raw[c * 4 + 1], (float)raw[c * 4 + 2], (float)raw[c * 4 + 3], lx, ly);
     out3[c] = __fsub_rn(__fmul_rn(mul, v), sub);
   }
+}
+
+// one resized + normalised pixel (3 channels).  The two halves above are split so that a thread can have the loads of
+// a second pixel in flight while it lerps the first one.
+__device__ __forceinline__ void resized_pixel(const FrameDesc& fd, const AxisTap& ty, const AxisTap& tx, float mul,
+                                              float sub, float* out3) {
+  uint32_t raw[12];
+  resized_pixel_load(fd, ty, tx, raw);
+  resized_pixel_lerp(raw, fd.fmt != WB_FMT_RGB24, tx.lerp, ty.lerp, mul, sub, out3);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -92,7 +100,7 @@ __device__ __forceinline__ StagePlan stage_plan(const FrameDesc& fd, int ry_a, i
                                                 float sx, int pitch, int max_rows) {
   StagePlan sp;
   sp.on = false;
-  if (pitch <= 0 || ry_a >= ry_b || rx_a >= rx_b) return sp;
+  if (pitch <= 0 || fd.fmt != WB_FMT_RGB24 || ry_a >= ry_b || rx_a >= rx_b) return sp;  // 4:2:0 frames are not staged
   sp.x_first = axis_tap(rx_a, fd.w, sx).lo;
   const int x_last = axis_tap(rx_b - 1, fd.w, sx).hi;
   sp.seg = (x_last - sp.x_first + 1) * 3;
@@ -200,7 +208,7 @@ __global__ void __launch_bounds__(PP_TY* PP_TX) k_preprocess_f32(const FrameDesc
   if (sp.on)
     resized_pixel_staged(fd, sp, s_stage, pitch, oy, ty, tx, mul, sub, v);
   else
-    resized_pixel(fd.ptr, fd.w, ty, tx, mul, sub, v);
+    resized_pixel(fd, ty, tx, mul, sub, v);
   float* o = out + (((size_t)blockIdx.z * oh + oy) * ow + ox) * 3;
   o[0] = v[0];
   o[1] = v[1];
@@ -276,7 +284,7 @@ __global__ void __launch_bounds__(ST_TY* ST_TX)
         if (sp.on)
           resized_pixel_staged(fd, sp, s_stage, pitch, ry, ty, tx, mul, sub, v);
         else
-          resized_pixel(fd.ptr, fd.w, ty, tx, mul, sub, v);
+          resized_pixel(fd, ty, tx, mul, sub, v);
       }
     }
     s_in[i * 3 + 0] = v[0];
@@ -391,7 +399,7 @@ __global__ void __launch_bounds__(256)
         if (inside[u]) {
           tys[u] = axis_tap(ry, fd.h, sy);
           txs[u] = axis_tap(rx, fd.w, sx);
-          resized_pixel_load(fd.ptr, fd.w, tys[u], txs[u], raw[u]);
+          resized_pixel_load(fd, tys[u], txs[u], raw[u]);
         }
       }
 #pragma unroll
@@ -399,7 +407,7 @@ __global__ void __launch_bounds__(256)
         const int i = i0 + u * 256;
         if (i < tile_h * tile_w) {
           float v[3] = {0.f, 0.f, 0.f};
-          if (inside[u]) resized_pixel_lerp(raw[u], txs[u].lerp, tys[u].lerp, mul, sub, v);
+          if (inside[u]) resized_pixel_lerp(raw[u], fd.fmt != WB_FMT_RGB24, txs[u].lerp, tys[u].lerp, mul, sub, v);
           s_in[i * 3 + 0] = v[0];
           s_in[i * 3 + 1] = v[1];
           s_in[i * 3 + 2] = v[2];
@@ -422,7 +430,7 @@ __global__ void __launch_bounds__(256)
         if (sp.on)
           resized_pixel_staged(fd, sp, s_stage, pitch, ry, ty, tx, mul, sub, v);
         else
-          resized_pixel(fd.ptr, fd.w, ty, tx, mul, sub, v);
+          resized_pixel(fd, ty, tx, mul, sub, v);
       }
     }
     s_in[i * 3 + 0] = v[0];

@@ -522,7 +522,9 @@ static int run_all(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags) {
   return run_post(c, s, st, n, flags);
 }
 
-// kernels of one batch, through a CUDA graph when possible (launch-bound at small batch)
+// kernels of one batch, through a CUDA graph when possible (launch-bound at small batch).  The pixel format is not part
+// of the graph's key: the kernels read it from the frame descriptors, which fill_desc copies to the device before every
+// launch, so one graph serves RGB24 and 4:2:0 batches alike.
 static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags) {
   const uint32_t gflags = flags & WB_F_FUSE_FILTERS;
   if (!c->use_graph) {
@@ -555,15 +557,26 @@ static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t 
   return 0;
 }
 
+// pixel format of a batch from its WB_F_* flags
+static int frame_format(uint32_t flags, int* fmt) {
+  REQUIRE(!((flags & WB_F_YUV420P) && (flags & WB_F_NV12)), "WB_F_YUV420P and WB_F_NV12 are mutually exclusive");
+  *fmt = (flags & WB_F_YUV420P) ? WB_FMT_YUV420P : (flags & WB_F_NV12) ? WB_FMT_NV12 : WB_FMT_RGB24;
+  return 0;
+}
+
 static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, const int32_t* cam_ids,
-                     bool on_device, cudaStream_t st) {
+                     bool on_device, int fmt, cudaStream_t st) {
   size_t total = 0;
   for (int i = 0; i < n; ++i) {
     int cam = cam_ids[i];
     REQUIRE(cam >= 0 && cam < WB_MAX_CAMERAS && c->h_cams[cam].width > 0,
             "cam_id " + std::to_string(cam) + " has not been configured with wb_set_camera");
     REQUIRE(frames == nullptr || frames[i] != nullptr, "NULL frame pointer");
-    total += ((size_t)c->h_cams[cam].width * c->h_cams[cam].height * 3 + 255) / 256 * 256;
+    const CameraCfg& cc = c->h_cams[cam];
+    REQUIRE(fmt == WB_FMT_RGB24 || (cc.width % 2 == 0 && cc.height % 2 == 0),
+            "cam_id " + std::to_string(cam) + " is " + std::to_string(cc.width) + "x" + std::to_string(cc.height) +
+                ": 4:2:0 frames need an even width and height");
+    total += (frame_bytes(fmt, cc.width, cc.height) + 255) / 256 * 256;
   }
   if (!on_device && frames != nullptr && total > s.d_frames_cap) {
     CK(cudaStreamSynchronize(st));
@@ -574,12 +587,12 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
   size_t off = 0;
   for (int i = 0; i < n; ++i) {
     const CameraCfg& cc = c->h_cams[cam_ids[i]];
-    size_t bytes = (size_t)cc.width * cc.height * 3;
+    size_t bytes = frame_bytes(fmt, cc.width, cc.height);
     FrameDesc d;
     d.w = cc.width;
     d.h = cc.height;
     d.cam = cam_ids[i];
-    d._pad = 0;
+    d.fmt = fmt;
     if (frames == nullptr) {
       d.ptr = nullptr;
     } else if (on_device) {
@@ -606,8 +619,10 @@ int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const in
   REQUIRE(!s.busy, "slot is busy: collect it first");
   CK(cudaSetDevice(c->device));
   cudaStream_t st = c->stream_of(slot);
+  int fmt = WB_FMT_RGB24;
+  if (int rc = frame_format(flags, &fmt)) return rc;
   CK(cudaEventRecord(s.ev0, st));
-  if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, st)) return rc;
+  if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st)) return rc;
   if (int rc = enqueue_kernels(c, s, st, n, flags)) return rc;
   if (!(flags & WB_F_OUT_ON_DEVICE)) {
     CK(cudaMemcpyAsync(s.h_out, s.d_out, sizeof(wb_detection) * (size_t)n * WB_MAX_DETECTIONS,
@@ -704,7 +719,7 @@ int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t*
   for (int i = 0; i < n; ++i) {
     size_t bytes = (size_t)widths[i] * heights[i] * 3;
     CK(cudaMemcpyAsync(s.d_frames + off, frames[i], bytes, cudaMemcpyHostToDevice, st));
-    s.h_desc[i] = FrameDesc{s.d_frames + off, widths[i], heights[i], -1, 0};
+    s.h_desc[i] = FrameDesc{s.d_frames + off, widths[i], heights[i], -1, WB_FMT_RGB24};
     off += bytes;
   }
   CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n, cudaMemcpyHostToDevice, st));
@@ -776,7 +791,7 @@ int wb_postprocess(wb_ctx* c, int n, const float* enc, const float* logits, cons
   const int NA = c->hdr.num_anchors, C1 = c->hdr.num_classes + 1;
   CK(cudaMemcpyAsync(s.d_enc, enc, sizeof(float) * (size_t)n * NA * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(s.d_logits, logits, sizeof(float) * (size_t)n * NA * C1, cudaMemcpyHostToDevice, st));
-  if (int rc = fill_desc(c, s, n, nullptr, cam_ids, false, st)) return rc;
+  if (int rc = fill_desc(c, s, n, nullptr, cam_ids, false, WB_FMT_RGB24, st)) return rc;
   s.launches = 0;
   if (int rc = run_post(c, s, st, n, flags, true)) return rc;
   const size_t B = c->max_batch;
@@ -834,7 +849,7 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
   Slot& s = c->slots[0];
   REQUIRE(!s.busy, "slot 0 is busy");
   cudaStream_t st = c->stream_of(0);
-  if (int rc = fill_desc(c, s, n, device_frames, cam_ids, true, st)) return rc;
+  if (int rc = fill_desc(c, s, n, device_frames, cam_ids, true, WB_FMT_RGB24, st)) return rc;
   const int nl = (int)c->layers.size();
   REQUIRE(max_launches >= nl + 1, "max_launches too small");
   std::vector<cudaEvent_t> ev(nl + 2);

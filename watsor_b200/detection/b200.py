@@ -101,15 +101,17 @@ class B200ObjectDetector(object):
             self.engine.register_host(addr, ctypes.sizeof(frame.image.get_obj()))
 
     def detect_batch(self, frames, cam_ids, detections, verdicts=None, fuse_filters=True,
-                     frames_on_device=False):
+                     frames_on_device=False, pixel_format='rgb24'):
+        """pixel_format: 'rgb24' (H, W, 3), or the 4:2:0 layouts decoders emit, 'yuv420p' / 'nv12' (H*3//2, W):
+        those are converted on the GPU exactly as cv2.cvtColor converts them.  One format per batch."""
         flags = (_lib.WB_F_FUSE_FILTERS if fuse_filters else 0) | \
                 (_lib.WB_F_FRAMES_ON_DEVICE if frames_on_device else 0)
-        return self.engine.detect(frames, cam_ids, detections, verdicts, flags)
+        return self.engine.detect(frames, cam_ids, detections, verdicts, flags, pixel_format)
 
-    def submit(self, slot, frames, cam_ids, fuse_filters=True, frames_on_device=False):
+    def submit(self, slot, frames, cam_ids, fuse_filters=True, frames_on_device=False, pixel_format='rgb24'):
         flags = (_lib.WB_F_FUSE_FILTERS if fuse_filters else 0) | \
                 (_lib.WB_F_FRAMES_ON_DEVICE if frames_on_device else 0)
-        self.engine.submit(slot, frames, cam_ids, flags)
+        self.engine.submit(slot, frames, cam_ids, flags, pixel_format)
 
     def collect(self, slot, detections=None, verdicts=None):
         return self.engine.collect(slot, detections, verdicts)

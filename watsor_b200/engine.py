@@ -15,6 +15,41 @@ from .stream.share import MAX_DETECTIONS, Detection
 # 0: fp32 CUDA-core convs; 1: bf16 wgmma; 2: fp32 storage, dense convs as 3xTF32 wgmma (fp32-faithful)
 PRECISION_FP32, PRECISION_BF16_TC, PRECISION_TF32X3 = 0, 1, 2
 
+# frame layouts the hot path reads, by ffmpeg's -pix_fmt names -> wb_detect / wb_submit flag
+PIXEL_FORMATS = {'rgb24': 0, 'yuv420p': _lib.WB_F_YUV420P, 'nv12': _lib.WB_F_NV12}
+
+
+def _check_format(pixel_format):
+    if pixel_format not in PIXEL_FORMATS:
+        raise ValueError('pixel_format must be one of %s, not %r' % (', '.join(PIXEL_FORMATS), pixel_format))
+
+
+def frame_shape(pixel_format, width, height):
+    """numpy shape of one packed uint8 frame of a `width` x `height` camera: (H, W, 3) for rgb24, (H*3//2, W) for the
+    4:2:0 formats (luma plane, then the chroma; include/watsor_b200.h), which need an even width and height."""
+    _check_format(pixel_format)
+    if pixel_format == 'rgb24':
+        return (height, width, 3)
+    if width % 2 or height % 2:
+        raise ValueError('%s frames need an even width and height; the camera is %dx%d' % (pixel_format, width, height))
+    return (height * 3 // 2, width)
+
+
+def check_frames(frames, sizes, pixel_format):
+    """Raises ValueError unless every numpy frame is a C-contiguous uint8 array of `frame_shape` for its camera's
+    (width, height) in `sizes`.  A size of None (a camera unknown here, which the library reports) and raw addresses
+    are passed through unchecked."""
+    _check_format(pixel_format)
+    for i, (frame, size) in enumerate(zip(frames, sizes)):
+        if size is None:
+            continue
+        shape = frame_shape(pixel_format, *size)
+        if isinstance(frame, np.ndarray) and (frame.dtype != np.uint8 or frame.shape != shape or
+                                              not frame.flags['C_CONTIGUOUS']):
+            raise ValueError('frame %d: a %s frame of a %dx%d camera is a C-contiguous uint8 array of shape %s, not %s %s%s'
+                             % (i, pixel_format, size[0], size[1], shape, frame.dtype, frame.shape,
+                                '' if frame.flags['C_CONTIGUOUS'] else ' (not C-contiguous)'))
+
 
 def _ptr_array(ptrs):
     arr = (c_void_p * len(ptrs))()
@@ -118,15 +153,22 @@ class Engine:
         vp = _ptr_array([_addr(v) for v in verdicts]) if verdicts is not None else None
         return n, fp, cams, op, vp
 
-    def detect(self, frames, cam_ids, out, verdicts=None, flags=0):
-        """frames: host uint8 arrays (or device pointers with WB_F_FRAMES_ON_DEVICE);
-        out: per frame a `Detection*100` ctypes array / address.  Returns device ms."""
+    def _format_flags(self, frames, cam_ids, pixel_format):
+        check_frames(frames, [self.cameras.get(c) for c in cam_ids], pixel_format)
+        return PIXEL_FORMATS[pixel_format]
+
+    def detect(self, frames, cam_ids, out, verdicts=None, flags=0, pixel_format='rgb24'):
+        """frames: host uint8 arrays (or device pointers with WB_F_FRAMES_ON_DEVICE) in `pixel_format`
+        ('rgb24', 'yuv420p' or 'nv12', see frame_shape); out: per frame a `Detection*100` ctypes array / address.
+        Returns device ms."""
+        flags |= self._format_flags(frames, cam_ids, pixel_format)
         n, fp, cams, op, vp = self._io(frames, cam_ids, out, verdicts)
         ms = c_float(0)
         check(self.lib.wb_detect(self._ctx, n, fp, cams, flags, op, vp, byref(ms)))
         return ms.value
 
-    def submit(self, slot, frames, cam_ids, flags=0):
+    def submit(self, slot, frames, cam_ids, flags=0, pixel_format='rgb24'):
+        flags |= self._format_flags(frames, cam_ids, pixel_format)
         n, fp, cams, _, _ = self._io(frames, cam_ids, None, None)
         check(self.lib.wb_submit(self._ctx, slot, n, fp, cams, flags))
 

@@ -17,10 +17,13 @@ import numpy as np
 
 from .. import _lib
 from ..config.coco import COCO_CLASSES, get_coco_class
+from ..engine import check_frames
 from ..stream.share import MAX_DETECTIONS, Detection
 from .font import FontAtlas
 
 WB_FX_BLEND, WB_FX_DRAW, WB_FX_CONTOURS, WB_FX_ON_DEVICE = 1, 2, 4, 8
+WB_FX_YUV420P, WB_FX_NV12 = 16, 32
+_FX_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_YUV420P, 'nv12': WB_FX_NV12}
 
 
 class _Font(Structure):
@@ -85,6 +88,7 @@ class EffectsEngine:
         self.atlas.lut = None            # 98 MB of host memory: resident on the device now
         self.device = device
         self._next_cam = 0
+        self._sizes = {}                 # cam_id -> (width, height)
         self.last_gpu_ms = 0.0
 
     def close(self):
@@ -115,11 +119,16 @@ class EffectsEngine:
         _check(self.lib.wb_fx_set_camera(self._fx, cam, width, height,
                                          None if alpha is None else alpha.ctypes.data,
                                          None if cont is None else cont.ctypes.data))
+        self._sizes[cam] = (width, height)
         return cam
 
-    def render(self, images_in, images_out, cam_ids, rows, flags):
+    def render(self, images_in, images_out, cam_ids, rows, flags, pixel_format='rgb24'):
         """images: uint8 arrays (or device pointers with WB_FX_ON_DEVICE); rows: per frame the `Detection * 100`
-        array of a frame header (or its address)."""
+        array of a frame header (or its address).  pixel_format: layout of images_in, 'rgb24' or a 4:2:0 layout
+        'yuv420p' / 'nv12' (converted as cv2.cvtColor does; see engine.frame_shape).  images_out are RGB24, and with
+        4:2:0 input they must be other buffers than images_in."""
+        check_frames(images_in, [self._sizes.get(c) for c in cam_ids], pixel_format)
+        flags |= _FX_FORMATS[pixel_format]
         n = len(images_in)
 
         def addr(x):
@@ -262,4 +271,4 @@ def new_rows():
 
 __all__ = ['EffectsEngine', 'CopyHeaderEffect', 'CopyImageEffect', 'BlendEffect', 'DrawEffect',
            'DrawEffectWithContours', 'FusedEffects', 'contour_bits', 'new_rows', 'WB_FX_BLEND', 'WB_FX_DRAW',
-           'WB_FX_CONTOURS', 'WB_FX_ON_DEVICE']
+           'WB_FX_CONTOURS', 'WB_FX_ON_DEVICE', 'WB_FX_YUV420P', 'WB_FX_NV12']
