@@ -35,8 +35,10 @@ bool tc_encode_map(void* map, const void* base, int elem_bytes, int rank, const 
                    const unsigned long long* strides_bytes, const unsigned* box, bool swizzle128, std::string* err,
                    const unsigned* elem_strides = nullptr);
 
-// fused depthwise 3x3 (+BN+ReLU6) -> 1x1 conv (+BN+ReLU6) on tensor cores (kernels_fused.cu); TF32X3 only
-bool fused_dwpw_supported(const TcWeights& tw, int pw_layer_index, const wb_layer& dw, const wb_layer& pw, int n);
+// fused depthwise 3x3 (+BN+ReLU6) -> 1x1 conv (+BN+ReLU6) (+ residual Add) on tensor cores (kernels_fused.cu);
+// TF32X3 only.  `supported` checks the layer shapes and sizes only: the caller checks the arena (the depthwise input
+// must not overlap the output).  `residual` is nullptr or the Add's other operand; `out` is then the Add's output.
+bool fused_dwpw_supported(const TcWeights& tw, int pw_layer_index, const wb_layer& dw, const wb_layer& pw);
 int fused_launch_dwpw(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_index, int n, const wb_layer& dw,
                       const wb_layer& pw, const void* in, const float* dw_w, const float* dw_scale, const float* dw_offset,
-                      const float* scale, const float* offset, void* out, std::string* err);
+                      const float* scale, const float* offset, const float* residual, void* out, std::string* err);

@@ -412,6 +412,54 @@ int wb_unregister_host(wb_ctx* c, void* ptr) {
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------------
+// Which layers run as one kernel.  Both the executor (run_layers) and the per-layer timer (wb_profile_layers) ask this,
+// so the timing table covers exactly what runs.
+enum SpanKind {
+  SPAN_ONE,        // layer li alone
+  SPAN_DW_PW,      // depthwise -> 1x1 (k_dwpw_tc_x3)
+  SPAN_DW_PW_ADD,  // depthwise -> linear 1x1 -> residual Add (k_dwpw_tc_x3, shortcut added in its epilogue)
+  SPAN_PW_ADD,     // linear 1x1 -> residual Add (k_gemm_tc, shortcut added in its epilogue)
+};
+struct Span {
+  size_t last;  // last layer of the span
+  SpanKind kind;
+};
+
+// a fused kernel reads the arena range of `reader`'s input while it writes that of `writer`'s output
+static bool arena_disjoint(const wb_layer& reader, const wb_layer& writer) {
+  const unsigned long long a0 = reader.in_off, a1 = a0 + (unsigned long long)reader.in_h * reader.in_w * reader.in_c;
+  const unsigned long long b0 = writer.out_off, b1 = b0 + (unsigned long long)writer.out_h * writer.out_w * writer.out_c;
+  return !(a0 < b1 && b0 < a1);
+}
+
+// the span of the program that starts at layer `li` (layers [li, end) are requested).  model.py plan_arena keeps each
+// fused kernel's input alive through its output layer; older blobs may not, and their pairs run unfused.
+static Span fused_span(const wb_ctx* c, size_t li, size_t end) {
+  const std::vector<wb_layer>& Ls = c->layers;
+  const wb_layer& L = Ls[li];
+  // layer p + 1 is `Add(shortcut, output of p)` (fp32 modes: the shortcut can be added in an fp32 epilogue)
+  auto residual_add_after = [&](size_t p) {
+    if (c->precision == 0 || c->precision == 1 || p + 1 >= end || getenv("WB_NO_FUSE_ADD") != nullptr) return false;
+    const wb_layer& P = Ls[p], &A = Ls[p + 1];
+    return P.op == WB_OP_PW && P.act == WB_ACT_NONE && A.op == WB_OP_ADD &&
+           (A.in_off == P.out_off || A.in2_off == P.out_off) && A.in_off != A.in2_off;
+  };
+  if (L.op == WB_OP_DW && c->precision == 2 && li + 1 < end && getenv("WB_NO_FUSE") == nullptr) {
+    const wb_layer& P = Ls[li + 1];
+    if (P.in_off == L.out_off && fused_dwpw_supported(c->tc, (int)li + 1, L, P)) {
+      if (residual_add_after(li + 1)) {
+        if (arena_disjoint(L, Ls[li + 2])) return {li + 2, SPAN_DW_PW_ADD};
+      } else if (arena_disjoint(L, P)) {
+        return {li + 1, SPAN_DW_PW};
+      }
+    }
+  }
+  if (L.op == WB_OP_PW && c->precision != 0 && tc_layer_supported(L) && residual_add_after(li) &&
+      arena_disjoint(L, Ls[li + 1]))
+    return {li + 1, SPAN_PW_ADD};
+  return {li, SPAN_ONE};
+}
+
 // the layer program.  `pre` != NULL feeds an already pre-processed input (wb_backbone); otherwise the
 // fused stem samples the frames directly.  When `times` is given every launch is bracketed by events.
 template <typename T>
@@ -435,18 +483,20 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
                        sc, of, outp, c->max_src_w);
         break;
       case WB_OP_DW: {
-        // depthwise -> 1x1 pairs run as one tensor-core kernel when both layers are in the requested range
-        if (c->precision == 2 && li + 1 < end) {
+        const Span sp = fused_span(c, li, end);
+        if (sp.kind == SPAN_DW_PW || sp.kind == SPAN_DW_PW_ADD) {
           const wb_layer& P = c->layers[li + 1];
-          if (P.in_off == L.out_off && fused_dwpw_supported(c->tc, (int)li + 1, L, P, n)) {
-            std::string err;
-            if (fused_launch_dwpw(lc, c->tc, (int)li + 1, n, L, P, static_cast<const void*>(in), w, sc, of,
-                                  c->tensor(P.scale_tensor), c->tensor(P.offset_tensor),
-                                  static_cast<void*>(arena + (size_t)P.out_off * n), &err))
-              return fail("layers " + std::string(L.name) + " + " + P.name + ": " + err);
-            ++li;  // the 1x1 layer is done
-            break;
-          }
+          const wb_layer& O = c->layers[sp.last];  // the layer whose output the kernel writes
+          const float* residual = nullptr;
+          if (sp.kind == SPAN_DW_PW_ADD)
+            residual = reinterpret_cast<const float*>(arena + (size_t)(O.in_off == P.out_off ? O.in2_off : O.in_off) * n);
+          std::string err;
+          if (fused_launch_dwpw(lc, c->tc, (int)li + 1, n, L, P, static_cast<const void*>(in), w, sc, of,
+                                c->tensor(P.scale_tensor), c->tensor(P.offset_tensor), residual,
+                                static_cast<void*>(arena + (size_t)O.out_off * n), &err))
+            return fail("layers " + std::string(L.name) + " .. " + O.name + ": " + err);
+          li = sp.last;
+          break;
         }
         launch_dw<T>(lc, n, L, in, w, sc, of, outp);
         break;
@@ -469,20 +519,12 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
           // the shortcut is added in the GEMM epilogue (fp32 modes) and the Add layer is skipped
           const void* residual = nullptr;
           void* dst = static_cast<void*>(outp);
-          bool fuse_add = false;
-          if (c->precision != 1 && L.op == WB_OP_PW && L.act == WB_ACT_NONE && li + 1 < end && getenv("WB_NO_FUSE_ADD") == nullptr) {
+          const bool fuse_add = fused_span(c, li, end).kind == SPAN_PW_ADD;
+          if (fuse_add) {
             const wb_layer& A = c->layers[li + 1];
-            // the fused kernel reads this layer's input while it writes the Add's output: they must not overlap
-            // (model.py plan_arena keeps the input alive through the Add; older blobs may not)
-            const unsigned long long a0 = L.in_off, a1 = a0 + (unsigned long long)L.in_h * L.in_w * L.in_c;
-            const unsigned long long b0 = A.out_off, b1 = b0 + (unsigned long long)A.out_h * A.out_w * A.out_c;
-            if (A.op == WB_OP_ADD && (A.in_off == L.out_off || A.in2_off == L.out_off) && A.in_off != A.in2_off &&
-                !(a0 < b1 && b0 < a1)) {
-              const uint32_t other = A.in_off == L.out_off ? A.in2_off : A.in_off;
-              residual = static_cast<const void*>(arena + (size_t)other * n);
-              dst = static_cast<void*>(arena + (size_t)A.out_off * n);
-              fuse_add = true;
-            }
+            const uint32_t other = A.in_off == L.out_off ? A.in2_off : A.in_off;
+            residual = static_cast<const void*>(arena + (size_t)other * n);
+            dst = static_cast<void*>(arena + (size_t)A.out_off * n);
           }
           std::string err;
           if (tc_launch_gemm(lc, c->tc, (int)li, n, L, static_cast<const void*>(in), sc, of, dst, s.d_enc, s.d_logits, NA,
@@ -862,26 +904,14 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
   s.launches = 0;
   CK(cudaEventRecord(ev[0], st));
   for (int li = 0; li < nl; ++li) {
-    // a depthwise layer that the executor fuses into the following 1x1 conv is timed together with it:
-    // the pair's time is reported on the 1x1 layer, the depthwise entry reads 0
-    int last = li;
-    if (c->precision == 2 && li + 1 < nl && c->layers[li].op == WB_OP_DW &&
-        c->layers[li + 1].in_off == c->layers[li].out_off &&
-        fused_dwpw_supported(c->tc, li + 1, c->layers[li], c->layers[li + 1], n))
-      last = li + 1;
-    // a linear projection + residual Add pair runs as one kernel too (same conditions as run_layers); the
-    // pair's time is reported on the Add entry, the projection entry reads 0
-    if (last == li && c->precision != 0 && c->precision != 1 && li + 1 < nl && c->layers[li].op == WB_OP_PW &&
-        c->layers[li].act == WB_ACT_NONE && c->layers[li + 1].op == WB_OP_ADD && tc_layer_supported(c->layers[li]) &&
-        (c->layers[li + 1].in_off == c->layers[li].out_off || c->layers[li + 1].in2_off == c->layers[li].out_off) &&
-        getenv("WB_NO_FUSE_ADD") == nullptr)
-      last = li + 1;
-    const int first = li;
-    const bool time_on_first = last != li && c->layers[li].op == WB_OP_PW;  // projection + Add: time on the GEMM
-    if (last != li && !time_on_first) {
-      CK(cudaEventRecord(ev[li + 1], st));  // zero-length interval for the depthwise entry
+    // a span the executor runs as one kernel is timed as a whole; its time is reported on the 1x1 (projection)
+    // entry and the span's other entries read 0
+    const Span sp = fused_span(c, li, nl);
+    const int first = li, last = (int)sp.last;
+    const int timed = sp.kind == SPAN_DW_PW || sp.kind == SPAN_DW_PW_ADD ? li + 1 : li;
+    for (; li < timed; ++li) {
+      CK(cudaEventRecord(ev[li + 1], st));  // zero-length interval
       kinds[li] = (int)c->layers[li].op;
-      ++li;
     }
     for (int r = 0; r < REPS; ++r) {
       int rc = c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, n, nullptr, first, last)
@@ -890,9 +920,9 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
     }
     CK(cudaEventRecord(ev[li + 1], st));
     kinds[li] = (int)c->layers[li].op;
-    if (time_on_first) {
+    while (li < last) {
       ++li;
-      CK(cudaEventRecord(ev[li + 1], st));  // zero-length interval for the Add entry
+      CK(cudaEventRecord(ev[li + 1], st));  // zero-length interval
       kinds[li] = (int)c->layers[li].op;
     }
   }

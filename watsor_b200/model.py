@@ -120,12 +120,17 @@ class Model:
             for t in (l.src, l.src2):
                 if t:
                     last_use[t] = i
-        # a depthwise layer may be fused into the following 1x1 conv (csrc/kernels_fused.cu): the fused kernel
-        # reads the depthwise INPUT while it writes the 1x1 OUTPUT, so that input must outlive the 1x1 layer
+        # a depthwise layer may be fused into the following 1x1 conv, and into the residual `Add` of that conv's output
+        # after it (csrc/kernels_fused.cu): the fused kernel reads the depthwise INPUT while it writes the 1x1 (or
+        # Add) OUTPUT, so that input must outlive the kernel's last layer
         for i, l in enumerate(self.layers[:-1]):
             nxt = self.layers[i + 1]
             if l.op == OP_DW and nxt.op == OP_PW and nxt.src == l.dst and l.src:
-                last_use[l.src] = max(last_use[l.src], i + 1)
+                end_ = i + 1
+                if i + 2 < len(self.layers) and self.layers[i + 2].op == OP_ADD and \
+                        nxt.dst in (self.layers[i + 2].src, self.layers[i + 2].src2):
+                    end_ = i + 2
+                last_use[l.src] = max(last_use[l.src], end_)
         # a linear 1x1 projection followed by the residual `Add` of its output runs as one kernel (the shortcut is
         # added in the GEMM epilogue, csrc/wb_api.cu run_layers): that kernel reads the projection's INPUT while it
         # writes the Add's OUTPUT, so the input must outlive the Add layer
@@ -133,17 +138,6 @@ class Model:
             nxt = self.layers[i + 1]
             if l.op == OP_PW and nxt.op == OP_ADD and l.dst in (nxt.src, nxt.src2) and l.src:
                 last_use[l.src] = max(last_use[l.src], i + 1)
-        # an inverted residual block (1x1 expand -> depthwise -> linear 1x1 projection [-> Add]) may run as ONE kernel
-        # (csrc/kernels_fused.cu k_irb_x3) that reads the block INPUT while it writes the block OUTPUT: the input must
-        # outlive the block's last layer
-        for i, l in enumerate(self.layers[:-2]):
-            d, p_ = self.layers[i + 1], self.layers[i + 2]
-            if l.op == OP_PW and d.op == OP_DW and p_.op == OP_PW and d.src == l.dst and p_.src == d.dst and l.src:
-                end_ = i + 2
-                if i + 3 < len(self.layers) and self.layers[i + 3].op == OP_ADD and \
-                        p_.dst in (self.layers[i + 3].src, self.layers[i + 3].src2):
-                    end_ = i + 3
-                last_use[l.src] = max(last_use[l.src], end_)
         size = {}
         for l in self.layers:
             if l.dst:
