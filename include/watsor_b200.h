@@ -101,6 +101,19 @@ int wb_set_camera(wb_ctx* ctx, int cam_id, int width, int height, int n_zones,
                   const uint8_t* zone_raster, int n_filters, const wb_class_filter* filters,
                   uint32_t flags);
 
+/* Detection windows of a camera (no counterpart in the reference, whose frames are always squeezed whole into the
+ * model's input).  xywh: n_windows rectangles (x, y, w, h) in the camera's pixels, each inside the frame set by
+ * wb_set_camera; (0, 0, width, height) is the whole frame.  Every window of every frame of the camera becomes one model
+ * image; max_batch counts model images.  A window's rows are those of the frame cropped to the window, shifted by
+ * (x, y).  The rows of a frame's windows are then merged into its 100 rows (k_window_merge, DESIGN.md 4.4): sorted by
+ * (confidence descending, window, row); a row is dropped when an already kept row of the same label from another
+ * window covers more than merge_threshold (in [0, 1]) of the smaller of the two inclusive pixel boxes; the first 100
+ * kept rows are filtered as the camera's rows always are.  In a batch with windows, a camera without any is one
+ * full-frame window.  4:2:0 batches need even window origins and sizes.  n_windows = 0 removes the windows;
+ * wb_set_camera clears them. */
+#define WB_MAX_WINDOWS 16
+int wb_set_camera_windows(wb_ctx* ctx, int cam_id, int n_windows, const int32_t* xywh, double merge_threshold);
+
 /* ---- the hot path ----------------------------------------------------------------------------- */
 /* pin host frame memory (multiprocessing shared ctypes arrays, share.py:40) for async H2D */
 int wb_register_host(wb_ctx* ctx, void* ptr, size_t bytes);
@@ -123,6 +136,8 @@ int wb_unregister_host(wb_ctx* ctx, void* ptr);
 #define WB_F_FRAMES_ON_DEVICE 1u /* frames[] are device pointers (no H2D)                        */
 #define WB_F_FUSE_FILTERS 2u     /* also write zones[] of rows that pass (state after track.py:26) */
 #define WB_F_OUT_ON_DEVICE 4u    /* out[]/verdicts[] are device pointers (no D2H)                 */
+/* n counts frames; a batch whose cameras have detection windows (wb_set_camera_windows) runs one model image per
+ * window and needs n_images <= max_batch */
 #define WB_F_YUV420P 8u          /* frames[] are yuv420p (ffmpeg -pix_fmt yuv420p)                */
 #define WB_F_NV12 16u            /* frames[] are NV12 (NVDEC's output, packed); not with YUV420P   */
 int wb_detect(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_t* cam_ids,

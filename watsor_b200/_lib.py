@@ -12,6 +12,7 @@ WB_F_FRAMES_ON_DEVICE, WB_F_FUSE_FILTERS, WB_F_OUT_ON_DEVICE = 1, 2, 4
 WB_F_YUV420P, WB_F_NV12 = 8, 16
 WB_V_LABEL, WB_V_CONFIDENCE, WB_V_AREA, WB_V_MASK, WB_V_PASS = 1, 2, 4, 8, 16
 WB_CAM_NO_LABEL_CHECK = 1
+WB_MAX_WINDOWS = 16
 
 
 class ClassFilter(Structure):
@@ -63,6 +64,7 @@ def load():
         'wb_model_info': (c_int, [c_void_p, P(c_int32), P(c_int32), P(c_int32), P(c_int32), P(c_int32)]),
         'wb_set_camera': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
                                   P(ClassFilter), c_uint32]),
+        'wb_set_camera_windows': (c_int, [c_void_p, c_int, c_int, P(c_int32), c_double]),
         'wb_register_host': (c_int, [c_void_p, c_void_p, c_size_t]),
         'wb_unregister_host': (c_int, [c_void_p, c_void_p]),
         'wb_detect': (c_int, [c_void_p, c_int, P(c_void_p), P(c_int32), c_uint32, P(c_void_p),
@@ -108,7 +110,8 @@ def load():
 
 
 EXPORTS = ['wb_abi_version', 'wb_last_error', 'wb_device_count', 'wb_create', 'wb_destroy',
-           'wb_device_name', 'wb_set_stream', 'wb_model_info', 'wb_set_camera', 'wb_register_host',
+           'wb_device_name', 'wb_set_stream', 'wb_model_info', 'wb_set_camera', 'wb_set_camera_windows',
+           'wb_register_host',
            'wb_unregister_host', 'wb_detect', 'wb_submit', 'wb_collect', 'wb_stream_fence', 'wb_comm_unique_id', 'wb_comm_init',
            'wb_scatter_frames', 'wb_comm_destroy', 'wb_preprocess', 'wb_backbone',
            'wb_postprocess', 'wb_filter_rows', 'wb_anchors', 'wb_last_launch_count', 'wb_profile_layers',

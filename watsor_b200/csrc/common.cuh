@@ -8,13 +8,27 @@
 #include "model_format.h"
 #include "yuv420.cuh"
 
-// One frame of a batch: where its pixels are and which camera it belongs to.
+// One model image of a batch: where its pixels are and which camera it belongs to.  The image is a whole frame or a
+// detection window of one (wb_set_camera_windows); either way its rows start at `ptr`, `pitch` bytes apart.
 // Replaces the (image_shape, image_np) pair of ObjectDetector.detect (tensorflow_cpu.py:74).
 struct FrameDesc {
-  const uint8_t* ptr;  // device pointer, packed frame_bytes(fmt, w, h) bytes: RGB24 HWC (share.py:68-73) or 4:2:0
+  const uint8_t* ptr;     // device pointer to pixel (0, 0): RGB24 HWC (share.py:68-73), or the luma of a 4:2:0 frame
+  const uint8_t* chroma;  // 4:2:0: the U sample of pixel (0, 0) (packed frame: ptr + w*h)
   int32_t w, h;
+  int32_t pitch;          // bytes between rows of the RGB24 / luma plane (packed frame: 3w / w)
+  int32_t cam;            // -1: no camera (a window's rows are filtered after the merge, k_window_merge)
+  int32_t fmt;            // WB_FMT_* (yuv420.cuh)
+  int32_t v_off;          // 4:2:0: bytes from a U sample to its V sample (ChromaLayout::v_off of the parent frame)
+};
+
+// The model images of one frame of a windowed batch, for k_window_merge: images [first, first + count) are its
+// windows, whose rows are shifted by the window's origin.
+struct WindowFrame {
+  int32_t first, count;
   int32_t cam;
-  int32_t fmt;         // WB_FMT_* (yuv420.cuh)
+  int32_t _pad;
+  double merge_thr;  // a row is dropped when a kept row of another window covers more than this share of the smaller box
+  int32_t x[WB_MAX_WINDOWS], y[WB_MAX_WINDOWS];
 };
 
 // Per-camera filter state resident in HBM (ConfidenceFilter / AreaFilter / MaskFilter __init__).
@@ -137,6 +151,9 @@ void launch_post(const LaunchCtx& lc, int n, const PostParams& pp, const float* 
                  float* dec_boxes, int* cand_count, unsigned long long* cand, int* sel_count,
                  unsigned long long* sel, wb_detection* out, uint32_t* verdicts, float* raw_boxes,
                  float* raw_scores, float* raw_classes, int* raw_num, int* kept_hist);
+void launch_window_merge(const LaunchCtx& lc, int n_frames, const PostParams& pp, const WindowFrame* win,
+                         const wb_detection* rows, const int* raw_num, const CameraCfg* cams, uint32_t flags,
+                         wb_detection* out, uint32_t* verdicts);
 void launch_filter_rows(const LaunchCtx& lc, const CameraCfg* cam, int n_rows, wb_detection* rows,
                         uint32_t* verdicts);
 void launch_build_sat(const LaunchCtx& lc, const uint8_t* raster, int n_zones, int h, int w, int32_t* sat);

@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(256, 5)
   if (yuv) {
     // 4 pixels starting at a multiple of 4 in an even-width frame: exactly 2 chroma samples
     const ChromaLayout cl = chroma_layout(fd.fmt, W, H);
-    const uint8_t* c = chroma_ptr(fd.in, W, H, cl, live ? xb : 0, live ? y : 0);
+    const uint8_t* c = chroma_ptr(fd.in + (size_t)W * H, cl, live ? xb : 0, live ? y : 0);
 #pragma unroll
     for (int p = 0; p < 4; ++p)
       if (p < npx) ws[0] |= (uint32_t)__ldg(src + p) << (8 * p);

@@ -625,6 +625,130 @@ void launch_post(const LaunchCtx& lc, int n, const PostParams& pp, const float* 
   ++*lc.launch_counter;
 }
 
+// ------------------------------------------------------------------------------------------- window merge
+// One block per frame of a batch with detection windows (wb_set_camera_windows).  k_merge_filter has written every
+// window's rows (camera -1: no predicates) and its number of valid rows (raw_num).  Those rows are sorted by the key
+// score_bits << 32 | ~(window << 8 | row) -- confidence descending, then window, then row: scores are >= 0, so the
+// float's bits order like its value, and padding keys (0) sort last.  One warp walks the sorted rows and keeps a row
+// unless an already kept row with the same label from ANOTHER window covers more than merge_thr of the smaller box
+// (intersection over the smaller of the two integer, inclusive pixel boxes, after the shift by the window's origin).
+// Rows of one window never suppress each other: the model's NMS has decided between them.  IoS rather than IoU: a part
+// of an object cut by a window border lies inside the whole box seen by a neighbouring or the full-frame window.  The
+// first max_total kept rows, then padding rows as k_merge_filter writes them, go through the camera's predicates.
+constexpr int WM_THREADS = 256;
+constexpr int WM_KEYS = 2048;  // >= WB_MAX_WINDOWS * WB_MAX_DETECTIONS, a power of two
+static_assert(WM_KEYS >= WB_MAX_WINDOWS * WB_MAX_DETECTIONS, "window merge keys");
+
+__global__ void __launch_bounds__(WM_THREADS)
+    k_window_merge(PostParams pp, const WindowFrame* __restrict__ win, const wb_detection* __restrict__ rows,
+                   const int* __restrict__ raw_num, const CameraCfg* __restrict__ cams, uint32_t flags,
+                   wb_detection* __restrict__ out, uint32_t* __restrict__ verdicts) {
+  __shared__ unsigned long long s_keys[WM_KEYS];
+  __shared__ int4 s_kbox[WB_MAX_DETECTIONS];  // kept rows: x_min, y_min, x_max, y_max in camera pixels
+  __shared__ long long s_karea[WB_MAX_DETECTIONS];
+  __shared__ int s_klab[WB_MAX_DETECTIONS], s_kid[WB_MAX_DETECTIONS];  // label, window << 8 | row
+  __shared__ int s_nvalid[WB_MAX_WINDOWS];
+  __shared__ int s_nkept;
+  const int f = blockIdx.x;
+  const WindowFrame& wf = win[f];
+  const int first = wf.first, count = wf.count;
+  const int max_out = min(pp.max_total, WB_MAX_DETECTIONS);
+  if ((int)threadIdx.x < count) s_nvalid[threadIdx.x] = min(raw_num[first + threadIdx.x], WB_MAX_DETECTIONS);
+  __syncthreads();
+  int P = 32;
+  while (P < count * WB_MAX_DETECTIONS) P <<= 1;
+  for (int i = threadIdx.x; i < P; i += blockDim.x) {
+    const int w = i / WB_MAX_DETECTIONS, r = i - w * WB_MAX_DETECTIONS;
+    unsigned long long k = 0ull;
+    if (w < count && r < s_nvalid[w]) {
+      const float score = (float)rows[(size_t)(first + w) * WB_MAX_DETECTIONS + r].confidence;  // exact: it was a float
+      k = ((unsigned long long)__float_as_uint(score) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(w << 8 | r));
+    }
+    s_keys[i] = k;
+  }
+  __syncthreads();
+  bitonic_desc(s_keys, P);
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    int total = 0;
+    for (int w = 0; w < count; ++w) total += s_nvalid[w];
+    const double thr = wf.merge_thr;
+    int nk = 0;
+    for (int base = 0; base < total && nk < max_out; base += 32) {
+      // lane l fetches candidate base + l; the candidates are then decided one after another
+      const int cnt = min(32, total - base);
+      int id = 0, lab = 0;
+      int4 b = make_int4(0, 0, 0, 0);
+      long long area = 0;
+      if (lane < cnt) {
+        id = (int)(0xFFFFFFFFu - (unsigned)(s_keys[base + lane] & 0xFFFFFFFFull));
+        const int w = id >> 8;
+        const wb_detection& d = rows[(size_t)(first + w) * WB_MAX_DETECTIONS + (id & 255)];
+        lab = d.label;
+        b = make_int4(d.bounding_box.x_min + wf.x[w], d.bounding_box.y_min + wf.y[w], d.bounding_box.x_max + wf.x[w],
+                      d.bounding_box.y_max + wf.y[w]);
+        area = (long long)(b.z - b.x + 1) * (long long)(b.w - b.y + 1);
+      }
+      for (int t = 0; t < cnt && nk < max_out; ++t) {
+        const int tid = __shfl_sync(0xffffffffu, id, t), tlab = __shfl_sync(0xffffffffu, lab, t);
+        const int4 tb = make_int4(__shfl_sync(0xffffffffu, b.x, t), __shfl_sync(0xffffffffu, b.y, t),
+                                  __shfl_sync(0xffffffffu, b.z, t), __shfl_sync(0xffffffffu, b.w, t));
+        const long long tarea = __shfl_sync(0xffffffffu, area, t);
+        bool sup = false;
+        for (int j = lane; j < nk; j += 32) {
+          if (s_klab[j] != tlab || (s_kid[j] >> 8) == (tid >> 8)) continue;
+          const int4 kb = s_kbox[j];
+          const long long iw = (long long)min(tb.z, kb.z) - max(tb.x, kb.x) + 1;
+          const long long ih = (long long)min(tb.w, kb.w) - max(tb.y, kb.y) + 1;
+          const long long inter = iw > 0 && ih > 0 ? iw * ih : 0;
+          sup |= (double)inter > __dmul_rn(thr, (double)min(tarea, s_karea[j]));
+        }
+        if (__any_sync(0xffffffffu, sup)) continue;  // warp-uniform
+        if (lane == t) {
+          s_kbox[nk] = b;
+          s_karea[nk] = area;
+          s_klab[nk] = lab;
+          s_kid[nk] = id;
+        }
+        ++nk;
+        __syncwarp();
+      }
+    }
+    if (lane == 0) s_nkept = nk;
+  }
+  __syncthreads();
+  const int r = threadIdx.x;
+  if (r >= WB_MAX_DETECTIONS) return;
+  wb_detection d;
+  for (int z = 0; z < WB_MAX_ZONES; ++z) d.zones[z] = 0;
+  if (r < s_nkept) {
+    const int id = s_kid[r];
+    const wb_detection& src = rows[(size_t)(first + (id >> 8)) * WB_MAX_DETECTIONS + (id & 255)];
+    const int4 b = s_kbox[r];
+    d.label = src.label;
+    d.confidence = src.confidence;
+    d.bounding_box.x_min = b.x;
+    d.bounding_box.y_min = b.y;
+    d.bounding_box.x_max = b.z;
+    d.bounding_box.y_max = b.w;
+  } else {  // k_merge_filter's padding row
+    d.label = (int)__fadd_rn(0.f, pp.class_offset);
+    d.confidence = 0.0;
+    d.bounding_box.x_min = d.bounding_box.y_min = d.bounding_box.x_max = d.bounding_box.y_max = 0;
+  }
+  const CameraCfg* cam = cams != nullptr && wf.cam >= 0 ? cams + wf.cam : nullptr;
+  const uint32_t v = apply_filters(cam, &d, (flags & WB_F_FUSE_FILTERS) != 0);
+  out[(size_t)f * WB_MAX_DETECTIONS + r] = d;
+  if (verdicts) verdicts[(size_t)f * WB_MAX_DETECTIONS + r] = v;
+}
+
+void launch_window_merge(const LaunchCtx& lc, int n_frames, const PostParams& pp, const WindowFrame* win,
+                         const wb_detection* rows, const int* raw_num, const CameraCfg* cams, uint32_t flags,
+                         wb_detection* out, uint32_t* verdicts) {
+  k_window_merge<<<n_frames, WM_THREADS, 0, lc.stream>>>(pp, win, rows, raw_num, cams, flags, out, verdicts);
+  ++*lc.launch_counter;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // stand-alone predicate chain on caller rows (ConfidenceFilter / AreaFilter / MaskFilter __call__)
 __global__ void k_filter_rows(const CameraCfg* __restrict__ cam, int n_rows, wb_detection* __restrict__ rows,

@@ -40,8 +40,8 @@ __device__ __forceinline__ float lerp_px(float tl, float tr, float bl, float br,
 __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const AxisTap& ty, const AxisTap& tx,
                                                    uint32_t (&raw)[12]) {
   if (fd.fmt == WB_FMT_RGB24) {
-    const uint8_t* r0 = fd.ptr + (size_t)ty.lo * fd.w * 3;
-    const uint8_t* r1 = fd.ptr + (size_t)ty.hi * fd.w * 3;
+    const uint8_t* r0 = fd.ptr + (size_t)ty.lo * fd.pitch;
+    const uint8_t* r1 = fd.ptr + (size_t)ty.hi * fd.pitch;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       raw[c * 4 + 0] = __ldg(r0 + tx.lo * 3 + c);
@@ -50,11 +50,13 @@ __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const Ax
       raw[c * 4 + 3] = __ldg(r1 + tx.hi * 3 + c);
     }
   } else {
-    const ChromaLayout cl = chroma_layout(fd.fmt, fd.w, fd.h);
-    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.lo, ty.lo, raw[0], raw[4], raw[8]);
-    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.hi, ty.lo, raw[1], raw[5], raw[9]);
-    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.lo, ty.hi, raw[2], raw[6], raw[10]);
-    yuv420_load(fd.ptr, fd.w, fd.h, cl, tx.hi, ty.hi, raw[3], raw[7], raw[11]);
+    // the chroma rows are half as many bytes apart as the luma rows (yuv420p) or as many (NV12's U, V pairs)
+    const bool nv12 = fd.fmt == WB_FMT_NV12;
+    const ChromaLayout cl{nv12 ? 2 : 1, nv12 ? fd.pitch : fd.pitch / 2, (size_t)fd.v_off};
+    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.lo, ty.lo, raw[0], raw[4], raw[8]);
+    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.hi, ty.lo, raw[1], raw[5], raw[9]);
+    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.lo, ty.hi, raw[2], raw[6], raw[10]);
+    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.hi, ty.hi, raw[3], raw[7], raw[11]);
   }
 }
 __device__ __forceinline__ void resized_pixel_lerp(uint32_t (&raw)[12], bool yuv, float lx, float ly, float mul,
@@ -122,14 +124,15 @@ __device__ __forceinline__ const uint8_t* stage_src(const FrameDesc& fd, const S
     AxisTap t = axis_tap(sp.ry_a + (r >> 1), fd.h, sy);
     y = (r & 1) ? t.hi : t.lo;
   }
-  return fd.ptr + ((size_t)y * fd.w + sp.x_first) * 3;
+  return fd.ptr + (size_t)y * fd.pitch + (size_t)sp.x_first * 3;
 }
 
 // all threads of the CTA; caller synchronises afterwards
 __device__ __forceinline__ void stage_rows(const FrameDesc& fd, const StagePlan& sp, float sy, uint8_t* s_stage,
                                            int pitch, int tid, int nthreads) {
+  // the image's own bytes: a window's rows are not contiguous, but nothing outside its first and last row is read
   const uint8_t* f_begin = fd.ptr;
-  const uint8_t* f_end = fd.ptr + (size_t)fd.h * fd.w * 3;
+  const uint8_t* f_end = fd.ptr + (size_t)(fd.h - 1) * fd.pitch + (size_t)fd.w * 3;
   for (int i = tid; i < sp.rows * sp.cpr; i += nthreads) {
     const int r = i / sp.cpr, k = i - r * sp.cpr;
     const uint8_t* src = stage_src(fd, sp, r, sy);
@@ -138,7 +141,7 @@ __device__ __forceinline__ void stage_rows(const FrameDesc& fd, const StagePlan&
     uint4 v;
     if (g >= f_begin && g + 16 <= f_end) {
       v = __ldg(reinterpret_cast<const uint4*>(g));
-    } else {  // first / last chunk of the frame: never touch bytes outside the buffer
+    } else {  // first / last chunk of the image: never touch bytes outside it
       uint32_t wds[4] = {0u, 0u, 0u, 0u};
       for (int b = 0; b < 16; ++b)
         if (g + b >= f_begin && g + b < f_end) wds[b >> 2] |= (uint32_t)__ldg(g + b) << (8 * (b & 3));
@@ -155,7 +158,7 @@ __device__ __forceinline__ void resized_pixel_staged(const FrameDesc& fd, const 
   const int r0 = sp.contiguous ? ty.lo - sp.y_first : 2 * (ry - sp.ry_a);
   const int r1 = sp.contiguous ? ty.hi - sp.y_first : 2 * (ry - sp.ry_a) + 1;
   const uintptr_t base = reinterpret_cast<uintptr_t>(fd.ptr) + (size_t)sp.x_first * 3;
-  const size_t row_bytes = (size_t)fd.w * 3;
+  const size_t row_bytes = (size_t)fd.pitch;
   const int sh0 = (int)((base + (size_t)ty.lo * row_bytes) & 15), sh1 = (int)((base + (size_t)ty.hi * row_bytes) & 15);
   const uint8_t* p0 = s_stage + (size_t)r0 * pitch + sh0;
   const uint8_t* p1 = s_stage + (size_t)r1 * pitch + sh1;

@@ -55,13 +55,20 @@ struct Slot {
   uint32_t *d_verdicts = nullptr, *h_verdicts = nullptr;
   float *d_raw = nullptr, *h_raw = nullptr;  // boxes[n][100][4] scores[n][100] classes[n][100]
   int *d_raw_num = nullptr, *h_raw_num = nullptr;
-  int n = 0;
+  // batches with detection windows: the frames' windows (copied before every launch) and their merged rows
+  WindowFrame *h_win = nullptr, *d_win = nullptr;
+  wb_detection* d_wout = nullptr;
+  uint32_t* d_wverd = nullptr;
+  int n = 0;         // frames of the batch in flight
+  bool windowed = false;
   uint32_t flags = 0;
   bool busy = false;
   int launches = 0;
-  // CUDA graph of the kernel sequence, keyed by (n, flags)
+  // CUDA graph of the kernel sequence, keyed by (model images, flags, frames, windowed)
   cudaGraphExec_t graph_exec = nullptr;
   int graph_n = -1;
+  int graph_frames = -1;
+  bool graph_windowed = false;
   uint32_t graph_flags = 0;
   int graph_src_w = 0;  // widest camera the captured stem kernel sized its staging for
 };
@@ -87,6 +94,8 @@ struct wb_ctx {
   CameraCfg* d_cams = nullptr;
   std::vector<CameraCfg> h_cams;
   std::vector<int32_t*> cam_sat;
+  std::vector<std::vector<int4>> cam_windows;  // wb_set_camera_windows: (x, y, w, h) per window
+  std::vector<double> cam_merge_thr;
   Slot slots[WB_SLOTS];
   cudaStream_t user_stream = nullptr;
   bool has_user_stream = false;
@@ -156,6 +165,11 @@ static int alloc_slot(wb_ctx* c, Slot& s) {
   CK(cudaMallocHost(&s.h_raw, sizeof(float) * (size_t)B * WB_MAX_DETECTIONS * 6));
   CK(cudaMalloc(&s.d_raw_num, sizeof(int) * B));
   CK(cudaMallocHost(&s.h_raw_num, sizeof(int) * B));
+  CK(cudaMallocHost(&s.h_win, sizeof(WindowFrame) * B));
+  CK(cudaMalloc(&s.d_win, sizeof(WindowFrame) * B));
+  CK(cudaMalloc(&s.d_wout, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(cudaMemset(s.d_wout, 0, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(cudaMalloc(&s.d_wverd, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
   return 0;
 }
 
@@ -237,6 +251,8 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   c->pp.class_offset = c->hdr.class_offset;
   c->h_cams.assign(WB_MAX_CAMERAS, CameraCfg{});
   c->cam_sat.assign(WB_MAX_CAMERAS, nullptr);
+  c->cam_windows.assign(WB_MAX_CAMERAS, {});
+  c->cam_merge_thr.assign(WB_MAX_CAMERAS, 0.5);
   CK(cudaMalloc(&c->d_cams, sizeof(CameraCfg) * WB_MAX_CAMERAS));
   CK(cudaMemset(c->d_cams, 0, sizeof(CameraCfg) * WB_MAX_CAMERAS));
   for (int s = 0; s < WB_SLOTS; ++s)
@@ -276,6 +292,10 @@ int wb_destroy(wb_ctx* c) {
     cudaFree(s.d_verdicts);
     cudaFree(s.d_raw);
     cudaFree(s.d_raw_num);
+    cudaFree(s.d_win);
+    cudaFree(s.d_wout);
+    cudaFree(s.d_wverd);
+    cudaFreeHost(s.h_win);
     cudaFreeHost(s.h_desc);
     cudaFreeHost(s.h_out);
     cudaFreeHost(s.h_verdicts);
@@ -385,7 +405,31 @@ int wb_set_camera(wb_ctx* c, int cam, int width, int height, int n_zones, const 
     cfg.sat = c->cam_sat[cam];
   }
   c->h_cams[cam] = cfg;
+  c->cam_windows[cam].clear();  // they were checked against the previous frame size
   CK(cudaMemcpy(c->d_cams + cam, &cfg, sizeof(cfg), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+int wb_set_camera_windows(wb_ctx* c, int cam, int n_windows, const int32_t* xywh, double merge_threshold) {
+  REQUIRE(c, "NULL ctx");
+  REQUIRE(cam >= 0 && cam < WB_MAX_CAMERAS, "cam_id out of range (0..255)");
+  REQUIRE(n_windows >= 0 && n_windows <= WB_MAX_WINDOWS, "a camera may have at most 16 detection windows");
+  REQUIRE(n_windows == 0 || xywh != nullptr, "xywh is NULL");
+  REQUIRE(merge_threshold >= 0.0 && merge_threshold <= 1.0, "merge_threshold must be in [0, 1]");
+  std::lock_guard<std::mutex> lock(c->mu);
+  const CameraCfg& cc = c->h_cams[cam];
+  REQUIRE(cc.width > 0, "cam_id " + std::to_string(cam) + " has not been configured with wb_set_camera");
+  std::vector<int4> wins(n_windows);
+  for (int i = 0; i < n_windows; ++i) {
+    const int x = xywh[4 * i], y = xywh[4 * i + 1], w = xywh[4 * i + 2], h = xywh[4 * i + 3];
+    REQUIRE(x >= 0 && y >= 0 && w >= 1 && h >= 1 && w <= cc.width - x && h <= cc.height - y,
+            "cam_id " + std::to_string(cam) + " window " + std::to_string(i) + " (" + std::to_string(x) + ", " +
+                std::to_string(y) + ", " + std::to_string(w) + ", " + std::to_string(h) + ") is not inside the " +
+                std::to_string(cc.width) + "x" + std::to_string(cc.height) + " frame or is empty");
+    wins[i] = make_int4(x, y, w, h);
+  }
+  c->cam_windows[cam] = wins;
+  c->cam_merge_thr[cam] = merge_threshold;
   return 0;
 }
 
@@ -543,49 +587,55 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
   return 0;
 }
 
-static int run_post(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, bool want_raw = false) {
+// windowed batch (n_frames frames in n model images): the windows' rows go to s.d_out unfiltered, with their valid row
+// counts in s.d_raw_num, and k_window_merge writes each frame's rows and verdicts to s.d_wout / s.d_wverd
+static int run_post(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, bool want_raw = false,
+                    int n_frames = 0, bool windowed = false) {
   LaunchCtx lc{st, &s.launches};
   // the float boxes / scores / classes of `sess.run` are a test hook (wb_postprocess); the product path writes
   // Detection rows only
   float* rb = want_raw ? s.d_raw : nullptr;
   float* rs = want_raw ? rb + (size_t)c->max_batch * WB_MAX_DETECTIONS * 4 : nullptr;
   float* rc = want_raw ? rs + (size_t)c->max_batch * WB_MAX_DETECTIONS : nullptr;
-  launch_post(lc, n, c->pp, s.d_enc, s.d_logits, c->tensor(c->hdr.anchors_tensor), s.d_desc, c->d_cams, flags,
-              s.d_dec, s.d_cand_count, s.d_cand, s.d_sel_count, s.d_sel, s.d_out, s.d_verdicts, rb, rs, rc,
-              want_raw ? s.d_raw_num : nullptr, s.d_kept_hist);
+  launch_post(lc, n, c->pp, s.d_enc, s.d_logits, c->tensor(c->hdr.anchors_tensor), s.d_desc,
+              windowed ? nullptr : c->d_cams, flags, s.d_dec, s.d_cand_count, s.d_cand, s.d_sel_count, s.d_sel, s.d_out,
+              s.d_verdicts, rb, rs, rc, (want_raw || windowed) ? s.d_raw_num : nullptr, s.d_kept_hist);
+  if (windowed)
+    launch_window_merge(lc, n_frames, c->pp, s.d_win, s.d_out, s.d_raw_num, c->d_cams, flags, s.d_wout, s.d_wverd);
   CK(cudaGetLastError());
   return 0;
 }
 
-static int run_all(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags) {
+static int run_all(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, int n_frames, bool windowed) {
   int rc = c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, n, nullptr, 0, -1)
                              : run_layers<float>(c, s, st, n, nullptr, 0, -1);
   if (rc) return rc;
-  return run_post(c, s, st, n, flags);
+  return run_post(c, s, st, n, flags, false, n_frames, windowed);
 }
 
 // kernels of one batch, through a CUDA graph when possible (launch-bound at small batch).  The pixel format is not part
 // of the graph's key: the kernels read it from the frame descriptors, which fill_desc copies to the device before every
 // launch, so one graph serves RGB24 and 4:2:0 batches alike.
-static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags) {
+static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, int n_frames, bool windowed) {
   const uint32_t gflags = flags & WB_F_FUSE_FILTERS;
   if (!c->use_graph) {
     s.launches = 0;
-    return run_all(c, s, st, n, gflags);
+    return run_all(c, s, st, n, gflags, n_frames, windowed);
   }
-  if (s.graph_exec == nullptr || s.graph_n != n || s.graph_flags != gflags || s.graph_src_w != c->max_src_w) {
+  if (s.graph_exec == nullptr || s.graph_n != n || s.graph_flags != gflags || s.graph_src_w != c->max_src_w ||
+      s.graph_frames != n_frames || s.graph_windowed != windowed) {
     if (s.graph_exec) {
       cudaGraphExecDestroy(s.graph_exec);
       s.graph_exec = nullptr;
     }
     // warm-up run outside capture (sets function attributes, validates launches)
     s.launches = 0;
-    if (int rc = run_all(c, s, st, n, gflags)) return rc;
+    if (int rc = run_all(c, s, st, n, gflags, n_frames, windowed)) return rc;
     CK(cudaStreamSynchronize(st));
     cudaGraph_t graph = nullptr;
     CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     s.launches = 0;
-    int rc = run_all(c, s, st, n, gflags);
+    int rc = run_all(c, s, st, n, gflags, n_frames, windowed);
     cudaError_t e = cudaStreamEndCapture(st, &graph);
     if (rc) return rc;
     if (e != cudaSuccess) return fail(std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e));
@@ -594,6 +644,8 @@ static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t 
     s.graph_n = n;
     s.graph_flags = gflags;
     s.graph_src_w = c->max_src_w;
+    s.graph_frames = n_frames;
+    s.graph_windowed = windowed;
   }
   CK(cudaGraphLaunch(s.graph_exec, st));
   return 0;
@@ -606,9 +658,16 @@ static int frame_format(uint32_t flags, int* fmt) {
   return 0;
 }
 
+// One descriptor per model image.  With use_windows and at least one camera of the batch having detection windows, the
+// batch is windowed: every window of a frame is one image (a camera without windows: one full-frame window, camera
+// -1), and s.h_win / s.d_win describe the frames for k_window_merge.  Otherwise an image is a frame, as always.  A host
+// frame is copied to the device once, whatever its window count; the windows point into that copy (or into the
+// caller's device frame).
 static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, const int32_t* cam_ids,
-                     bool on_device, int fmt, cudaStream_t st) {
+                     bool on_device, int fmt, cudaStream_t st, bool use_windows, int* n_images_out) {
   size_t total = 0;
+  bool windowed = false;
+  int n_images = 0;
   for (int i = 0; i < n; ++i) {
     int cam = cam_ids[i];
     REQUIRE(cam >= 0 && cam < WB_MAX_CAMERAS && c->h_cams[cam].width > 0,
@@ -619,7 +678,20 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
             "cam_id " + std::to_string(cam) + " is " + std::to_string(cc.width) + "x" + std::to_string(cc.height) +
                 ": 4:2:0 frames need an even width and height");
     total += (frame_bytes(fmt, cc.width, cc.height) + 255) / 256 * 256;
+    const int nw = use_windows ? (int)c->cam_windows[cam].size() : 0;
+    windowed |= nw > 0;
+    n_images += std::max(nw, 1);
+    for (int k = 0; k < nw; ++k) {
+      const int4 wd = c->cam_windows[cam][k];
+      REQUIRE(fmt == WB_FMT_RGB24 || (wd.x % 2 == 0 && wd.y % 2 == 0 && wd.z % 2 == 0 && wd.w % 2 == 0),
+              "cam_id " + std::to_string(cam) + " window " + std::to_string(k) + " (" + std::to_string(wd.x) + ", " +
+                  std::to_string(wd.y) + ", " + std::to_string(wd.z) + ", " + std::to_string(wd.w) +
+                  "): 4:2:0 frames need an even window origin, width and height");
+    }
   }
+  REQUIRE(n_images <= c->max_batch, "the batch's detection windows add up to " + std::to_string(n_images) +
+                                        " model images, more than max_batch (" + std::to_string(c->max_batch) + ")");
+  if (!windowed) n_images = n;
   if (!on_device && frames != nullptr && total > s.d_frames_cap) {
     CK(cudaStreamSynchronize(st));
     if (s.d_frames) CK(cudaFree(s.d_frames));
@@ -627,26 +699,54 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
     CK(cudaMalloc(&s.d_frames, s.d_frames_cap));
   }
   size_t off = 0;
+  int img = 0;
   for (int i = 0; i < n; ++i) {
-    const CameraCfg& cc = c->h_cams[cam_ids[i]];
-    size_t bytes = frame_bytes(fmt, cc.width, cc.height);
-    FrameDesc d;
-    d.w = cc.width;
-    d.h = cc.height;
-    d.cam = cam_ids[i];
-    d.fmt = fmt;
-    if (frames == nullptr) {
-      d.ptr = nullptr;
-    } else if (on_device) {
-      d.ptr = frames[i];
-    } else {
-      d.ptr = s.d_frames + off;
+    const int cam = cam_ids[i];
+    const CameraCfg& cc = c->h_cams[cam];
+    const size_t bytes = frame_bytes(fmt, cc.width, cc.height);
+    const uint8_t* base = nullptr;
+    if (frames != nullptr && on_device) {
+      base = frames[i];
+    } else if (frames != nullptr) {
+      base = s.d_frames + off;
       CK(cudaMemcpyAsync(s.d_frames + off, frames[i], bytes, cudaMemcpyHostToDevice, st));
       off += (bytes + 255) / 256 * 256;
     }
-    s.h_desc[i] = d;
+    const ChromaLayout cl = chroma_layout(fmt, cc.width, cc.height);
+    const int bpp = fmt == WB_FMT_RGB24 ? 3 : 1;  // bytes per pixel of the RGB24 / luma plane
+    const std::vector<int4>& wins = c->cam_windows[cam];
+    const int nw = windowed ? std::max((int)wins.size(), 1) : 1;
+    if (windowed) {
+      WindowFrame& wf = s.h_win[i];
+      wf.first = img;
+      wf.count = nw;
+      wf.cam = cam;
+      wf._pad = 0;
+      wf.merge_thr = wins.empty() ? 0.5 : c->cam_merge_thr[cam];
+    }
+    for (int k = 0; k < nw; ++k) {
+      const int4 wd = (windowed && !wins.empty()) ? wins[k] : make_int4(0, 0, cc.width, cc.height);
+      FrameDesc d;
+      d.ptr = base ? base + ((size_t)wd.y * cc.width + wd.x) * bpp : nullptr;
+      d.chroma = base ? base + (size_t)cc.width * cc.height + (size_t)(wd.y >> 1) * cl.row + (size_t)(wd.x >> 1) * cl.step
+                      : nullptr;
+      d.w = wd.z;
+      d.h = wd.w;
+      d.pitch = cc.width * bpp;
+      d.cam = windowed ? -1 : cam;
+      d.fmt = fmt;
+      d.v_off = (int32_t)cl.v_off;
+      if (windowed) {
+        s.h_win[i].x[k] = wd.x;
+        s.h_win[i].y[k] = wd.y;
+      }
+      s.h_desc[img++] = d;
+    }
   }
-  CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n_images, cudaMemcpyHostToDevice, st));
+  if (windowed) CK(cudaMemcpyAsync(s.d_win, s.h_win, sizeof(WindowFrame) * n, cudaMemcpyHostToDevice, st));
+  s.windowed = windowed;
+  if (n_images_out) *n_images_out = n_images;
   return 0;
 }
 
@@ -664,13 +764,15 @@ int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const in
   int fmt = WB_FMT_RGB24;
   if (int rc = frame_format(flags, &fmt)) return rc;
   CK(cudaEventRecord(s.ev0, st));
-  if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st)) return rc;
-  if (int rc = enqueue_kernels(c, s, st, n, flags)) return rc;
+  int n_images = n;
+  if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &n_images))
+    return rc;
+  if (int rc = enqueue_kernels(c, s, st, n_images, flags, n, s.windowed)) return rc;
   if (!(flags & WB_F_OUT_ON_DEVICE)) {
-    CK(cudaMemcpyAsync(s.h_out, s.d_out, sizeof(wb_detection) * (size_t)n * WB_MAX_DETECTIONS,
+    CK(cudaMemcpyAsync(s.h_out, s.windowed ? s.d_wout : s.d_out, sizeof(wb_detection) * (size_t)n * WB_MAX_DETECTIONS,
                        cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(s.h_verdicts, s.d_verdicts, sizeof(uint32_t) * (size_t)n * WB_MAX_DETECTIONS,
-                       cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(s.h_verdicts, s.windowed ? s.d_wverd : s.d_verdicts,
+                       sizeof(uint32_t) * (size_t)n * WB_MAX_DETECTIONS, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaEventRecord(s.ev1, st));
   s.n = n;
@@ -694,12 +796,14 @@ int wb_collect(wb_ctx* c, int slot, wb_detection* const* out, uint32_t* const* v
   if (gpu_ms) CK(cudaEventElapsedTime(gpu_ms, s.ev0, s.ev1));
   if (s.flags & WB_F_OUT_ON_DEVICE) {
     cudaStream_t st = c->stream_of(slot);
+    const wb_detection* d_out = s.windowed ? s.d_wout : s.d_out;
+    const uint32_t* d_verd = s.windowed ? s.d_wverd : s.d_verdicts;
     for (int i = 0; i < s.n; ++i) {
       if (out && out[i])
-        CK(cudaMemcpyAsync(out[i], s.d_out + (size_t)i * WB_MAX_DETECTIONS, sizeof(wb_detection) * WB_MAX_DETECTIONS,
+        CK(cudaMemcpyAsync(out[i], d_out + (size_t)i * WB_MAX_DETECTIONS, sizeof(wb_detection) * WB_MAX_DETECTIONS,
                            cudaMemcpyDeviceToDevice, st));
       if (verdicts && verdicts[i])
-        CK(cudaMemcpyAsync(verdicts[i], s.d_verdicts + (size_t)i * WB_MAX_DETECTIONS,
+        CK(cudaMemcpyAsync(verdicts[i], d_verd + (size_t)i * WB_MAX_DETECTIONS,
                            sizeof(uint32_t) * WB_MAX_DETECTIONS, cudaMemcpyDeviceToDevice, st));
     }
     CK(cudaStreamSynchronize(st));
@@ -761,7 +865,8 @@ int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t*
   for (int i = 0; i < n; ++i) {
     size_t bytes = (size_t)widths[i] * heights[i] * 3;
     CK(cudaMemcpyAsync(s.d_frames + off, frames[i], bytes, cudaMemcpyHostToDevice, st));
-    s.h_desc[i] = FrameDesc{s.d_frames + off, widths[i], heights[i], -1, WB_FMT_RGB24};
+    s.h_desc[i] = FrameDesc{s.d_frames + off, s.d_frames + off + (size_t)widths[i] * heights[i], widths[i], heights[i],
+                            widths[i] * 3, -1, WB_FMT_RGB24, 0};
     off += bytes;
   }
   CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n, cudaMemcpyHostToDevice, st));
@@ -833,7 +938,7 @@ int wb_postprocess(wb_ctx* c, int n, const float* enc, const float* logits, cons
   const int NA = c->hdr.num_anchors, C1 = c->hdr.num_classes + 1;
   CK(cudaMemcpyAsync(s.d_enc, enc, sizeof(float) * (size_t)n * NA * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(s.d_logits, logits, sizeof(float) * (size_t)n * NA * C1, cudaMemcpyHostToDevice, st));
-  if (int rc = fill_desc(c, s, n, nullptr, cam_ids, false, WB_FMT_RGB24, st)) return rc;
+  if (int rc = fill_desc(c, s, n, nullptr, cam_ids, false, WB_FMT_RGB24, st, false, nullptr)) return rc;
   s.launches = 0;
   if (int rc = run_post(c, s, st, n, flags, true)) return rc;
   const size_t B = c->max_batch;
@@ -891,7 +996,7 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
   Slot& s = c->slots[0];
   REQUIRE(!s.busy, "slot 0 is busy");
   cudaStream_t st = c->stream_of(0);
-  if (int rc = fill_desc(c, s, n, device_frames, cam_ids, true, WB_FMT_RGB24, st)) return rc;
+  if (int rc = fill_desc(c, s, n, device_frames, cam_ids, true, WB_FMT_RGB24, st, false, nullptr)) return rc;
   const int nl = (int)c->layers.size();
   REQUIRE(max_launches >= nl + 1, "max_launches too small");
   std::vector<cudaEvent_t> ev(nl + 2);
@@ -900,7 +1005,7 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
   // never write their own input), so host launch gaps do not leak into the per-kernel time
   const int REPS = 10;
   s.launches = 0;
-  if (int rc = run_all(c, s, st, n, 0)) return rc;  // warm-up, also fills every activation buffer
+  if (int rc = run_all(c, s, st, n, 0, n, false)) return rc;  // warm-up, also fills every activation buffer
   s.launches = 0;
   CK(cudaEventRecord(ev[0], st));
   for (int li = 0; li < nl; ++li) {

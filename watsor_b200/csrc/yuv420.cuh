@@ -32,18 +32,18 @@ __host__ __device__ __forceinline__ size_t frame_bytes(int fmt, int w, int h) {
   return fmt == WB_FMT_RGB24 ? (size_t)w * h * 3 : (size_t)w * h * 3 / 2;
 }
 
-// address of the U sample of pixel (x, y); the V sample is at + v_off
-__device__ __forceinline__ const uint8_t* chroma_ptr(const uint8_t* frame, int w, int h, const ChromaLayout& cl, int x,
-                                                     int y) {
-  return frame + (size_t)w * h + (size_t)(y >> 1) * cl.row + (size_t)(x >> 1) * cl.step;
+// address of the U sample of pixel (x, y) given that of pixel (0, 0); the V sample is at + v_off.  A window of a frame
+// (x0, y0 even) has its own origin `chroma` and keeps the parent frame's layout.
+__device__ __forceinline__ const uint8_t* chroma_ptr(const uint8_t* chroma, const ChromaLayout& cl, int x, int y) {
+  return chroma + (size_t)(y >> 1) * cl.row + (size_t)(x >> 1) * cl.step;
 }
 
-// Y, U, V bytes of pixel (x, y); yuv_to_rgb below converts them (two halves, so that a caller can have the loads of
-// several pixels in flight before it converts any)
-__device__ __forceinline__ void yuv420_load(const uint8_t* __restrict__ frame, int w, int h, const ChromaLayout& cl,
-                                            int x, int y, uint32_t& Y, uint32_t& U, uint32_t& V) {
-  const uint8_t* c = chroma_ptr(frame, w, h, cl, x, y);
-  Y = __ldg(frame + (size_t)y * w + x);
+// Y, U, V bytes of pixel (x, y) of the frame whose luma rows start at `luma`, `pitch` bytes apart; yuv_to_rgb below
+// converts them (two halves, so that a caller can have the loads of several pixels in flight before it converts any)
+__device__ __forceinline__ void yuv420_load(const uint8_t* __restrict__ luma, int pitch, const uint8_t* __restrict__ chroma,
+                                            const ChromaLayout& cl, int x, int y, uint32_t& Y, uint32_t& U, uint32_t& V) {
+  const uint8_t* c = chroma_ptr(chroma, cl, x, y);
+  Y = __ldg(luma + (size_t)y * pitch + x);
   U = __ldg(c);
   V = __ldg(c + cl.v_off);
 }

@@ -90,9 +90,15 @@ class B200ObjectDetector(object):
     # ------------------------------------------------------------------ batched API
     def configure_camera(self, cam_id, width, height, camera_config=None):
         """Per-camera filter state (main.py:294-299 builds the same from the camera dict):
-        `camera_config` = {'width','height','detect':[{label:{confidence,area,zones}}],['mask']}."""
+        `camera_config` = {'width','height','detect':[{label:{confidence,area,zones}}],['mask']}.
+        Optional keys: 'windows', a list of [x, y, w, h] detection windows in the camera's pixels (e.g.
+        watsor_b200.windows.grid_windows), and 'window_merge_threshold' (default 0.5), see Engine.set_camera_windows."""
         rasters, filters = camera_tables(camera_config, width, height)
         self.engine.set_camera(cam_id, width, height, rasters, filters)
+        windows = (camera_config or {}).get('windows')
+        if windows:
+            self.engine.set_camera_windows(cam_id, [tuple(w) for w in windows],
+                                           camera_config.get('window_merge_threshold', 0.5))
 
     def register_frame_buffer(self, frame_buffer):
         """Pin the shared-memory images of a FrameBuffer (share.py:76-81) for async H2D."""

@@ -32,6 +32,11 @@ from .b200 import COMPILED_MODEL, MODEL_FILES
 from .devices import b200_gpus
 
 
+def max_windows(camera_configs):
+    """The largest number of detection windows of any camera (1 without any): a frame's model images."""
+    return max([len((cfg or {}).get('windows') or ()) for cfg in (camera_configs or {}).values()] + [1])
+
+
 def has_model(model_path):
     return any(path.isfile(path.join(model_path, f)) for f in (COMPILED_MODEL,) + MODEL_FILES)
 
@@ -124,7 +129,8 @@ class ObjectDetector(Work):
     #    result write-back / latch hand-over of tick k-1 and the queue drain of tick k+1
     def _process(self, frame_queue, *args, **kwargs):
         object_detector = args[-1]
-        limit = getattr(object_detector, 'max_batch', 1)
+        # max_batch counts model images: a camera with detection windows makes one per window
+        limit = max(1, getattr(object_detector, 'max_batch', 1) // max_windows(kwargs.get('camera_configs')))
         payloads = []
         busy = bool(getattr(self, '_in_flight', None))
         try:

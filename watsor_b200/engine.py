@@ -10,6 +10,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import ClassFilter, check
+from .windows import check_windows
 from .stream.share import MAX_DETECTIONS, Detection
 
 # 0: fp32 CUDA-core convs; 1: bf16 wgmma; 2: fp32 storage, dense convs as 3xTF32 wgmma (fp32-faithful)
@@ -87,6 +88,7 @@ class Engine:
         self.input_h, self.input_w = ih.value, iw.value
         self.num_classes, self.num_anchors, self.num_layers = nc.value, na.value, nl.value
         self.cameras = {}
+        self.windows = {}                       # cam_id -> [(x, y, w, h)] (set_camera_windows)
 
     # ------------------------------------------------------------------ life cycle
     def close(self):
@@ -136,6 +138,24 @@ class Engine:
         check(self.lib.wb_set_camera(self._ctx, cam_id, width, height, n_zones, raster_ptr,
                                      len(class_filters), arr, flags))
         self.cameras[cam_id] = (width, height)
+        self.windows.pop(cam_id, None)          # the library clears them too: the frame size may have changed
+
+    def set_camera_windows(self, cam_id, windows, merge_threshold=0.5):
+        """Detection windows of a configured camera: (x, y, w, h) rectangles in its pixels (see windows.grid_windows),
+        each of which becomes one model image per frame; max_batch counts model images.  The windows' rows are merged
+        into the frame's 100 rows: a row is dropped when a kept row of the same label from another window covers more
+        than `merge_threshold` of the smaller box.  An empty list removes the windows."""
+        if cam_id not in self.cameras:
+            raise ValueError('camera %r has not been configured with set_camera' % (cam_id,))
+        windows = check_windows(windows, *self.cameras[cam_id])
+        if not 0.0 <= merge_threshold <= 1.0:
+            raise ValueError('merge_threshold must be in [0, 1], not %r' % (merge_threshold,))
+        xywh = (c_int32 * max(1, 4 * len(windows)))(*[v for win in windows for v in win])
+        check(self.lib.wb_set_camera_windows(self._ctx, cam_id, len(windows), xywh, float(merge_threshold)))
+        if windows:
+            self.windows[cam_id] = windows
+        else:
+            self.windows.pop(cam_id, None)
 
     def register_host(self, address, nbytes):
         check(self.lib.wb_register_host(self._ctx, address, nbytes))
@@ -155,6 +175,9 @@ class Engine:
 
     def _format_flags(self, frames, cam_ids, pixel_format):
         check_frames(frames, [self.cameras.get(c) for c in cam_ids], pixel_format)
+        for c in set(cam_ids):
+            if c in self.windows:
+                check_windows(self.windows[c], *self.cameras[c], pixel_format)
         return PIXEL_FORMATS[pixel_format]
 
     def detect(self, frames, cam_ids, out, verdicts=None, flags=0, pixel_format='rgb24'):
