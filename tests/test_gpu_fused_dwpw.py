@@ -89,3 +89,27 @@ def test_block_fused_equals_unfused(hw, stride, C, N, residual, n):
     assert launches_u - launches_f == 1
     assert np.array_equal(y_f, y_u)
     assert np.abs(y_f).max() > 0
+    # and both are right: float64 depthwise -> projection [-> Add] on the depthwise layer's GPU input
+    from tests import layer_reference as R
+    (_, _, e), _ = _run(m.to_blob(), pre, False, stop_layer=1, layer_shape=(hw, hw, C))
+    e = e.astype(np.float64)
+    dw, pw = m.layers[2], m.layers[3]
+
+    def vec(L, t):
+        return np.asarray(m.tensors[t], np.float64)[:L.out_c]
+
+    wd = np.asarray(m.tensors[dw.w_tensor], np.float64).reshape(3, 3, C)
+    zd, Pd = R.depthwise(e, wd, stride), R.depthwise(np.abs(e), np.abs(wd), stride)
+    d = R.affine(zd, vec(dw, dw.scale_tensor), vec(dw, dw.offset_tensor), dw.act)
+    bd = R.chain_bound(Pd, zd * vec(dw, dw.scale_tensor), d, vec(dw, dw.scale_tensor), vec(dw, dw.offset_tensor), 9)
+    wp = np.asarray(m.tensors[pw.w_tensor], np.float64).reshape(C, pw.n_pad)[:, :N]
+    sp, op = vec(pw, pw.scale_tensor), vec(pw, pw.offset_tensor)
+    z, P = d @ wp, (np.abs(d) + bd) @ np.abs(wp)
+    want = R.affine(z, sp, op, pw.act)
+    # the projection's own bound (tf32x3, no split below 16 k-blocks) plus the depthwise error carried through it
+    bound = R.dense_bound(P, z * sp, want, sp, op, 2, k_blocks=-(-C // 32)) + (bd @ np.abs(wp)) * np.abs(sp) * (1 + 1e-6)
+    if residual:
+        (_, _, x), _ = _run(m.to_blob(), pre, False, stop_layer=0, layer_shape=(hw, hw, N))
+        want = want + x
+        bound = bound + R.U * (np.abs(want) + bound)
+    assert np.all(np.abs(y_f - want) <= bound), float(np.max(np.abs(y_f - want) / bound))

@@ -31,7 +31,10 @@ CASES = [(512, 512, 19, 4), (32, 64, 32, 2), (1024, 1024, 10, 8), (256, 48, 3, 1
          (128, 96, 7, 2), (16, 16, 5, 1),
          # more output tiles than SMs; the last row tile is partial in each (M = 22500, 28125, 20172) and
          # 256 columns make two N tiles
-         (32, 64, 150, 1), (64, 128, 75, 5), (128, 256, 41, 12), (24, 128, 150, 2)]
+         (32, 64, 150, 1), (64, 128, 75, 5), (128, 256, 41, 12), (24, 128, 150, 2),
+         # split-K clusters of 4, 3 (ragged N), 5 (the last k-block holds 20 of 32 values and the last split is
+         # shorter) and 8 members (the portable cluster limit) on 132 SMs
+         (1024, 128, 7, 1), (768, 96, 19, 2), (1300, 48, 10, 1), (2048, 64, 10, 1)]
 
 
 @pytest.mark.parametrize('precision,rel_tol', [(2, 3e-6), (3, 4e-3), (1, 1.5e-2)],

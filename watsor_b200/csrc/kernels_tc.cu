@@ -454,8 +454,12 @@ int pick_block_n(int n_pad) { return n_pad <= 32 ? 32 : (n_pad <= 64 ? 64 : 128)
 
 }  // namespace
 
-bool tc_layer_supported(const wb_layer& L) {
-  if ((L.op == WB_OP_PW || L.op == WB_OP_HEAD) && L.kh == 1 && L.kw == 1 && L.stride == 1 && L.in_c % 4 == 0) return true;
+bool tc_layer_supported(const wb_layer& L, int mode) {
+  // 1x1: the activation and weight rows are K-major tensor maps, whose row stride must be a multiple of 16 bytes
+  // (K % 4 in fp32, K % 8 in bf16)
+  const int elem = mode == TC_BF16 ? 2 : 4;
+  if ((L.op == WB_OP_PW || L.op == WB_OP_HEAD) && L.kh == 1 && L.kw == 1 && L.stride == 1 && (L.in_c * elem) % 16 == 0)
+    return true;
   // KxK / strided dense convolutions (the SSD extra layers): implicit GEMM, one filter tap x 32 (64 bf16) channels
   // per k-block; a CTA's tile is a whole number of output images, so the maps must be small (<= 128 pixels)
   return L.op == WB_OP_CONV && L.in_c % 64 == 0 && L.out_h * L.out_w <= (uint32_t)BLOCK_M && L.stride <= 8 &&
@@ -468,7 +472,7 @@ int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb
   out->layers.assign(layers.size(), TcLayerWeights{});
   for (size_t li = 0; li < layers.size(); ++li) {
     const wb_layer& L = layers[li];
-    if (!tc_layer_supported(L)) continue;
+    if (!tc_layer_supported(L, mode)) continue;
     TcLayerWeights& w = out->layers[li];
     const int K = L.kh * L.kw * L.in_c, NP = L.n_pad;             // conv: k = tap * in_c + channel
     const float* src = host_data + tensors[L.w_tensor].offset;  // [K][NP]

@@ -21,7 +21,8 @@ struct TcWeights {
   std::vector<TcLayerWeights> layers;  // indexed by layer number (unset entries for non-GEMM layers)
 };
 
-bool tc_layer_supported(const wb_layer& L);
+// whether the tensor-core GEMM of operand mode `mode` (TcMode) runs layer L
+bool tc_layer_supported(const wb_layer& L, int mode);
 int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb_tensor_entry>& tensors,
                        const float* host_data, int mode, TcWeights* out, std::string* err);
 void tc_free_weights(TcWeights* w);

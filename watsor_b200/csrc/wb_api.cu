@@ -498,7 +498,7 @@ static Span fused_span(const wb_ctx* c, size_t li, size_t end) {
       }
     }
   }
-  if (L.op == WB_OP_PW && c->precision != 0 && tc_layer_supported(L) && residual_add_after(li) &&
+  if (L.op == WB_OP_PW && c->precision != 0 && tc_layer_supported(L, c->tc.mode) && residual_add_after(li) &&
       arena_disjoint(L, Ls[li + 1]))
     return {li + 1, SPAN_PW_ADD};
   return {li, SPAN_ONE};
@@ -558,7 +558,7 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
       case WB_OP_PW:
       case WB_OP_CONV:
       case WB_OP_HEAD:
-        if (c->precision != 0 && tc_layer_supported(L)) {
+        if (c->precision != 0 && tc_layer_supported(L, c->tc.mode)) {
           // MobileNet-v2 bottleneck: a linear projection followed by `Add(shortcut, projection)` runs as one kernel,
           // the shortcut is added in the GEMM epilogue (fp32 modes) and the Add layer is skipped
           const void* residual = nullptr;
