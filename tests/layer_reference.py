@@ -222,7 +222,7 @@ CC_SPLIT_TILES, CC_SPLIT_CTAS = 120, 296      # launch_gemm_cc: split below 120 
 
 # every branch of every gate that plan() can report; a test case has to claim each of them
 BRANCHES = frozenset(
-    ['stem:3x3s2_c32', 'stem:generic', 'dw:strip_s1', 'dw:strip_s2', 'dw:generic',
+    ['stem:3x3s2_c32', 'stem:generic', 'dw:strip_s1', 'dw:strip_s2',
      'tc:pw', 'tc:head', 'tc:conv', 'tc:unsupported_conv', 'tc:unsupported_1x1', 'tc:bn32', 'tc:bn64', 'tc:bn128',
      'tc:no_split_tiles', 'tc:no_split_kblocks', 'tc:no_split_env'] +
     ['tc:split%d' % s for s in range(2, 9)] +
@@ -261,9 +261,9 @@ def plan(L, n, precision, sms, env=(), fuse_add_next=False):
         return dict(kernel='k_stem_3x3s2_c32' if big else 'k_stem', launches=1,
                     branches={'stem:3x3s2_c32' if big else 'stem:generic'})
     if L.op == OP_DW:
-        if L.stride in (1, 2) and L.out_w >= 4:
-            return dict(kernel='k_dw_strip', stride=L.stride, launches=1, branches={'dw:strip_s%d' % L.stride})
-        return dict(kernel='k_dw', launches=1, branches={'dw:generic'})
+        if L.stride not in (1, 2):
+            raise ValueError('wb_create refuses a depthwise stride of %d' % L.stride)
+        return dict(kernel='k_dw_strip', stride=L.stride, launches=1, branches={'dw:strip_s%d' % L.stride})
     if L.op in (OP_MAXPOOL, OP_AVGPOOL):
         return dict(kernel='k_pool', launches=1, branches={'pool:max' if L.op == OP_MAXPOOL else 'pool:avg'})
     if L.op == OP_ADD:

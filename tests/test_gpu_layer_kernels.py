@@ -115,13 +115,13 @@ CASES += [
     case('cc_conv3x3_10_cin48_n1', 'cc', ('gemm', 10, 48, 64, 3, 1, ACT_NONE), 1, (2,), {'all': {'kernel': 'k_gemm_cc'}}),
     case('cc_conv3x3_10_cin48_n3', 'cc', ('gemm', 10, 48, 64, 3, 1, ACT_NONE), 3, (2, 0), {'all': {'kernel': 'k_gemm_cc'}}),
 ]
-# depthwise 3x3 -- ('dw', hw, C, stride); out_w mod 4 = 3, 2, 1, 0 on the strip kernel, maps under 4 px on k_dw
-for hw, s, kern in ((19, 1, 'k_dw_strip'), (38, 1, 'k_dw_strip'), (9, 1, 'k_dw_strip'), (12, 1, 'k_dw_strip'),
-                    (75, 2, 'k_dw_strip'), (19, 2, 'k_dw_strip'), (9, 2, 'k_dw_strip'), (14, 2, 'k_dw_strip'),
-                    (3, 2, 'k_dw'), (2, 2, 'k_dw'), (3, 1, 'k_dw')):
+# depthwise 3x3 -- ('dw', hw, C, stride); out_w mod 4 = 3, 2, 1, 0, and maps narrower than one 4-pixel strip (the
+# strip kernel's bounds-checked column loads and its stores that stop at out_w)
+for hw, s in ((19, 1), (38, 1), (9, 1), (12, 1), (75, 2), (19, 2), (9, 2), (14, 2), (3, 2), (2, 2), (3, 1)):
     for n in (1, 3):
-        CASES.append(case('dw_%d_s%d_n%d' % (hw, s, n), 'dw', ('dw', hw, 48 if hw % 2 else 32, s), n, (0, 1),
-                          {'all': {'kernel': kern}}))
+        name = ('dw_narrow_%d_s%d_n%d' if hw < 4 else 'dw_%d_s%d_n%d') % (hw, s, n)
+        CASES.append(case(name, 'dw', ('dw', hw, 48 if hw % 2 else 32, s), n, (0, 1),
+                          {'all': {'kernel': 'k_dw_strip', 'stride': s}}))
 # pooling, bit-exact -- ('pool', hw, C, k, stride, kind)
 for hw in (75, 38, 19, 10, 2):
     for s in (1, 2):
@@ -329,8 +329,6 @@ def test_layer_kernel(c, precision):
         last -= 1
     tested = kernels[last]
     assert R.kernel_name_pattern(p, bf16) in tested[0], (tested, p, names)
-    if p['kernel'] == 'k_dw':
-        assert not any('k_dw_strip' in k for k in names)
     if p['kernel'] == 'k_gemm_tc' and tested[1] is not None:
         assert tested[1][2] == p['splits'], (tested, p)
 

@@ -114,13 +114,11 @@ struct LaunchCtx {
 };
 
 void launch_preprocess_f32(const LaunchCtx& lc, const FrameDesc* frames, int n, float* out, int oh, int ow,
-                           float mul, float sub, int max_src_w);
-// max_src_w: widest source frame the launch may see (sizes the shared-memory staging of source rows; frames that do
-// not fit take the direct path inside the kernel); 0 = never stage
+                           float mul, float sub);
 template <typename T>
 void launch_stem(const LaunchCtx& lc, const FrameDesc* frames, const float* pre, int n, const wb_layer& L,
                  int in_h, int in_w, float mul, float sub, const float* w, const float* scale,
-                 const float* offset, T* out, int max_src_w);
+                 const float* offset, T* out);
 template <typename T>
 void launch_dw(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, const float* w, const float* scale,
                const float* offset, T* out);
@@ -130,18 +128,6 @@ template <typename T>
 void launch_pool(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, T* out);
 template <typename T>
 void launch_copy_channels(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, T* out);
-struct SplitKReduceArgs {
-  const float* partial;  // [splits][M][ld] raw accumulators
-  const float* scale;
-  const float* offset;
-  void* out;  // fp32 or bf16 [M][N]
-  int out_is_bf16;
-  float* enc;
-  float* logits;
-  int M, N, ld, splits, act;
-  int is_head, anchors_per_loc, row_off, n_box, num_anchors, ncp1, hw;
-};
-void launch_splitk_reduce(const LaunchCtx& lc, const SplitKReduceArgs& r);
 template <typename T>
 void launch_gemm_cc(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, const float* w,
                     const float* scale, const float* offset, T* out, float* enc, float* logits,

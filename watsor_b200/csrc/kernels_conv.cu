@@ -10,50 +10,9 @@
 #include "common.cuh"
 
 // ---------------------------------------------------------------------------------------------------
-// depthwise 3x3 (any stride) + affine + ReLU6; one thread per (pixel, 4 channels)
-template <typename T>
-__global__ void __launch_bounds__(256)
-    k_dw(int n, wb_layer L, const T* __restrict__ in, const float* __restrict__ w, const float* __restrict__ scale,
-         const float* __restrict__ offset, T* __restrict__ out) {
-  const int c4n = L.out_c >> 2;
-  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  size_t total = (size_t)n * L.out_h * L.out_w * c4n;
-  if (idx >= total) return;
-  int c = (int)(idx % c4n) * 4;
-  size_t p = idx / c4n;
-  int ox = (int)(p % L.out_w);
-  p /= L.out_w;
-  int oy = (int)(p % L.out_h);
-  int f = (int)(p / L.out_h);
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  const T* base = in + (size_t)f * L.in_h * L.in_w * L.in_c + c;
-  const int iy0 = oy * (int)L.stride - (int)L.pad_t, ix0 = ox * (int)L.stride - (int)L.pad_l;
-#pragma unroll
-  for (int ky = 0; ky < 3; ++ky) {
-    int iy = iy0 + ky;
-    if (iy < 0 || iy >= (int)L.in_h) continue;
-#pragma unroll
-    for (int kx = 0; kx < 3; ++kx) {
-      int ix = ix0 + kx;
-      if (ix < 0 || ix >= (int)L.in_w) continue;
-      float4 x = ActIO<T>::ld4(base + ((size_t)iy * L.in_w + ix) * L.in_c);
-      float4 ww = __ldg(reinterpret_cast<const float4*>(w + (ky * 3 + kx) * L.out_c + c));
-      acc.x = fmaf(x.x, ww.x, acc.x);
-      acc.y = fmaf(x.y, ww.y, acc.y);
-      acc.z = fmaf(x.z, ww.z, acc.z);
-      acc.w = fmaf(x.w, ww.w, acc.w);
-    }
-  }
-  float4 s = __ldg(reinterpret_cast<const float4*>(scale + c));
-  float4 o = __ldg(reinterpret_cast<const float4*>(offset + c));
-  float4 v = make_float4(affine_rn(acc.x, s.x, o.x), affine_rn(acc.y, s.y, o.y), affine_rn(acc.z, s.z, o.z),
-                         affine_rn(acc.w, s.w, o.w));
-  if (L.act == WB_ACT_RELU6) v = make_float4(relu6f(v.x), relu6f(v.y), relu6f(v.z), relu6f(v.w));
-  ActIO<T>::st4(out + idx * 4, v);
-}
-
-// strip variant: one thread = 4 consecutive output pixels x 4 channels; the (4-1)*S+3 input columns
-// of a row are loaded once and reused by the four outputs (2x fewer loads at stride 1)
+// depthwise 3x3, stride S = 1 or 2 (wb_create refuses others), + affine + ReLU6; one thread = 4 consecutive output
+// pixels x 4 channels; the (4-1)*S+3 input columns of a row are loaded once and reused by the four outputs (2x fewer
+// loads at stride 1).  Columns outside the input are zeros, and outputs beyond out_w are not stored, so any width works.
 template <typename T, int S>
 __global__ void __launch_bounds__(256)
     k_dw_strip(int n, wb_layer L, const T* __restrict__ in, const float* __restrict__ w, const float* __restrict__ scale,
@@ -116,18 +75,12 @@ __global__ void __launch_bounds__(256)
 template <typename T>
 void launch_dw(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, const float* w, const float* scale,
                const float* offset, T* out) {
-  if ((L.stride == 1 || L.stride == 2) && L.out_w >= 4) {
-    size_t total = (size_t)n * L.out_h * ((L.out_w + 3) >> 2) * (L.out_c >> 2);
-    unsigned blocks = (unsigned)((total + 255) / 256);
-    if (L.stride == 1)
-      k_dw_strip<T, 1><<<blocks, 256, 0, lc.stream>>>(n, L, in, w, scale, offset, out);
-    else
-      k_dw_strip<T, 2><<<blocks, 256, 0, lc.stream>>>(n, L, in, w, scale, offset, out);
-    ++*lc.launch_counter;
-    return;
-  }
-  size_t total = (size_t)n * L.out_h * L.out_w * (L.out_c >> 2);
-  k_dw<T><<<(unsigned)((total + 255) / 256), 256, 0, lc.stream>>>(n, L, in, w, scale, offset, out);
+  size_t total = (size_t)n * L.out_h * ((L.out_w + 3) >> 2) * (L.out_c >> 2);
+  unsigned blocks = (unsigned)((total + 255) / 256);
+  if (L.stride == 1)
+    k_dw_strip<T, 1><<<blocks, 256, 0, lc.stream>>>(n, L, in, w, scale, offset, out);
+  else
+    k_dw_strip<T, 2><<<blocks, 256, 0, lc.stream>>>(n, L, in, w, scale, offset, out);
   ++*lc.launch_counter;
 }
 template void launch_dw<float>(const LaunchCtx&, int, const wb_layer&, const float*, const float*, const float*,
@@ -424,6 +377,69 @@ __global__ void __launch_bounds__(256) k_gemm_cc(GemmArgs<T> g) {
     }
 }
 
+namespace {
+
+struct SplitKReduceArgs {
+  const float* partial;  // [splits][M][ld] raw accumulators
+  const float* scale;
+  const float* offset;
+  void* out;  // fp32 or bf16 [M][N]
+  int out_is_bf16;
+  float* enc;
+  float* logits;
+  int M, N, ld, splits, act;
+  int is_head, anchors_per_loc, row_off, n_box, num_anchors, ncp1, hw;
+};
+
+// sums the split-K partial tiles in split order and applies the layer epilogue (affine, ReLU6, store
+// or head scatter).  One thread per 4 output columns.
+__global__ void __launch_bounds__(256) k_splitk_reduce(SplitKReduceArgs r) {
+  const int n4 = r.ld >> 2;
+  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)r.M * n4) return;
+  const int m = (int)(idx / n4), n = (int)(idx % n4) * 4;
+  if (n >= r.N) return;
+  float4 acc = *reinterpret_cast<const float4*>(r.partial + (size_t)m * r.ld + n);
+  for (int z = 1; z < r.splits; ++z) {
+    float4 p = *reinterpret_cast<const float4*>(r.partial + ((size_t)z * r.M + m) * r.ld + n);
+    acc.x = __fadd_rn(acc.x, p.x);
+    acc.y = __fadd_rn(acc.y, p.y);
+    acc.z = __fadd_rn(acc.z, p.z);
+    acc.w = __fadd_rn(acc.w, p.w);
+  }
+  float v[4] = {acc.x, acc.y, acc.z, acc.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float x = affine_rn(v[j], __ldg(r.scale + n + j), __ldg(r.offset + n + j));
+    v[j] = r.act == WB_ACT_RELU6 ? relu6f(x) : x;
+  }
+  if (r.is_head) {
+    const int f = m / r.hw, p = m - f * r.hw;
+    const size_t row = (size_t)f * r.num_anchors + r.row_off + (size_t)p * r.anchors_per_loc;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int nn = n + j;
+      if (nn >= r.N) break;
+      if (nn < r.n_box)
+        r.enc[row * 4 + nn] = v[j];
+      else
+        r.logits[row * r.ncp1 + (nn - r.n_box)] = v[j];
+    }
+  } else if (r.out_is_bf16) {
+    ActIO<__nv_bfloat16>::st4(reinterpret_cast<__nv_bfloat16*>(r.out) + (size_t)m * r.N + n, make_float4(v[0], v[1], v[2], v[3]));
+  } else {
+    *reinterpret_cast<float4*>(reinterpret_cast<float*>(r.out) + (size_t)m * r.N + n) = make_float4(v[0], v[1], v[2], v[3]);
+  }
+}
+
+void launch_splitk_reduce(const LaunchCtx& lc, const SplitKReduceArgs& r) {
+  size_t total = (size_t)r.M * (r.ld >> 2);
+  k_splitk_reduce<<<(unsigned)((total + 255) / 256), 256, 0, lc.stream>>>(r);
+  ++*lc.launch_counter;
+}
+
+}  // namespace
+
 template <typename T>
 void launch_gemm_cc(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, const float* w,
                     const float* scale, const float* offset, T* out, float* enc, float* logits,
@@ -514,53 +530,6 @@ void launch_gemm_cc(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, 
     r.hw = g.out_h * g.out_w;
     launch_splitk_reduce(lc, r);
   }
-}
-
-// sums the split-K partial tiles in split order and applies the layer epilogue (affine, ReLU6, store
-// or head scatter).  One thread per 4 output columns.
-__global__ void __launch_bounds__(256) k_splitk_reduce(SplitKReduceArgs r) {
-  const int n4 = r.ld >> 2;
-  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (size_t)r.M * n4) return;
-  const int m = (int)(idx / n4), n = (int)(idx % n4) * 4;
-  if (n >= r.N) return;
-  float4 acc = *reinterpret_cast<const float4*>(r.partial + (size_t)m * r.ld + n);
-  for (int z = 1; z < r.splits; ++z) {
-    float4 p = *reinterpret_cast<const float4*>(r.partial + ((size_t)z * r.M + m) * r.ld + n);
-    acc.x = __fadd_rn(acc.x, p.x);
-    acc.y = __fadd_rn(acc.y, p.y);
-    acc.z = __fadd_rn(acc.z, p.z);
-    acc.w = __fadd_rn(acc.w, p.w);
-  }
-  float v[4] = {acc.x, acc.y, acc.z, acc.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float x = affine_rn(v[j], __ldg(r.scale + n + j), __ldg(r.offset + n + j));
-    v[j] = r.act == WB_ACT_RELU6 ? relu6f(x) : x;
-  }
-  if (r.is_head) {
-    const int f = m / r.hw, p = m - f * r.hw;
-    const size_t row = (size_t)f * r.num_anchors + r.row_off + (size_t)p * r.anchors_per_loc;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int nn = n + j;
-      if (nn >= r.N) break;
-      if (nn < r.n_box)
-        r.enc[row * 4 + nn] = v[j];
-      else
-        r.logits[row * r.ncp1 + (nn - r.n_box)] = v[j];
-    }
-  } else if (r.out_is_bf16) {
-    ActIO<__nv_bfloat16>::st4(reinterpret_cast<__nv_bfloat16*>(r.out) + (size_t)m * r.N + n, make_float4(v[0], v[1], v[2], v[3]));
-  } else {
-    *reinterpret_cast<float4*>(reinterpret_cast<float*>(r.out) + (size_t)m * r.N + n) = make_float4(v[0], v[1], v[2], v[3]);
-  }
-}
-
-void launch_splitk_reduce(const LaunchCtx& lc, const SplitKReduceArgs& r) {
-  size_t total = (size_t)r.M * (r.ld >> 2);
-  k_splitk_reduce<<<(unsigned)((total + 255) / 256), 256, 0, lc.stream>>>(r);
-  ++*lc.launch_counter;
 }
 
 template void launch_gemm_cc<float>(const LaunchCtx&, int, const wb_layer&, const float*, const float*, const float*,

@@ -36,15 +36,6 @@ namespace {
 
 constexpr int F_TH = 8, F_TW = 16;  // output tile (pixels) = 128 GEMM rows
 
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
-                                            int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
-          "r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
 struct FusedArgs {
   const float* dw_w;  // [9][C]
   const float* dw_scale;
@@ -67,9 +58,6 @@ constexpr int F_PRODUCER_WARPS = 8;
 constexpr int F_FIRST_PRODUCER_THREAD = 32 * F_CONSUMER_WARPS;                   // 256
 constexpr int F_TMA_WARP = F_CONSUMER_WARPS + F_PRODUCER_WARPS;                  // 16
 constexpr int F_THREADS = F_FIRST_PRODUCER_THREAD + 32 * F_PRODUCER_WARPS + 32;  // 544
-
-// barrier among the 128 threads of consumer warpgroup `wg` (hardware barriers 2 and 3)
-__device__ __forceinline__ void f_wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
 
 template <int S, int BN>
 __global__ void __launch_bounds__(F_THREADS, 1)
@@ -168,7 +156,7 @@ __global__ void __launch_bounds__(F_THREADS, 1)
         const uint32_t a_lo = a_hi + A_TILE_BYTES;
         const uint32_t b_hi = smem_u32(ab0 + (size_t)s * AB_BYTES) + 2 * A_TILE_BYTES, b_lo = b_hi + B_TILE_BYTES;
         wg_x3_kblock_sum<BN>(acc, part, a_hi, a_lo, b_hi, b_lo);
-        f_wg_bar_sync(wg);  // every warp of the warpgroup has seen its MMAs complete: the stage may be refilled
+        wg_bar_sync(wg);  // every warp of the warpgroup has seen its MMAs complete: the stage may be refilled
         if ((threadIdx.x & 127) == 0) mbar_arrive(smem_u32(&empty[s]));
       }
       // folded BN + ReLU6 of this thread's two rows, 8-byte stores (a lane quad covers 32 contiguous bytes)

@@ -82,136 +82,20 @@ __device__ __forceinline__ void resized_pixel(const FrameDesc& fd, const AxisTap
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Source staging.  `resized_pixel` above issues 12 dependent single-byte global loads per resized pixel; a CTA that
-// builds a tile of resized pixels instead copies the source rows the tile samples into shared memory with aligned
-// 16-byte loads (all in flight at once, every sector fetched once) and lerps out of shared memory.  The bytes are the
-// same bytes and the lerp is the same code, so the result is bit-identical (tests/test_gpu_stages.py).
-//
-// Resized rows [ry_a, ry_b) x columns [rx_a, rx_b) of frame `fd` sample source columns [x_first, x_last] (lo/hi are
-// monotone in the destination index) of either a contiguous range of source rows (small scale factors) or of the
-// {lo, hi} row pair of every resized row (scale > 2: rows in between are never touched and are not fetched).
-struct StagePlan {
-  int x_first, seg;     // first source column, bytes per row segment
-  int y_first;          // contiguous mode: first staged source row
-  int ry_a;             // pair mode: staged row 2*(ry - ry_a) + {0, 1}
-  int rows, cpr;        // staged rows, 16-byte chunks per row (upper bound)
-  bool contiguous, on;
-};
-
-__device__ __forceinline__ StagePlan stage_plan(const FrameDesc& fd, int ry_a, int ry_b, int rx_a, int rx_b, float sy,
-                                                float sx, int pitch, int max_rows) {
-  StagePlan sp;
-  sp.on = false;
-  if (pitch <= 0 || fd.fmt != WB_FMT_RGB24 || ry_a >= ry_b || rx_a >= rx_b) return sp;  // 4:2:0 frames are not staged
-  sp.x_first = axis_tap(rx_a, fd.w, sx).lo;
-  const int x_last = axis_tap(rx_b - 1, fd.w, sx).hi;
-  sp.seg = (x_last - sp.x_first + 1) * 3;
-  sp.y_first = axis_tap(ry_a, fd.h, sy).lo;
-  const int y_last = axis_tap(ry_b - 1, fd.h, sy).hi;
-  sp.ry_a = ry_a;
-  sp.contiguous = y_last - sp.y_first + 1 <= max_rows;
-  sp.rows = sp.contiguous ? y_last - sp.y_first + 1 : 2 * (ry_b - ry_a);
-  sp.cpr = (sp.seg + 30) >> 4;
-  sp.on = sp.seg + 30 <= pitch && sp.rows <= max_rows;
-  return sp;
-}
-
-__device__ __forceinline__ const uint8_t* stage_src(const FrameDesc& fd, const StagePlan& sp, int r, float sy) {
-  int y;
-  if (sp.contiguous) {
-    y = sp.y_first + r;
-  } else {
-    AxisTap t = axis_tap(sp.ry_a + (r >> 1), fd.h, sy);
-    y = (r & 1) ? t.hi : t.lo;
-  }
-  return fd.ptr + (size_t)y * fd.pitch + (size_t)sp.x_first * 3;
-}
-
-// all threads of the CTA; caller synchronises afterwards
-__device__ __forceinline__ void stage_rows(const FrameDesc& fd, const StagePlan& sp, float sy, uint8_t* s_stage,
-                                           int pitch, int tid, int nthreads) {
-  // the image's own bytes: a window's rows are not contiguous, but nothing outside its first and last row is read
-  const uint8_t* f_begin = fd.ptr;
-  const uint8_t* f_end = fd.ptr + (size_t)(fd.h - 1) * fd.pitch + (size_t)fd.w * 3;
-  for (int i = tid; i < sp.rows * sp.cpr; i += nthreads) {
-    const int r = i / sp.cpr, k = i - r * sp.cpr;
-    const uint8_t* src = stage_src(fd, sp, r, sy);
-    const uint8_t* g = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(src) & ~(uintptr_t)15) + 16 * k;
-    if (g >= src + sp.seg) continue;
-    uint4 v;
-    if (g >= f_begin && g + 16 <= f_end) {
-      v = __ldg(reinterpret_cast<const uint4*>(g));
-    } else {  // first / last chunk of the image: never touch bytes outside it
-      uint32_t wds[4] = {0u, 0u, 0u, 0u};
-      for (int b = 0; b < 16; ++b)
-        if (g + b >= f_begin && g + b < f_end) wds[b >> 2] |= (uint32_t)__ldg(g + b) << (8 * (b & 3));
-      v = make_uint4(wds[0], wds[1], wds[2], wds[3]);
-    }
-    *reinterpret_cast<uint4*>(s_stage + (size_t)r * pitch + 16 * k) = v;
-  }
-}
-
-// resized_pixel() reading the staged rows
-__device__ __forceinline__ void resized_pixel_staged(const FrameDesc& fd, const StagePlan& sp, const uint8_t* s_stage,
-                                                     int pitch, int ry, const AxisTap& ty, const AxisTap& tx, float mul,
-                                                     float sub, float* out3) {
-  const int r0 = sp.contiguous ? ty.lo - sp.y_first : 2 * (ry - sp.ry_a);
-  const int r1 = sp.contiguous ? ty.hi - sp.y_first : 2 * (ry - sp.ry_a) + 1;
-  const uintptr_t base = reinterpret_cast<uintptr_t>(fd.ptr) + (size_t)sp.x_first * 3;
-  const size_t row_bytes = (size_t)fd.pitch;
-  const int sh0 = (int)((base + (size_t)ty.lo * row_bytes) & 15), sh1 = (int)((base + (size_t)ty.hi * row_bytes) & 15);
-  const uint8_t* p0 = s_stage + (size_t)r0 * pitch + sh0;
-  const uint8_t* p1 = s_stage + (size_t)r1 * pitch + sh1;
-  const int xl = (tx.lo - sp.x_first) * 3, xh = (tx.hi - sp.x_first) * 3;
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    float tl = (float)p0[xl + c], tr = (float)p0[xh + c];
-    float bl = (float)p1[xl + c], br = (float)p1[xh + c];
-    float v = lerp_px(tl, tr, bl, br, tx.lerp, ty.lerp);
-    out3[c] = __fsub_rn(__fmul_rn(mul, v), sub);
-  }
-}
-
-// bytes per staged row for frames up to `max_src_w` wide resized to `in_w`, tile of `tile_w` resized columns; 0 = do
-// not stage (unknown width, or the rows would not fit)
-static int stage_pitch_for(int max_src_w, int in_w, int tile_w, int rows) {
-  // opt-in (WB_STAGE=1): the direct path reads the source bytes through L1 and is issue bound, not latency bound, so
-  // staging rows in shared memory is not the default
-  const char* on = getenv("WB_STAGE");
-  if (max_src_w <= 0 || on == nullptr || on[0] != '1' || getenv("WB_NO_STAGE")) return 0;
-  const double scale = (double)max_src_w / in_w;
-  int px = (int)(tile_w * (scale > 1.0 ? scale : 1.0)) + 4;
-  if (px > max_src_w) px = max_src_w;
-  int pitch = (px * 3 + 30 + 15) & ~15;
-  return (size_t)pitch * rows <= 96 * 1024 ? pitch : 0;
-}
-
-// ---------------------------------------------------------------------------------------------------
 // K1 stand-alone: u8 HWC (any size) -> f32 [n][oh][ow][3].  Used by wb_preprocess (parity tests)
 // and by wb_backbone-less debugging; the production path is the fused stem below.
 constexpr int PP_TY = 8, PP_TX = 32;  // resized pixels per CTA of the stand-alone kernel
 
 __global__ void __launch_bounds__(PP_TY* PP_TX) k_preprocess_f32(const FrameDesc* __restrict__ frames,
                                                                   float* __restrict__ out, int oh, int ow, float mul,
-                                                                  float sub, int pitch) {
-  extern __shared__ uint4 s_dyn[];
-  uint8_t* s_stage = reinterpret_cast<uint8_t*>(s_dyn);
+                                                                  float sub) {
   const FrameDesc fd = frames[blockIdx.z];
   const float sy = axis_scale(fd.h, oh), sx = axis_scale(fd.w, ow);
-  const int oy0 = blockIdx.y * PP_TY, ox0 = blockIdx.x * PP_TX;
-  const StagePlan sp = stage_plan(fd, oy0, min(oy0 + PP_TY, oh), ox0, min(ox0 + PP_TX, ow), sy, sx, pitch, 2 * PP_TY);
-  if (sp.on) {
-    stage_rows(fd, sp, sy, s_stage, pitch, threadIdx.x, PP_TY * PP_TX);
-    __syncthreads();
-  }
-  const int oy = oy0 + (int)threadIdx.x / PP_TX, ox = ox0 + (int)threadIdx.x % PP_TX;
+  const int oy = blockIdx.y * PP_TY + (int)threadIdx.x / PP_TX, ox = blockIdx.x * PP_TX + (int)threadIdx.x % PP_TX;
   if (oy >= oh || ox >= ow) return;
   AxisTap ty = axis_tap(oy, fd.h, sy), tx = axis_tap(ox, fd.w, sx);
   float v[3];
-  if (sp.on)
-    resized_pixel_staged(fd, sp, s_stage, pitch, oy, ty, tx, mul, sub, v);
-  else
-    resized_pixel(fd, ty, tx, mul, sub, v);
+  resized_pixel(fd, ty, tx, mul, sub, v);
   float* o = out + (((size_t)blockIdx.z * oh + oy) * ow + ox) * 3;
   o[0] = v[0];
   o[1] = v[1];
@@ -219,16 +103,9 @@ __global__ void __launch_bounds__(PP_TY* PP_TX) k_preprocess_f32(const FrameDesc
 }
 
 void launch_preprocess_f32(const LaunchCtx& lc, const FrameDesc* frames, int n, float* out, int oh, int ow,
-                           float mul, float sub, int max_src_w) {
+                           float mul, float sub) {
   dim3 grid((ow + PP_TX - 1) / PP_TX, (oh + PP_TY - 1) / PP_TY, n);
-  const int pitch = stage_pitch_for(max_src_w, ow, PP_TX, 2 * PP_TY);
-  const size_t smem = (size_t)pitch * 2 * PP_TY;
-  static PerDeviceFlag attr_done;
-  if (!attr_done.get()) {
-    cudaFuncSetAttribute(k_preprocess_f32, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-    attr_done.set();
-  }
-  k_preprocess_f32<<<grid, PP_TY * PP_TX, smem, lc.stream>>>(frames, out, oh, ow, mul, sub, pitch);
+  k_preprocess_f32<<<grid, PP_TY * PP_TX, 0, lc.stream>>>(frames, out, oh, ow, mul, sub);
   ++*lc.launch_counter;
 }
 
@@ -242,13 +119,12 @@ template <typename T>
 __global__ void __launch_bounds__(ST_TY* ST_TX)
     k_stem(const FrameDesc* __restrict__ frames, const float* __restrict__ pre, wb_layer L, int in_h, int in_w,
            float mul, float sub, const float* __restrict__ w, const float* __restrict__ scale,
-           const float* __restrict__ offset, T* __restrict__ out, int pitch) {
+           const float* __restrict__ offset, T* __restrict__ out) {
   extern __shared__ float smem[];
   const int K = L.kh, S = L.stride;
   const int tile_h = (ST_TY - 1) * S + K, tile_w = (ST_TX - 1) * S + K;
   float* s_in = smem;                              // [tile_h][tile_w][3]
   float* s_w = smem + ((tile_h * tile_w * 3 + 3) & ~3);  // [K*K*3][n_pad], 16-byte aligned
-  uint8_t* s_stage = reinterpret_cast<uint8_t*>(s_w + ((K * K * 3 * (int)L.n_pad + 3) & ~3));  // [2*tile_h][pitch]
   const int f = blockIdx.z;
   const int oy0 = blockIdx.y * ST_TY, ox0 = blockIdx.x * ST_TX;
   const int tid = threadIdx.x;
@@ -259,18 +135,10 @@ __global__ void __launch_bounds__(ST_TY* ST_TX)
   const int ry0 = oy0 * S - (int)L.pad_t, rx0 = ox0 * S - (int)L.pad_l;
   FrameDesc fd;
   float sy = 1.f, sx = 1.f;
-  StagePlan sp;
-  sp.on = false;
   if (pre == nullptr) {
     fd = frames[f];
     sy = axis_scale(fd.h, in_h);  // hoisted: one division per thread, not per sampled pixel
     sx = axis_scale(fd.w, in_w);
-    sp = stage_plan(fd, max(ry0, 0), min(ry0 + tile_h, in_h), max(rx0, 0), min(rx0 + tile_w, in_w), sy, sx, pitch,
-                    2 * tile_h);
-    if (sp.on) {
-      stage_rows(fd, sp, sy, s_stage, pitch, tid, (int)blockDim.x);
-      __syncthreads();
-    }
   }
   for (int i = tid; i < tile_h * tile_w; i += blockDim.x) {
     int ly = i / tile_w, lx = i - ly * tile_w;
@@ -284,10 +152,7 @@ __global__ void __launch_bounds__(ST_TY* ST_TX)
         v[2] = p[2];
       } else {
         AxisTap ty = axis_tap(ry, fd.h, sy), tx = axis_tap(rx, fd.w, sx);
-        if (sp.on)
-          resized_pixel_staged(fd, sp, s_stage, pitch, ry, ty, tx, mul, sub, v);
-        else
-          resized_pixel(fd, ty, tx, mul, sub, v);
+        resized_pixel(fd, ty, tx, mul, sub, v);
       }
     }
     s_in[i * 3 + 0] = v[0];
@@ -352,9 +217,7 @@ template <typename T>
 __global__ void __launch_bounds__(256)
     k_stem_3x3s2_c32(const FrameDesc* __restrict__ frames, const float* __restrict__ pre, wb_layer L, int in_h, int in_w,
                      float mul, float sub, const float* __restrict__ w, const float* __restrict__ scale,
-                     const float* __restrict__ offset, T* __restrict__ out, int pitch) {
-  extern __shared__ uint4 s_dyn[];  // [2*tile_h][pitch] staged source rows
-  uint8_t* s_stage = reinterpret_cast<uint8_t*>(s_dyn);
+                     const float* __restrict__ offset, T* __restrict__ out) {
   constexpr int K = 3, S = 2, OC = 32;
   constexpr int tile_h = (ST_TY - 1) * S + K, tile_w = (ST_TX - 1) * S + K;  // 17 x 65
   __shared__ __align__(16) float s_in[tile_h * tile_w * 3];
@@ -372,22 +235,9 @@ __global__ void __launch_bounds__(256)
     wreg[j] = i < K * K * 3 * OC ? __ldg(w + (i / OC) * L.n_pad + (i % OC)) : 0.f;
   }
   const int ry0 = oy0 * S - (int)L.pad_t, rx0 = ox0 * S - (int)L.pad_l;
-  FrameDesc fd;
-  float sy = 1.f, sx = 1.f;
-  StagePlan sp;
-  sp.on = false;
   if (pre == nullptr) {
-    fd = frames[f];
-    sy = axis_scale(fd.h, in_h);
-    sx = axis_scale(fd.w, in_w);
-    sp = stage_plan(fd, max(ry0, 0), min(ry0 + tile_h, in_h), max(rx0, 0), min(rx0 + tile_w, in_w), sy, sx, pitch,
-                    2 * tile_h);
-    if (sp.on) {
-      stage_rows(fd, sp, sy, s_stage, pitch, tid, 256);
-      __syncthreads();
-    }
-  }
-  if (pre == nullptr && !sp.on) {
+    const FrameDesc fd = frames[f];
+    const float sy = axis_scale(fd.h, in_h), sx = axis_scale(fd.w, in_w);
     // two pixels per round: the byte loads of both are in flight before either is interpolated
     for (int i0 = tid; i0 < tile_h * tile_w; i0 += 512) {
       uint32_t raw[2][12];
@@ -417,28 +267,21 @@ __global__ void __launch_bounds__(256)
         }
       }
     }
-  } else
-  for (int i = tid; i < tile_h * tile_w; i += 256) {
-    int ly = i / tile_w, lx = i - ly * tile_w;
-    int ry = ry0 + ly, rx = rx0 + lx;
-    float v[3] = {0.f, 0.f, 0.f};
-    if (ry >= 0 && ry < in_h && rx >= 0 && rx < in_w) {
-      if (pre != nullptr) {
+  } else {
+    for (int i = tid; i < tile_h * tile_w; i += 256) {
+      int ly = i / tile_w, lx = i - ly * tile_w;
+      int ry = ry0 + ly, rx = rx0 + lx;
+      float v[3] = {0.f, 0.f, 0.f};
+      if (ry >= 0 && ry < in_h && rx >= 0 && rx < in_w) {
         const float* p = pre + (((size_t)f * in_h + ry) * in_w + rx) * 3;
         v[0] = p[0];
         v[1] = p[1];
         v[2] = p[2];
-      } else {
-        AxisTap ty = axis_tap(ry, fd.h, sy), tx = axis_tap(rx, fd.w, sx);
-        if (sp.on)
-          resized_pixel_staged(fd, sp, s_stage, pitch, ry, ty, tx, mul, sub, v);
-        else
-          resized_pixel(fd, ty, tx, mul, sub, v);
       }
+      s_in[i * 3 + 0] = v[0];
+      s_in[i * 3 + 1] = v[1];
+      s_in[i * 3 + 2] = v[2];
     }
-    s_in[i * 3 + 0] = v[0];
-    s_in[i * 3 + 1] = v[1];
-    s_in[i * 3 + 2] = v[2];
   }
 #pragma unroll
   for (int j = 0; j < WREGS; ++j) {
@@ -502,36 +345,27 @@ __global__ void __launch_bounds__(256)
 template <typename T>
 void launch_stem(const LaunchCtx& lc, const FrameDesc* frames, const float* pre, int n, const wb_layer& L,
                  int in_h, int in_w, float mul, float sub, const float* w, const float* scale,
-                 const float* offset, T* out, int max_src_w) {
-  const int tile_h = (ST_TY - 1) * L.stride + L.kh, tile_w = (ST_TX - 1) * L.stride + L.kw;
-  const int pitch = pre == nullptr ? stage_pitch_for(max_src_w, in_w, tile_w, 2 * tile_h) : 0;
-  const size_t stage = (size_t)pitch * 2 * tile_h;
+                 const float* offset, T* out) {
   dim3 grid((L.out_w + ST_TX - 1) / ST_TX, (L.out_h + ST_TY - 1) / ST_TY, n);
   if (L.kh == 3 && L.kw == 3 && L.stride == 2 && L.out_c == 32) {
-    static PerDeviceFlag attr3;
-    if (!attr3.get()) {
-      cudaFuncSetAttribute(k_stem_3x3s2_c32<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-      attr3.set();
-    }
-    k_stem_3x3s2_c32<T><<<grid, 256, stage, lc.stream>>>(frames, pre, L, in_h, in_w, mul, sub, w, scale, offset, out,
-                                                        pitch);
+    k_stem_3x3s2_c32<T><<<grid, 256, 0, lc.stream>>>(frames, pre, L, in_h, in_w, mul, sub, w, scale, offset, out);
     ++*lc.launch_counter;
     return;
   }
+  const int tile_h = (ST_TY - 1) * L.stride + L.kh, tile_w = (ST_TX - 1) * L.stride + L.kw;
   const size_t smem = ((((size_t)tile_h * tile_w * 3 + 3) & ~(size_t)3) +
-                       (((size_t)L.kh * L.kw * 3 * L.n_pad + 3) & ~(size_t)3)) * sizeof(float) + stage;
+                       (((size_t)L.kh * L.kw * 3 * L.n_pad + 3) & ~(size_t)3)) * sizeof(float);
   static PerDeviceFlag attr_done;
   if (!attr_done.get()) {
     cudaFuncSetAttribute(k_stem<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     attr_done.set();
   }
-  k_stem<T><<<grid, ST_TY * ST_TX, smem, lc.stream>>>(frames, pre, L, in_h, in_w, mul, sub, w, scale, offset, out,
-                                                     pitch);
+  k_stem<T><<<grid, ST_TY * ST_TX, smem, lc.stream>>>(frames, pre, L, in_h, in_w, mul, sub, w, scale, offset, out);
   ++*lc.launch_counter;
 }
 
 template void launch_stem<float>(const LaunchCtx&, const FrameDesc*, const float*, int, const wb_layer&, int,
-                                 int, float, float, const float*, const float*, const float*, float*, int);
+                                 int, float, float, const float*, const float*, const float*, float*);
 template void launch_stem<__nv_bfloat16>(const LaunchCtx&, const FrameDesc*, const float*, int,
                                          const wb_layer&, int, int, float, float, const float*, const float*,
-                                         const float*, __nv_bfloat16*, int);
+                                         const float*, __nv_bfloat16*);

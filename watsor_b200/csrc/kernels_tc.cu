@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "kernels_tc.cuh"
 #include "tc_common.cuh"
@@ -32,9 +33,7 @@ struct TcArgs {
   float* logits;
   int M, N, n_pad, K;  // K in elements
   int block_n, stages, k_blocks;
-  int splits, kb_per;  // split-K over blockIdx.z (partials reduced by k_splitk_reduce)
-  float* partial;      // [splits][M][n_pad]
-  int* tile_counters;  // split-K: arrival ticket per output tile (zero on entry, reset by the last-arriving CTA)
+  int splits, kb_per;  // split-K over blockIdx.z (one thread-block cluster per tile, reduced in distributed smem)
   const void* residual;  // != NULL: y = (acc*scale + offset) + residual[m][n]  (MobileNet-v2 bottleneck `Add`)
   // KxK / strided convolutions: the A tile of k-block kb is the tap (kb / cpb) of the filter window, channel block
   // kb % cpb, fetched by a 4-D TMA box {32 ch, OW, OH, imgs} whose traversal strides are the conv stride
@@ -43,15 +42,6 @@ struct TcArgs {
   int rows_per_tile;  // GEMM rows one CTA produces (128, or imgs_per_tile*OH*OW for conv tiles)
   int act, is_head, anchors_per_loc, row_off, n_box, num_anchors, ncp1, hw;
 };
-
-__device__ __forceinline__ void tma_load_4d_tc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
-                                               int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
-          "r"(dst),
-      "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
 
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -71,12 +61,12 @@ __device__ __forceinline__ float4 ld_dsmem128(uint32_t addr, uint32_t rank) {
 }
 
 // One output row of the tile from the staging tile(s) to global memory, lanes along the columns (coalesced).
-// members == 1: the row already carries the layer epilogue.  members > 1 (split-K cluster): the row is the sum of the
-// members' raw partial rows in rank order, then folded BN / bias, ReLU6.  Then the optional bottleneck shortcut, and
-// the store: dense [M][N], or the head scatter into the concatenated box-encoding / class-logit tensors.
+// The row's raw accumulators are this CTA's own (members == 1) or, in a split-K cluster, the sum of the members'
+// partial rows in rank order; then folded BN / bias, ReLU6, the optional bottleneck shortcut, and the store: dense
+// [M][N], or the head scatter into the concatenated box-encoding / class-logit tensors.
 template <bool TF32>
 __device__ __forceinline__ void copy_out_row(const TcArgs& g, const uint8_t* smem, int pitch, int r, int m0, int n0,
-                                             int lane, int members, int reduce) {
+                                             int lane, int members) {
   const int mm = m0 + r;
   const uint32_t src = smem_u32(smem) + (uint32_t)(r * pitch * 4);
   size_t hr = 0;
@@ -87,26 +77,21 @@ __device__ __forceinline__ void copy_out_row(const TcArgs& g, const uint8_t* sme
   for (int j = lane * 4; j < g.block_n; j += 128) {
     const int nn = n0 + j;
     if (nn >= g.N) break;
-    float4 y;
-    if (reduce) {
-      float4 p[8];  // members <= 8 (portable cluster size): all remote loads in flight, then the ordered sum
-      if (members == 1) {
-        p[0] = lds128(src + (uint32_t)(j * 4));
-      } else {
-#pragma unroll
-        for (int z = 0; z < 8; ++z)
-          if (z < members) p[z] = ld_dsmem128(src + (uint32_t)(j * 4), (uint32_t)z);
-      }
-      y = p[0];
-#pragma unroll
-      for (int z = 1; z < 8; ++z)
-        if (z < members) y = make_float4(__fadd_rn(y.x, p[z].x), __fadd_rn(y.y, p[z].y), __fadd_rn(y.z, p[z].z), __fadd_rn(y.w, p[z].w));
-      const float4 sc = *reinterpret_cast<const float4*>(g.scale + nn), of = *reinterpret_cast<const float4*>(g.offset + nn);
-      y = make_float4(affine_rn(y.x, sc.x, of.x), affine_rn(y.y, sc.y, of.y), affine_rn(y.z, sc.z, of.z), affine_rn(y.w, sc.w, of.w));
-      if (g.act == WB_ACT_RELU6) y = make_float4(relu6f(y.x), relu6f(y.y), relu6f(y.z), relu6f(y.w));
+    float4 p[8];  // members <= 8 (portable cluster size): all remote loads in flight, then the ordered sum
+    if (members == 1) {
+      p[0] = lds128(src + (uint32_t)(j * 4));
     } else {
-      y = lds128(src + (uint32_t)(j * 4));
+#pragma unroll
+      for (int z = 0; z < 8; ++z)
+        if (z < members) p[z] = ld_dsmem128(src + (uint32_t)(j * 4), (uint32_t)z);
     }
+    float4 y = p[0];
+#pragma unroll
+    for (int z = 1; z < 8; ++z)
+      if (z < members) y = make_float4(__fadd_rn(y.x, p[z].x), __fadd_rn(y.y, p[z].y), __fadd_rn(y.z, p[z].z), __fadd_rn(y.w, p[z].w));
+    const float4 sc = *reinterpret_cast<const float4*>(g.scale + nn), of = *reinterpret_cast<const float4*>(g.offset + nn);
+    y = make_float4(affine_rn(y.x, sc.x, of.x), affine_rn(y.y, sc.y, of.y), affine_rn(y.z, sc.z, of.z), affine_rn(y.w, sc.w, of.w));
+    if (g.act == WB_ACT_RELU6) y = make_float4(relu6f(y.x), relu6f(y.y), relu6f(y.z), relu6f(y.w));
     if (g.is_head) {
       const float ys[4] = {y.x, y.y, y.z, y.w};
 #pragma unroll
@@ -132,9 +117,6 @@ __device__ __forceinline__ void copy_out_row(const TcArgs& g, const uint8_t* sme
 
 constexpr int GEMM_THREADS = 288;
 constexpr int GEMM_PRODUCER_WARP = 8;
-
-// barrier among the 128 threads of consumer warpgroup `wg` (hardware barriers 2 and 3)
-__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
 
 // MODE 0: bf16 operands; MODE 1: tf32 single product (diagnostic); MODE 2: tf32 x3 split.  BN: N tile (32 / 64 / 128).
 template <int MODE, int BN>
@@ -189,7 +171,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           mbar_expect_tx(bar, g.rows_per_tile * ROW_BYTES + B_TILE_BYTES * SLOTS);
           const int tap = kb / g.cpb, cb = kb - tap * g.cpb;
           const int ky = tap / g.conv_kw, kx = tap - ky * g.conv_kw;
-          tma_load_4d_tc(smem_u32(st), &map_a, bar, cb * K_PER_BLOCK, kx - g.conv_pad_l, ky - g.conv_pad_t, m0 / g.hw);
+          tma_load_4d(smem_u32(st), &map_a, bar, cb * K_PER_BLOCK, kx - g.conv_pad_l, ky - g.conv_pad_t, m0 / g.hw);
         } else {
           mbar_expect_tx(bar, A_TILE_BYTES + B_TILE_BYTES * SLOTS);
           tma_load_2d(smem_u32(st), &map_a, bar, kb * K_PER_BLOCK, m0);
@@ -255,111 +237,61 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     cluster_sync_all();
     const int z = (int)cluster_ctarank();
     for (int r = z + g.splits * warp; r < rows; r += n_warps * g.splits)
-      copy_out_row<TF32>(g, smem, pitch, r, m0, n0, lane, g.splits, 1);
+      copy_out_row<TF32>(g, smem, pitch, r, m0, n0, lane, g.splits);
     __syncwarp();
     cluster_sync_all();  // nobody exits while a peer still reads its staging tile
   } else if (g.is_head) {
-    for (int r = warp; r < rows; r += n_warps) copy_out_row<TF32>(g, smem, pitch, r, m0, n0, lane, 1, 1);
+    for (int r = warp; r < rows; r += n_warps) copy_out_row<TF32>(g, smem, pitch, r, m0, n0, lane, 1);
   } else {
-    // dense [M][N] output: the tile's rows x block_n/4 float4 columns as one flat item list over all threads, 4 items
-    // per thread in flight, consecutive lanes on consecutive 16-byte columns
-    const int c4n = g.block_n >> 2;
-    const int items = rows * c4n;
-    const int T = (int)blockDim.x;
-    const uint32_t sbase = smem_u32(smem);
-    int inc_r = T / c4n, inc_c = T - inc_r * c4n;  // item index advances by T per step
-    int r_it = (int)threadIdx.x / c4n, c_it = (int)threadIdx.x - r_it * c4n;
-    if (TF32 && inc_r >= 1) {
-      // use the largest thread count that is a multiple of the row length (block_n = 144: 288 of the 320 threads), so
-      // that every thread keeps its 4 columns
-      inc_c = 0;
-      if ((int)threadIdx.x >= inc_r * c4n) r_it = rows;  // surplus threads idle
-    }
-    if (inc_c == 0 && TF32) {
-      // the thread count is a multiple of the row length (block_n = 16/32/64/80/128/160): a thread keeps its 4 columns
-      // and walks down the rows -- folded BN / bias in registers, pointers advanced by a constant, ~20 instructions per
-      // float4 instead of ~50 (this phase is issue bound: 2.5 warps per scheduler)
-      const int nn = n0 + c_it * 4;
-      if (nn < g.N && r_it < rows) {
-        const float4 sc = __ldg(reinterpret_cast<const float4*>(g.scale + nn)), of = __ldg(reinterpret_cast<const float4*>(g.offset + nn));
-        const bool relu = g.act == WB_ACT_RELU6;
-        uint32_t sp = sbase + (uint32_t)((r_it * pitch + c_it * 4) * 4);
-        const uint32_t sstep = (uint32_t)(inc_r * pitch * 4);
-        float* op = reinterpret_cast<float*>(g.out) + (size_t)(m0 + r_it) * g.N + nn;
-        const float* rp = g.residual != nullptr ? reinterpret_cast<const float*>(g.residual) + (size_t)(m0 + r_it) * g.N + nn : nullptr;
-        const size_t gstep = (size_t)inc_r * g.N;
-        int r = r_it;
-        for (; r + 3 * inc_r < rows; r += 4 * inc_r) {
-          float4 y[4], rs[4];
+    // dense [M][N] output: the thread count is a multiple of the row's BN / 4 float4 columns, so a thread keeps its 4
+    // columns and walks down the rows -- folded BN / bias in registers, pointers advanced by a constant, ~20
+    // instructions per float4 (this phase is issue bound: 2.5 warps per scheduler)
+    static_assert(GEMM_THREADS % (BN / 4) == 0, "every thread of the dense epilogue keeps its 4 columns");
+    constexpr int C4N = BN / 4, ROW_STEP = GEMM_THREADS / C4N;
+    using OutT = typename std::conditional<TF32, float, __nv_bfloat16>::type;
+    const int r_it = (int)threadIdx.x / C4N, c_it = (int)threadIdx.x % C4N;
+    const int nn = n0 + c_it * 4;
+    if (nn < g.N && r_it < rows) {
+      const float4 sc = __ldg(reinterpret_cast<const float4*>(g.scale + nn)), of = __ldg(reinterpret_cast<const float4*>(g.offset + nn));
+      const bool relu = g.act == WB_ACT_RELU6;
+      uint32_t sp = smem_u32(smem) + (uint32_t)((r_it * pitch + c_it * 4) * 4);
+      constexpr uint32_t sstep = (uint32_t)(ROW_STEP * pitch * 4);
+      OutT* op = reinterpret_cast<OutT*>(g.out) + (size_t)(m0 + r_it) * g.N + nn;
+      // the bottleneck shortcut is fused in the fp32 modes only
+      const float* rp = TF32 && g.residual != nullptr ? reinterpret_cast<const float*>(g.residual) + (size_t)(m0 + r_it) * g.N + nn : nullptr;
+      const size_t gstep = (size_t)ROW_STEP * g.N;
+      int r = r_it;
+      for (; r + 3 * ROW_STEP < rows; r += 4 * ROW_STEP) {
+        float4 y[4], rs[4];
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            y[u] = lds128(sp + u * sstep);
-            if (rp != nullptr) rs[u] = *reinterpret_cast<const float4*>(rp + u * gstep);
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            float4 v = make_float4(affine_rn(y[u].x, sc.x, of.x), affine_rn(y[u].y, sc.y, of.y), affine_rn(y[u].z, sc.z, of.z),
-                                   affine_rn(y[u].w, sc.w, of.w));
-            if (relu) v = make_float4(relu6f(v.x), relu6f(v.y), relu6f(v.z), relu6f(v.w));
-            if (rp != nullptr) v = make_float4(__fadd_rn(v.x, rs[u].x), __fadd_rn(v.y, rs[u].y), __fadd_rn(v.z, rs[u].z), __fadd_rn(v.w, rs[u].w));
-            *reinterpret_cast<float4*>(op + u * gstep) = v;
-          }
-          sp += 4 * sstep;
-          op += 4 * gstep;
-          if (rp != nullptr) rp += 4 * gstep;
+        for (int u = 0; u < 4; ++u) {
+          y[u] = lds128(sp + u * sstep);
+          if (rp != nullptr) rs[u] = *reinterpret_cast<const float4*>(rp + u * gstep);
         }
-        for (; r < rows; r += inc_r) {
-          const float4 y = lds128(sp);
-          float4 v = make_float4(affine_rn(y.x, sc.x, of.x), affine_rn(y.y, sc.y, of.y), affine_rn(y.z, sc.z, of.z), affine_rn(y.w, sc.w, of.w));
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          float4 v = make_float4(affine_rn(y[u].x, sc.x, of.x), affine_rn(y[u].y, sc.y, of.y), affine_rn(y[u].z, sc.z, of.z),
+                                 affine_rn(y[u].w, sc.w, of.w));
           if (relu) v = make_float4(relu6f(v.x), relu6f(v.y), relu6f(v.z), relu6f(v.w));
-          if (rp != nullptr) {
-            const float4 r4 = *reinterpret_cast<const float4*>(rp);
-            v = make_float4(__fadd_rn(v.x, r4.x), __fadd_rn(v.y, r4.y), __fadd_rn(v.z, r4.z), __fadd_rn(v.w, r4.w));
-            rp += gstep;
-          }
-          *reinterpret_cast<float4*>(op) = v;
-          sp += sstep;
-          op += gstep;
+          if (rp != nullptr) v = make_float4(__fadd_rn(v.x, rs[u].x), __fadd_rn(v.y, rs[u].y), __fadd_rn(v.z, rs[u].z), __fadd_rn(v.w, rs[u].w));
+          ActIO<OutT>::st4(op + u * gstep, v);
         }
+        sp += 4 * sstep;
+        op += 4 * gstep;
+        if (rp != nullptr) rp += 4 * gstep;
       }
-    } else
-    for (int i0 = threadIdx.x; i0 < items; i0 += 4 * T) {
-      float4 y[4], sc[4], of[4];
-      int rr[4], cc[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        rr[u] = r_it;
-        cc[u] = c_it * 4;
-        if (i0 + T * u < items && n0 + cc[u] < g.N) {
-          y[u] = lds128(sbase + (uint32_t)((rr[u] * pitch + cc[u]) * 4));
-          // folded BN / bias of these 4 columns (every row re-reads the same few lines: L1 hits)
-          sc[u] = __ldg(reinterpret_cast<const float4*>(g.scale + n0 + cc[u]));
-          of[u] = __ldg(reinterpret_cast<const float4*>(g.offset + n0 + cc[u]));
+      for (; r < rows; r += ROW_STEP) {
+        const float4 y = lds128(sp);
+        float4 v = make_float4(affine_rn(y.x, sc.x, of.x), affine_rn(y.y, sc.y, of.y), affine_rn(y.z, sc.z, of.z), affine_rn(y.w, sc.w, of.w));
+        if (relu) v = make_float4(relu6f(v.x), relu6f(v.y), relu6f(v.z), relu6f(v.w));
+        if (rp != nullptr) {
+          const float4 r4 = *reinterpret_cast<const float4*>(rp);
+          v = make_float4(__fadd_rn(v.x, r4.x), __fadd_rn(v.y, r4.y), __fadd_rn(v.z, r4.z), __fadd_rn(v.w, r4.w));
+          rp += gstep;
         }
-        r_it += inc_r;
-        c_it += inc_c;
-        if (c_it >= c4n) {
-          c_it -= c4n;
-          ++r_it;
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int nn = n0 + cc[u];
-        if (i0 + T * u >= items || nn >= g.N) continue;
-        const size_t o = (size_t)(m0 + rr[u]) * g.N + nn;
-        y[u] = make_float4(affine_rn(y[u].x, sc[u].x, of[u].x), affine_rn(y[u].y, sc[u].y, of[u].y),
-                           affine_rn(y[u].z, sc[u].z, of[u].z), affine_rn(y[u].w, sc[u].w, of[u].w));
-        if (g.act == WB_ACT_RELU6) y[u] = make_float4(relu6f(y[u].x), relu6f(y[u].y), relu6f(y[u].z), relu6f(y[u].w));
-        if (TF32) {
-          if (g.residual != nullptr) {
-            const float4 r4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(g.residual) + o);
-            y[u] = make_float4(__fadd_rn(y[u].x, r4.x), __fadd_rn(y[u].y, r4.y), __fadd_rn(y[u].z, r4.z), __fadd_rn(y[u].w, r4.w));
-          }
-          *reinterpret_cast<float4*>(reinterpret_cast<float*>(g.out) + o) = y[u];
-        } else {
-          ActIO<__nv_bfloat16>::st4(reinterpret_cast<__nv_bfloat16*>(g.out) + o, y[u]);
-        }
+        ActIO<OutT>::st4(op, v);
+        sp += sstep;
+        op += gstep;
       }
     }
   }
@@ -534,8 +466,7 @@ void tc_free_weights(TcWeights* w) {
 
 int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, int n, const wb_layer& L, const void* in,
                    const float* scale, const float* offset, void* out, float* enc, float* logits, int num_anchors,
-                   int num_classes_p1, float* partial, size_t partial_floats, int* tile_counters, const void* residual,
-                   std::string* err) {
+                   int num_classes_p1, const void* residual, std::string* err) {
   const TcLayerWeights& w = tw.layers[layer_index];
   if (!w.ready) {
     *err = "no tensor-core weights for this layer";
@@ -554,7 +485,6 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
   g.n_pad = L.n_pad;
   g.K = L.kh * L.kw * L.in_c;
   g.block_n = w.block_n;
-  g.tile_counters = tile_counters;
   g.residual = mode == TC_BF16 ? nullptr : residual;
   g.conv = L.op == WB_OP_CONV;
   g.cpb = (L.in_c * elem) / ROW_BYTES;
@@ -581,7 +511,6 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
   // latency-bound shapes: split K so that about one wave of CTAs exists (deterministic cluster reduce)
   g.splits = 1;
   g.kb_per = g.k_blocks;
-  g.partial = partial;
   const long tiles = (long)grid.x * grid.y;
   // the cluster barriers + DSMEM reduction of a split cost several k-blocks' worth of time: splitting only pays for
   // long accumulation chains, and every split keeps >= 8 k-blocks

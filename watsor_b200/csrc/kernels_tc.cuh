@@ -28,8 +28,7 @@ int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb
 void tc_free_weights(TcWeights* w);
 int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, int n, const wb_layer& L, const void* in,
                    const float* scale, const float* offset, void* out, float* enc, float* logits, int num_anchors,
-                   int num_classes_p1, float* partial, size_t partial_floats, int* tile_counters, const void* residual,
-                   std::string* err);
+                   int num_classes_p1, const void* residual, std::string* err);
 
 // generic tiled tensor-map encoder (rank <= 5); `map` points to 128 bytes aligned to 64
 bool tc_encode_map(void* map, const void* base, int elem_bytes, int rank, const unsigned long long* dims,

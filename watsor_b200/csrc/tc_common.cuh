@@ -1,6 +1,6 @@
 // tc_common.cuh -- inline PTX wrappers shared by the tensor-core kernels (kernels_tc.cu, kernels_fused.cu):
-// mbarrier, TMA (cp.async.bulk.tensor load / store), wgmma (warpgroup MMA with the accumulator in registers) and the
-// shared-memory matrix descriptor (bit layout as in cute/arch/mma_sm90_desc.hpp).  sm_90a.
+// mbarrier, TMA (cp.async.bulk.tensor load / store), the consumer warpgroups' named barrier, wgmma (warpgroup MMA with
+// the accumulator in registers) and the shared-memory matrix descriptor (bit layout as in cute/arch/mma_sm90_desc.hpp).  sm_90a.
 #pragma once
 #include <cuda.h>
 
@@ -42,6 +42,16 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
+                                            int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
+          "r"(dst),
+      "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+// barrier among the 128 threads of consumer warpgroup `wg` (hardware barriers 2 and 3)
+__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
 // One elected lane of a converged warp.  Unlike `lane == 0`, ptxas knows the guarded region runs in a single
 // thread, so the TMA operands move to uniform registers without a per-instruction uniformisation loop.
 __device__ __forceinline__ bool elect_one() {

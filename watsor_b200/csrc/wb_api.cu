@@ -47,7 +47,6 @@ struct Slot {
   float *d_enc = nullptr, *d_logits = nullptr, *d_dec = nullptr;
   float* d_partial = nullptr;  // split-K scratch
   size_t partial_floats = 0;
-  int* d_tile_counters = nullptr;  // split-K arrival tickets (zero between launches)
   int *d_cand_count = nullptr, *d_sel_count = nullptr;
   int* d_kept_hist = nullptr;  // [B][1024] per-frame histogram of kept scores (exact NMS early exit)
   unsigned long long *d_cand = nullptr, *d_sel = nullptr;
@@ -70,7 +69,6 @@ struct Slot {
   int graph_frames = -1;
   bool graph_windowed = false;
   uint32_t graph_flags = 0;
-  int graph_src_w = 0;  // widest camera the captured stem kernel sized its staging for
 };
 
 struct wb_ctx {
@@ -78,7 +76,6 @@ struct wb_ctx {
   int max_batch = 0;
   int precision = 0;
   bool use_graph = true;
-  int max_src_w = 0;  // widest configured camera: sizes the stem's shared-memory staging of source rows
   // frame scatter (wb_comm_*): NCCL communicator bound at run time, its stream and the event the slots wait on
   void* comm = nullptr;
   int comm_rank = -1, comm_world = 0;
@@ -150,8 +147,6 @@ static int alloc_slot(wb_ctx* c, Slot& s) {
   CK(cudaMalloc(&s.d_dec, sizeof(float) * (size_t)B * N * 4));
   s.partial_floats = (size_t)4 * 1024 * 1024 + (size_t)B * 512 * 1024;
   CK(cudaMalloc(&s.d_partial, sizeof(float) * s.partial_floats));
-  CK(cudaMalloc(&s.d_tile_counters, sizeof(int) * 4096));
-  CK(cudaMemset(s.d_tile_counters, 0, sizeof(int) * 4096));
   CK(cudaMalloc(&s.d_cand_count, sizeof(int) * (size_t)B * C));
   CK(cudaMalloc(&s.d_sel_count, sizeof(int) * (size_t)B * C));
   CK(cudaMalloc(&s.d_kept_hist, sizeof(int) * (size_t)B * 1024));
@@ -220,7 +215,9 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
       REQUIRE(L.in_c % 4 == 0, std::string("layer ") + L.name + ": in_c must be a multiple of 4");
     if (L.op == WB_OP_CONV)
       REQUIRE(L.in_c % 16 == 0, std::string("layer ") + L.name + ": KxK convs need in_c to be a multiple of 16");
-    if (L.op == WB_OP_DW) REQUIRE(L.out_c % 4 == 0 && L.kh == 3 && L.kw == 3, "depthwise must be 3x3, C%4==0");
+    if (L.op == WB_OP_DW)
+      REQUIRE(L.out_c % 4 == 0 && L.kh == 3 && L.kw == 3 && (L.stride == 1 || L.stride == 2),
+              "depthwise must be 3x3 with stride 1 or 2, C%4==0");
     if (L.op == WB_OP_PW || L.op == WB_OP_CONV) REQUIRE(L.out_c % 4 == 0, "out_c must be a multiple of 4");
     if (L.op == WB_OP_MAXPOOL || L.op == WB_OP_AVGPOOL)
       REQUIRE(L.out_c % 4 == 0 && L.in_c == L.out_c && L.kh >= 1 && L.kw >= 1, "pooling needs C % 4 == 0");
@@ -282,7 +279,6 @@ int wb_destroy(wb_ctx* c) {
     cudaFree(s.d_logits);
     cudaFree(s.d_dec);
     cudaFree(s.d_partial);
-    cudaFree(s.d_tile_counters);
     cudaFree(s.d_cand_count);
     cudaFree(s.d_sel_count);
     cudaFree(s.d_kept_hist);
@@ -364,7 +360,6 @@ int wb_set_camera(wb_ctx* c, int cam, int width, int height, int n_zones, const 
   memset(&cfg, 0, sizeof(cfg));
   cfg.width = width;
   cfg.height = height;
-  c->max_src_w = std::max(c->max_src_w, width);
   cfg.n_zones = n_zones;
   cfg.has_mask = raster != nullptr ? 1 : 0;
   cfg.check_label = (cam_flags & WB_CAM_NO_LABEL_CHECK) ? 0 : 1;
@@ -524,7 +519,7 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
     switch (L.op) {
       case WB_OP_STEM:
         launch_stem<T>(lc, s.d_desc, pre, n, L, c->hdr.input_h, c->hdr.input_w, c->hdr.pre_mul, c->hdr.pre_sub, w,
-                       sc, of, outp, c->max_src_w);
+                       sc, of, outp);
         break;
       case WB_OP_DW: {
         const Span sp = fused_span(c, li, end);
@@ -572,7 +567,7 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
           }
           std::string err;
           if (tc_launch_gemm(lc, c->tc, (int)li, n, L, static_cast<const void*>(in), sc, of, dst, s.d_enc, s.d_logits, NA,
-                             C1, s.d_partial, s.partial_floats, s.d_tile_counters, residual, &err))
+                             C1, residual, &err))
             return fail("layer " + std::string(L.name) + ": " + err);
           if (fuse_add) ++li;  // the Add layer is done
         } else {
@@ -622,8 +617,8 @@ static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t 
     s.launches = 0;
     return run_all(c, s, st, n, gflags, n_frames, windowed);
   }
-  if (s.graph_exec == nullptr || s.graph_n != n || s.graph_flags != gflags || s.graph_src_w != c->max_src_w ||
-      s.graph_frames != n_frames || s.graph_windowed != windowed) {
+  if (s.graph_exec == nullptr || s.graph_n != n || s.graph_flags != gflags || s.graph_frames != n_frames ||
+      s.graph_windowed != windowed) {
     if (s.graph_exec) {
       cudaGraphExecDestroy(s.graph_exec);
       s.graph_exec = nullptr;
@@ -643,7 +638,6 @@ static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t 
     CK(cudaGraphDestroy(graph));
     s.graph_n = n;
     s.graph_flags = gflags;
-    s.graph_src_w = c->max_src_w;
     s.graph_frames = n_frames;
     s.graph_windowed = windowed;
   }
@@ -871,10 +865,7 @@ int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t*
   }
   CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n, cudaMemcpyHostToDevice, st));
   LaunchCtx lc{st, &s.launches};
-  int max_w = 0;
-  for (int i = 0; i < n; ++i) max_w = std::max(max_w, (int)widths[i]);
-  launch_preprocess_f32(lc, s.d_desc, n, s.d_pre, c->hdr.input_h, c->hdr.input_w, c->hdr.pre_mul, c->hdr.pre_sub,
-                        max_w);
+  launch_preprocess_f32(lc, s.d_desc, n, s.d_pre, c->hdr.input_h, c->hdr.input_w, c->hdr.pre_mul, c->hdr.pre_sub);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, s.d_pre, sizeof(float) * (size_t)n * c->hdr.input_h * c->hdr.input_w * 3,
                      cudaMemcpyDeviceToHost, st));
