@@ -232,6 +232,16 @@ int wb_preprocess(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_
  * copies that layer's activation (float32 NHWC) to layer_out. */
 int wb_backbone(wb_ctx* ctx, int n, const float* pre, float* enc, float* logits, int stop_layer,
                 float* layer_out, size_t layer_out_floats);
+/* the product path's own input handling (frames as wb_submit takes them: host or device, rgb24 / yuv420p / nv12,
+ * a camera's detection windows expanded into model images), run to stop_layer; n_images = model images of the batch.
+ * flags: WB_F_YUV420P, WB_F_NV12, WB_F_FRAMES_ON_DEVICE, WB_F_FUSE_FILTERS.  Runs on slot 0.
+ *   stop_layer >= 0: the layers up to stop_layer, eagerly; layer_out as for wb_backbone, for n_images images.
+ *   stop_layer == -1: the kernels of wb_submit (CUDA graph, post stage, window merge).
+ * enc / logits (optional): [n_images][anchors][4] / [n_images][anchors][classes+1] as the run left them -- unlike
+ * wb_backbone, they are not cleared first; size them from the cameras' windows. */
+int wb_backbone_frames(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_t* cam_ids, uint32_t flags,
+                       float* enc, float* logits, int stop_layer, float* layer_out, size_t layer_out_floats,
+                       int32_t* n_images);
 /* Postprocessor/... + tensorflow_cpu.py:79-90 + filters, from given head outputs (host);
  * boxes/scores/classes (optional, host): the graph outputs detection_boxes[n][100][4],
  * detection_scores[n][100], detection_classes[n][100], num[n] before integer conversion */

@@ -78,6 +78,8 @@ def load():
         'wb_comm_destroy': (c_int, [c_void_p]),
         'wb_preprocess': (c_int, [c_void_p, c_int, P(c_void_p), P(c_int32), P(c_int32), c_void_p]),
         'wb_backbone': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t]),
+        'wb_backbone_frames': (c_int, [c_void_p, c_int, P(c_void_p), P(c_int32), c_uint32, c_void_p, c_void_p, c_int,
+                                       c_void_p, c_size_t, P(c_int32)]),
         'wb_postprocess': (c_int, [c_void_p, c_int, c_void_p, c_void_p, P(c_int32), c_uint32,
                                    P(c_void_p), P(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p]),
         'wb_filter_rows': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
@@ -113,7 +115,7 @@ EXPORTS = ['wb_abi_version', 'wb_last_error', 'wb_device_count', 'wb_create', 'w
            'wb_device_name', 'wb_set_stream', 'wb_model_info', 'wb_set_camera', 'wb_set_camera_windows',
            'wb_register_host',
            'wb_unregister_host', 'wb_detect', 'wb_submit', 'wb_collect', 'wb_stream_fence', 'wb_comm_unique_id', 'wb_comm_init',
-           'wb_scatter_frames', 'wb_comm_destroy', 'wb_preprocess', 'wb_backbone',
+           'wb_scatter_frames', 'wb_comm_destroy', 'wb_preprocess', 'wb_backbone', 'wb_backbone_frames',
            'wb_postprocess', 'wb_filter_rows', 'wb_anchors', 'wb_last_launch_count', 'wb_profile_layers',
            'wb_tracker_create', 'wb_tracker_destroy', 'wb_tracker_update', 'wb_sieve_rows', 'wb_debug_pyset_order',
            'wb_debug_unused_order', 'wb_debug_argsort', 'wb_fx_create', 'wb_fx_set_camera', 'wb_fx_render',

@@ -3,9 +3,10 @@
 // Restates graph nodes `Cast`, `Preprocessor/map/while/ResizeImage/resize/ResizeBilinear`
 // (align_corners=false, half_pixel_centers=false), `Preprocessor/mul`, `Preprocessor/sub` and
 // `FeatureExtractor/.../Conv2d_0/{Conv2D,BatchNorm,Relu6}` of the frozen graph that
-// watsor/detection/tensorflow_cpu.py:114 runs.  Compiled with -fmad=false: the bilinear lerp is
-// a chain of separately rounded fp32 ops, exactly like TF's CPU kernel, so K1 is bit-exact
-// against the oracle.
+// watsor/detection/tensorflow_cpu.py:114 runs.  The bilinear lerp is written with the explicit
+// round-to-nearest intrinsics (__fadd_rn / __fsub_rn / __fmul_rn / __fdiv_rn), which the compiler never
+// contracts into a multiply-add: a chain of separately rounded fp32 ops, exactly like TF's CPU kernel, so K1
+// is bit-exact against the oracle, and the fused stem's resize equals K1 bit for bit.
 #include "common.cuh"
 
 struct AxisTap {

@@ -873,6 +873,29 @@ int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t*
   return 0;
 }
 
+}  // extern "C"
+
+// the stage hooks' copy of layer `li`'s activation (n images, float32 NHWC; bf16 storage is widened) from slot s
+static int copy_layer_out(wb_ctx* c, Slot& s, int n, int li, float* layer_out, size_t layer_out_floats) {
+  const wb_layer& L = c->layers[li];
+  REQUIRE(L.op != WB_OP_HEAD, "head layers have no activation output");
+  size_t elems = (size_t)n * L.out_h * L.out_w * L.out_c;
+  REQUIRE(layer_out_floats >= elems, "layer_out too small");
+  if (c->elem_size() == 4) {
+    CK(cudaMemcpy(layer_out, static_cast<float*>(s.arena) + (size_t)L.out_off * n, elems * 4, cudaMemcpyDeviceToHost));
+  } else {
+    std::vector<uint16_t> tmp(elems);
+    CK(cudaMemcpy(tmp.data(), static_cast<uint16_t*>(s.arena) + (size_t)L.out_off * n, elems * 2, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < elems; ++i) {
+      uint32_t u = (uint32_t)tmp[i] << 16;
+      memcpy(&layer_out[i], &u, 4);
+    }
+  }
+  return 0;
+}
+
+extern "C" {
+
 int wb_backbone(wb_ctx* c, int n, const float* pre, float* enc, float* logits, int stop_layer, float* layer_out,
                 size_t layer_out_floats) {
   REQUIRE(c && pre, "NULL argument");
@@ -896,22 +919,46 @@ int wb_backbone(wb_ctx* c, int n, const float* pre, float* enc, float* logits, i
     CK(cudaMemcpyAsync(logits, s.d_logits, sizeof(float) * (size_t)n * c->hdr.num_anchors * (c->hdr.num_classes + 1),
                        cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  if (stop_layer >= 0 && layer_out) {
-    const wb_layer& L = c->layers[stop_layer];
-    REQUIRE(L.op != WB_OP_HEAD, "head layers have no activation output");
-    size_t elems = (size_t)n * L.out_h * L.out_w * L.out_c;
-    REQUIRE(layer_out_floats >= elems, "layer_out too small");
-    if (c->elem_size() == 4) {
-      CK(cudaMemcpy(layer_out, static_cast<float*>(s.arena) + (size_t)L.out_off * n, elems * 4, cudaMemcpyDeviceToHost));
-    } else {
-      std::vector<uint16_t> tmp(elems);
-      CK(cudaMemcpy(tmp.data(), static_cast<uint16_t*>(s.arena) + (size_t)L.out_off * n, elems * 2, cudaMemcpyDeviceToHost));
-      for (size_t i = 0; i < elems; ++i) {
-        uint32_t u = (uint32_t)tmp[i] << 16;
-        memcpy(&layer_out[i], &u, 4);
-      }
-    }
+  if (stop_layer >= 0 && layer_out)
+    if (int rc = copy_layer_out(c, s, n, stop_layer, layer_out, layer_out_floats)) return rc;
+  c->last_launches = s.launches;
+  return 0;
+}
+
+int wb_backbone_frames(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t* cam_ids, uint32_t flags,
+                       float* enc, float* logits, int stop_layer, float* layer_out, size_t layer_out_floats,
+                       int32_t* n_images) {
+  REQUIRE(c && frames && cam_ids, "NULL argument");
+  REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range");
+  REQUIRE(stop_layer >= -1 && stop_layer < (int)c->layers.size(), "stop_layer out of range");
+  REQUIRE((flags & ~(WB_F_YUV420P | WB_F_NV12 | WB_F_FRAMES_ON_DEVICE | WB_F_FUSE_FILTERS)) == 0,
+          "flags may only hold WB_F_YUV420P, WB_F_NV12, WB_F_FRAMES_ON_DEVICE and WB_F_FUSE_FILTERS");
+  std::lock_guard<std::mutex> lock(c->mu);
+  CK(cudaSetDevice(c->device));
+  Slot& s = c->slots[0];
+  REQUIRE(!s.busy, "slot 0 is busy");
+  cudaStream_t st = c->stream_of(0);
+  int fmt = WB_FMT_RGB24;
+  if (int rc = frame_format(flags, &fmt)) return rc;
+  int ni = n;
+  if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &ni)) return rc;
+  if (stop_layer >= 0) {
+    s.launches = 0;
+    int rc = c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, ni, nullptr, 0, stop_layer)
+                               : run_layers<float>(c, s, st, ni, nullptr, 0, stop_layer);
+    if (rc) return rc;
+  } else if (int rc = enqueue_kernels(c, s, st, ni, flags, n, s.windowed)) {
+    return rc;
   }
+  // the head buffers as the run left them: not cleared first, so a head row that no kernel wrote keeps stale values
+  if (enc) CK(cudaMemcpyAsync(enc, s.d_enc, sizeof(float) * (size_t)ni * c->hdr.num_anchors * 4, cudaMemcpyDeviceToHost, st));
+  if (logits)
+    CK(cudaMemcpyAsync(logits, s.d_logits, sizeof(float) * (size_t)ni * c->hdr.num_anchors * (c->hdr.num_classes + 1),
+                       cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (stop_layer >= 0 && layer_out)
+    if (int rc = copy_layer_out(c, s, ni, stop_layer, layer_out, layer_out_floats)) return rc;
+  if (n_images) *n_images = ni;
   c->last_launches = s.launches;
   return 0;
 }

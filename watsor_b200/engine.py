@@ -251,6 +251,30 @@ class Engine:
                                    layer_out.size if layer_out is not None else 0))
         return enc, logits, layer_out
 
+    def backbone_frames(self, frames, cam_ids, stop_layer=-1, layer_shape=None, pixel_format='rgb24',
+                        frames_on_device=False, flags=0):
+        """`backbone` fed as the product path is: frames as `detect` takes them (host arrays, or device pointers with
+        frames_on_device), each camera's detection windows expanded into model images.  stop_layer -1 runs `submit`'s
+        kernels (CUDA graph, post stage, window merge) on slot 0.  Returns (enc, logits, layer_out, n_images); the head
+        buffers are returned as the run left them, without being cleared first."""
+        flags |= self._format_flags(frames, cam_ids, pixel_format)
+        if frames_on_device:
+            flags |= _lib.WB_F_FRAMES_ON_DEVICE
+        windowed = any(c in self.windows for c in cam_ids)
+        n_img = sum(max(len(self.windows.get(c, ())), 1) for c in cam_ids) if windowed else len(cam_ids)
+        n, fp, cams, _, _ = self._io(frames, cam_ids, None, None)
+        enc = np.empty((n_img, self.num_anchors, 4), np.float32)
+        logits = np.empty((n_img, self.num_anchors, self.num_classes + 1), np.float32)
+        layer_out = None
+        if stop_layer >= 0 and layer_shape is not None:
+            layer_out = np.empty((n_img,) + tuple(layer_shape), np.float32)
+        got = c_int32(0)
+        check(self.lib.wb_backbone_frames(self._ctx, n, fp, cams, flags, enc.ctypes.data, logits.ctypes.data,
+                                          stop_layer, layer_out.ctypes.data if layer_out is not None else None,
+                                          layer_out.size if layer_out is not None else 0, byref(got)))
+        assert got.value == n_img, (got.value, n_img)
+        return enc, logits, layer_out, got.value
+
     def postprocess(self, enc, logits, cam_ids, flags=0):
         enc = np.ascontiguousarray(enc, dtype=np.float32)
         logits = np.ascontiguousarray(logits, dtype=np.float32)
