@@ -88,24 +88,10 @@ __global__ void __launch_bounds__(256)
 }
 
 // ------------------------------------------------------------------------------------------- K8
-// TF non_max_suppression_op.cc IOU<float>() -- same op order, separately rounded
-__device__ __forceinline__ float iou_tf(float4 bi, float4 bj) {
-  float ymin_i = fminf(bi.x, bi.z), xmin_i = fminf(bi.y, bi.w);
-  float ymax_i = fmaxf(bi.x, bi.z), xmax_i = fmaxf(bi.y, bi.w);
-  float ymin_j = fminf(bj.x, bj.z), xmin_j = fminf(bj.y, bj.w);
-  float ymax_j = fmaxf(bj.x, bj.z), xmax_j = fmaxf(bj.y, bj.w);
-  float area_i = __fmul_rn(__fsub_rn(ymax_i, ymin_i), __fsub_rn(xmax_i, xmin_i));
-  float area_j = __fmul_rn(__fsub_rn(ymax_j, ymin_j), __fsub_rn(xmax_j, xmin_j));
-  if (area_i <= 0.f || area_j <= 0.f) return 0.f;
-  float iy0 = fmaxf(ymin_i, ymin_j), ix0 = fmaxf(xmin_i, xmin_j);
-  float iy1 = fminf(ymax_i, ymax_j), ix1 = fminf(xmax_i, xmax_j);
-  float inter = __fmul_rn(fmaxf(__fsub_rn(iy1, iy0), 0.f), fmaxf(__fsub_rn(ix1, ix0), 0.f));
-  return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_i, area_j), inter));
-}
-
-// Same predicate as `iou_tf(a, b) > thr` for boxes whose corners were normalised (min/max) and whose areas
-// were computed once: disjoint boxes are rejected after 4 min/max + 2 subtractions, without the IEEE
-// division.  inter = max(dy,0)*max(dx,0) is 0 when dy <= 0 or dx <= 0, so IoU is 0 <= thr there.
+// `IOU(a, b) > thr` of TF non_max_suppression_op.cc (IOU<float>(): same op order, each operation separately rounded)
+// for boxes whose corners were normalised (min/max) and whose areas were computed once: disjoint boxes are rejected
+// after 4 min/max + 2 subtractions, without the IEEE division.  TF's inter = max(dy,0)*max(dx,0) is 0 when dy <= 0 or
+// dx <= 0, so its IoU is 0 <= thr there; it also returns 0 when either area is <= 0.
 struct NBox {
   float4 c;  // ymin, xmin, ymax, xmax (normalised)
   float area;

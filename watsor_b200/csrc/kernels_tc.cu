@@ -386,7 +386,7 @@ int pick_block_n(int n_pad) { return n_pad <= 32 ? 32 : (n_pad <= 64 ? 64 : 128)
 
 }  // namespace
 
-bool tc_layer_supported(const wb_layer& L, int mode) {
+bool tc_layer_supported(const wb_layer& L, int mode, bool conv) {
   // 1x1: the activation and weight rows are K-major tensor maps, whose row stride must be a multiple of 16 bytes
   // (K % 4 in fp32, K % 8 in bf16)
   const int elem = mode == TC_BF16 ? 2 : 4;
@@ -394,17 +394,16 @@ bool tc_layer_supported(const wb_layer& L, int mode) {
     return true;
   // KxK / strided dense convolutions (the SSD extra layers): implicit GEMM, one filter tap x 32 (64 bf16) channels
   // per k-block; a CTA's tile is a whole number of output images, so the maps must be small (<= 128 pixels)
-  return L.op == WB_OP_CONV && L.in_c % 64 == 0 && L.out_h * L.out_w <= (uint32_t)BLOCK_M && L.stride <= 8 &&
-         getenv("WB_NO_TC_CONV") == nullptr;
+  return L.op == WB_OP_CONV && L.in_c % 64 == 0 && L.out_h * L.out_w <= (uint32_t)BLOCK_M && L.stride <= 8 && conv;
 }
 
 int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb_tensor_entry>& tensors,
-                       const float* host_data, int mode, TcWeights* out, std::string* err) {
+                       const float* host_data, int mode, bool conv, TcWeights* out, std::string* err) {
   out->mode = mode;
   out->layers.assign(layers.size(), TcLayerWeights{});
   for (size_t li = 0; li < layers.size(); ++li) {
     const wb_layer& L = layers[li];
-    if (!tc_layer_supported(L, mode)) continue;
+    if (!tc_layer_supported(L, mode, conv)) continue;
     TcLayerWeights& w = out->layers[li];
     const int K = L.kh * L.kw * L.in_c, NP = L.n_pad;             // conv: k = tap * in_c + channel
     const float* src = host_data + tensors[L.w_tensor].offset;  // [K][NP]
@@ -466,7 +465,7 @@ void tc_free_weights(TcWeights* w) {
 
 int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, int n, const wb_layer& L, const void* in,
                    const float* scale, const float* offset, void* out, float* enc, float* logits, int num_anchors,
-                   int num_classes_p1, const void* residual, std::string* err) {
+                   int num_classes_p1, const void* residual, bool split_k, std::string* err) {
   const TcLayerWeights& w = tw.layers[layer_index];
   if (!w.ready) {
     *err = "no tensor-core weights for this layer";
@@ -514,7 +513,7 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
   const long tiles = (long)grid.x * grid.y;
   // the cluster barriers + DSMEM reduction of a split cost several k-blocks' worth of time: splitting only pays for
   // long accumulation chains, and every split keeps >= 8 k-blocks
-  if (tiles < num_sms_hint() / 2 && g.k_blocks >= 16 && getenv("WB_NO_SPLITK") == nullptr) {
+  if (tiles < num_sms_hint() / 2 && g.k_blocks >= 16 && split_k) {
     int want = std::max(1, (int)(num_sms_hint() / tiles));  // at most one wave: tiles * splits <= SMs (a second wave of a
                                                             // few CTAs doubles the kernel's duration)
     int splits = std::min(std::min(want, g.k_blocks / 8), 8);  // 8 = portable thread-block cluster size

@@ -21,14 +21,15 @@ struct TcWeights {
   std::vector<TcLayerWeights> layers;  // indexed by layer number (unset entries for non-GEMM layers)
 };
 
-// whether the tensor-core GEMM of operand mode `mode` (TcMode) runs layer L
-bool tc_layer_supported(const wb_layer& L, int mode);
+// whether the tensor-core GEMM of operand mode `mode` (TcMode) runs layer L; KxK convs only with `conv`
+bool tc_layer_supported(const wb_layer& L, int mode, bool conv);
 int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb_tensor_entry>& tensors,
-                       const float* host_data, int mode, TcWeights* out, std::string* err);
+                       const float* host_data, int mode, bool conv, TcWeights* out, std::string* err);
 void tc_free_weights(TcWeights* w);
+// `split_k`: latency-bound shapes may split K over a thread-block cluster
 int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, int n, const wb_layer& L, const void* in,
                    const float* scale, const float* offset, void* out, float* enc, float* logits, int num_anchors,
-                   int num_classes_p1, const void* residual, std::string* err);
+                   int num_classes_p1, const void* residual, bool split_k, std::string* err);
 
 // generic tiled tensor-map encoder (rank <= 5); `map` points to 128 bytes aligned to 64
 bool tc_encode_map(void* map, const void* base, int elem_bytes, int rank, const unsigned long long* dims,

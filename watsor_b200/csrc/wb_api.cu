@@ -1,5 +1,5 @@
 // wb_api.cu -- the C-ABI of libwatsor_b200.so (include/watsor_b200.h): context, model upload,
-// per-camera filter state, the layer-program executor, two-slot asynchronous pipeline and the
+// per-camera filter state, the layer-program executor, the asynchronous pipeline of WB_SLOTS slots and the
 // stage-level entry points the parity tests use.
 #include <dlfcn.h>
 #include <nccl.h>  // types only: the functions are bound with dlopen in wb_comm_*
@@ -35,36 +35,70 @@ static int fail(const std::string& msg) {
     if (!(cond)) return fail(msg); \
   } while (0)
 
+// An owned CUDA handle (a device or pinned allocation, a stream, an event or a graph exec), released with the Slot,
+// wb_ctx or scope that holds it, so that neither wb_destroy nor an early error return has to list it.  It converts to
+// the raw handle.
+template <typename H, auto Release>
+struct Owned {
+  H h = nullptr;
+  Owned() = default;
+  Owned(const Owned&) = delete;
+  Owned& operator=(const Owned&) = delete;
+  ~Owned() { reset(); }
+  operator H() const { return h; }
+  cudaError_t reset() {
+    const cudaError_t e = h ? Release(h) : cudaSuccess;
+    h = nullptr;
+    return e;
+  }
+};
+template <typename T>
+using DevBuf = Owned<T*, cudaFree>;
+template <typename T>
+using PinnedBuf = Owned<T*, cudaFreeHost>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+
+// (re-)allocate `bytes` of device or pinned memory; the previous allocation is released first
+template <typename T, auto Release>
+static cudaError_t alloc(Owned<T*, Release>& b, size_t bytes) {
+  if (cudaError_t e = b.reset()) return e;
+  return Release == cudaFreeHost ? cudaMallocHost(&b.h, bytes) : cudaMalloc(&b.h, bytes);
+}
+static cudaError_t create(Stream& s) { return cudaStreamCreateWithFlags(&s.h, cudaStreamNonBlocking); }
+static cudaError_t create(Event& e) { return cudaEventCreate(&e.h); }
+
 struct Slot {
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  FrameDesc* h_desc = nullptr;  // pinned
-  FrameDesc* d_desc = nullptr;
-  uint8_t* d_frames = nullptr;
+  Stream stream;
+  Event ev0, ev1;
+  PinnedBuf<FrameDesc> h_desc;
+  DevBuf<FrameDesc> d_desc;
+  DevBuf<uint8_t> d_frames;
   size_t d_frames_cap = 0;
-  void* arena = nullptr;
-  float* d_pre = nullptr;
-  float *d_enc = nullptr, *d_logits = nullptr, *d_dec = nullptr;
-  float* d_partial = nullptr;  // split-K scratch
+  DevBuf<void> arena;
+  DevBuf<float> d_enc, d_logits, d_dec;
+  DevBuf<float> d_partial;  // split-K scratch
   size_t partial_floats = 0;
-  int *d_cand_count = nullptr, *d_sel_count = nullptr;
-  int* d_kept_hist = nullptr;  // [B][1024] per-frame histogram of kept scores (exact NMS early exit)
-  unsigned long long *d_cand = nullptr, *d_sel = nullptr;
-  wb_detection *d_out = nullptr, *h_out = nullptr;
-  uint32_t *d_verdicts = nullptr, *h_verdicts = nullptr;
-  float *d_raw = nullptr, *h_raw = nullptr;  // boxes[n][100][4] scores[n][100] classes[n][100]
-  int *d_raw_num = nullptr, *h_raw_num = nullptr;
+  DevBuf<int> d_cand_count, d_sel_count;
+  DevBuf<int> d_kept_hist;  // [B][1024] per-frame histogram of kept scores (exact NMS early exit)
+  DevBuf<unsigned long long> d_cand, d_sel;
+  DevBuf<wb_detection> d_out;
+  PinnedBuf<wb_detection> h_out;
+  DevBuf<uint32_t> d_verdicts;
+  PinnedBuf<uint32_t> h_verdicts;
+  DevBuf<int> d_raw_num;  // valid rows per image: wb_postprocess's `num`, and k_window_merge's input
   // batches with detection windows: the frames' windows (copied before every launch) and their merged rows
-  WindowFrame *h_win = nullptr, *d_win = nullptr;
-  wb_detection* d_wout = nullptr;
-  uint32_t* d_wverd = nullptr;
+  PinnedBuf<WindowFrame> h_win;
+  DevBuf<WindowFrame> d_win;
+  DevBuf<wb_detection> d_wout;
+  DevBuf<uint32_t> d_wverd;
   int n = 0;         // frames of the batch in flight
   bool windowed = false;
   uint32_t flags = 0;
   bool busy = false;
   int launches = 0;
   // CUDA graph of the kernel sequence, keyed by (model images, flags, frames, windowed)
-  cudaGraphExec_t graph_exec = nullptr;
+  Owned<cudaGraphExec_t, cudaGraphExecDestroy> graph_exec;
   int graph_n = -1;
   int graph_frames = -1;
   bool graph_windowed = false;
@@ -75,22 +109,26 @@ struct wb_ctx {
   int device = 0;
   int max_batch = 0;
   int precision = 0;
-  bool use_graph = true;
+  // path switches (INTEGRATION.md §4), read from the environment once, in wb_create: an engine keeps the paths it was
+  // created with, and routes to the tensor cores exactly the layers whose weights it prepared for them
+  struct {
+    bool graph, fuse_dwpw, fuse_add, tc_conv, split_k;
+  } sw;
   // frame scatter (wb_comm_*): NCCL communicator bound at run time, its stream and the event the slots wait on
   void* comm = nullptr;
   int comm_rank = -1, comm_world = 0;
-  cudaStream_t comm_stream = nullptr;
-  cudaEvent_t comm_ev = nullptr;
+  Stream comm_stream;
+  Event comm_ev;
   cudaDeviceProp prop;
   wb_model_header hdr;
   std::vector<wb_layer> layers;
   std::vector<wb_tensor_entry> tensors;
-  float* d_weights = nullptr;
+  DevBuf<float> d_weights;
   TcWeights tc;  // bf16 copies of the GEMM weights (precision 1)
   PostParams pp;
-  CameraCfg* d_cams = nullptr;
+  DevBuf<CameraCfg> d_cams;
   std::vector<CameraCfg> h_cams;
-  std::vector<int32_t*> cam_sat;
+  DevBuf<int32_t> cam_sat[WB_MAX_CAMERAS];
   std::vector<std::vector<int4>> cam_windows;  // wb_set_camera_windows: (x, y, w, h) per window
   std::vector<double> cam_merge_thr;
   Slot slots[WB_SLOTS];
@@ -106,14 +144,22 @@ struct wb_ctx {
   // results are back.
   std::mutex mu;
   // wb_filter_rows: its own stream and staging buffers (never slot 0's: a detector batch may be in flight there)
-  cudaStream_t fstream = nullptr;
-  wb_detection* d_frows = nullptr;
-  uint32_t* d_fverd = nullptr;
+  Stream fstream;
+  DevBuf<wb_detection> d_frows;
+  DevBuf<uint32_t> d_fverd;
   int frows_cap = 0;
+  // read by the stage hooks only, which run on slot 0: wb_backbone's pre-processed input and wb_postprocess's float
+  // outputs, boxes[n][100][4] scores[n][100] classes[n][100] and the valid rows per image
+  DevBuf<float> d_pre;
+  DevBuf<float> d_raw;
+  PinnedBuf<float> h_raw;
+  PinnedBuf<int> h_raw_num;
 
   const float* tensor(int idx) const { return d_weights + tensors[idx].offset; }
   size_t elem_size() const { return precision == 1 ? 2 : 4; }
   cudaStream_t stream_of(int s) { return has_user_stream ? user_stream : slots[s].stream; }
+  // whether layer L runs on the tensor-core GEMM
+  bool tc_runs(const wb_layer& L) const { return precision != 0 && tc_layer_supported(L, tc.mode, sw.tc_conv); }
 };
 
 extern "C" {
@@ -135,36 +181,32 @@ int wb_device_count(int* count) {
 
 static int alloc_slot(wb_ctx* c, Slot& s) {
   const int B = c->max_batch, N = c->hdr.num_anchors, C = c->hdr.num_classes, MP = c->hdr.max_per_class;
-  CK(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-  CK(cudaEventCreate(&s.ev0));
-  CK(cudaEventCreate(&s.ev1));
-  CK(cudaMallocHost(&s.h_desc, sizeof(FrameDesc) * B));
-  CK(cudaMalloc(&s.d_desc, sizeof(FrameDesc) * B));
-  CK(cudaMalloc(&s.arena, (size_t)B * c->hdr.arena_elems * c->elem_size() + 1024));
-  CK(cudaMalloc(&s.d_pre, sizeof(float) * (size_t)B * c->hdr.input_h * c->hdr.input_w * 3));
-  CK(cudaMalloc(&s.d_enc, sizeof(float) * (size_t)B * N * 4));
-  CK(cudaMalloc(&s.d_logits, sizeof(float) * (size_t)B * N * (C + 1)));
-  CK(cudaMalloc(&s.d_dec, sizeof(float) * (size_t)B * N * 4));
+  CK(create(s.stream));
+  CK(create(s.ev0));
+  CK(create(s.ev1));
+  CK(alloc(s.h_desc, sizeof(FrameDesc) * B));
+  CK(alloc(s.d_desc, sizeof(FrameDesc) * B));
+  CK(alloc(s.arena, (size_t)B * c->hdr.arena_elems * c->elem_size() + 1024));
+  CK(alloc(s.d_enc, sizeof(float) * (size_t)B * N * 4));
+  CK(alloc(s.d_logits, sizeof(float) * (size_t)B * N * (C + 1)));
+  CK(alloc(s.d_dec, sizeof(float) * (size_t)B * N * 4));
   s.partial_floats = (size_t)4 * 1024 * 1024 + (size_t)B * 512 * 1024;
-  CK(cudaMalloc(&s.d_partial, sizeof(float) * s.partial_floats));
-  CK(cudaMalloc(&s.d_cand_count, sizeof(int) * (size_t)B * C));
-  CK(cudaMalloc(&s.d_sel_count, sizeof(int) * (size_t)B * C));
-  CK(cudaMalloc(&s.d_kept_hist, sizeof(int) * (size_t)B * 1024));
-  CK(cudaMalloc(&s.d_cand, sizeof(unsigned long long) * (size_t)B * C * N));
-  CK(cudaMalloc(&s.d_sel, (sizeof(unsigned long long) + sizeof(int)) * (size_t)B * C * MP));
-  CK(cudaMalloc(&s.d_out, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
-  CK(cudaMallocHost(&s.h_out, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
-  CK(cudaMalloc(&s.d_verdicts, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
-  CK(cudaMallocHost(&s.h_verdicts, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
-  CK(cudaMalloc(&s.d_raw, sizeof(float) * (size_t)B * WB_MAX_DETECTIONS * 6));
-  CK(cudaMallocHost(&s.h_raw, sizeof(float) * (size_t)B * WB_MAX_DETECTIONS * 6));
-  CK(cudaMalloc(&s.d_raw_num, sizeof(int) * B));
-  CK(cudaMallocHost(&s.h_raw_num, sizeof(int) * B));
-  CK(cudaMallocHost(&s.h_win, sizeof(WindowFrame) * B));
-  CK(cudaMalloc(&s.d_win, sizeof(WindowFrame) * B));
-  CK(cudaMalloc(&s.d_wout, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(alloc(s.d_partial, sizeof(float) * s.partial_floats));
+  CK(alloc(s.d_cand_count, sizeof(int) * (size_t)B * C));
+  CK(alloc(s.d_sel_count, sizeof(int) * (size_t)B * C));
+  CK(alloc(s.d_kept_hist, sizeof(int) * (size_t)B * 1024));
+  CK(alloc(s.d_cand, sizeof(unsigned long long) * (size_t)B * C * N));
+  CK(alloc(s.d_sel, (sizeof(unsigned long long) + sizeof(int)) * (size_t)B * C * MP));
+  CK(alloc(s.d_out, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(alloc(s.h_out, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(alloc(s.d_verdicts, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(alloc(s.h_verdicts, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(alloc(s.d_raw_num, sizeof(int) * B));
+  CK(alloc(s.h_win, sizeof(WindowFrame) * B));
+  CK(alloc(s.d_win, sizeof(WindowFrame) * B));
+  CK(alloc(s.d_wout, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
   CK(cudaMemset(s.d_wout, 0, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
-  CK(cudaMalloc(&s.d_wverd, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
+  CK(alloc(s.d_wverd, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
   return 0;
 }
 
@@ -184,7 +226,12 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   c->device = device;
   c->max_batch = max_batch;
   c->precision = precision;
-  if (const char* g = getenv("WB_NO_GRAPH")) c->use_graph = !(g[0] == '1');
+  const char* no_graph = getenv("WB_NO_GRAPH");
+  c->sw.graph = !(no_graph && no_graph[0] == '1');
+  c->sw.fuse_dwpw = getenv("WB_NO_FUSE") == nullptr;
+  c->sw.fuse_add = getenv("WB_NO_FUSE_ADD") == nullptr;
+  c->sw.tc_conv = getenv("WB_NO_TC_CONV") == nullptr;
+  c->sw.split_k = getenv("WB_NO_SPLITK") == nullptr;
   CK(cudaGetDeviceProperties(&c->prop, device));
   REQUIRE(c->prop.major == 9 && c->prop.minor == 0, std::string("libwatsor_b200 is built for sm_90a only; device is ") +
                                    c->prop.name + " (sm_" + std::to_string(c->prop.major) +
@@ -226,12 +273,12 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
               "channel copy: slice must be 4-aligned and inside the destination");
     REQUIRE(L.op >= WB_OP_STEM && L.op <= WB_OP_COPY, std::string("layer ") + L.name + ": unknown op");
   }
-  CK(cudaMalloc(&c->d_weights, floats * sizeof(float)));
+  CK(alloc(c->d_weights, floats * sizeof(float)));
   CK(cudaMemcpy(c->d_weights, p, floats * sizeof(float), cudaMemcpyHostToDevice));
   if (precision != 0) {
     std::string err;
     const int mode = precision == 1 ? TC_BF16 : (precision == 2 ? TC_TF32X3 : TC_TF32X1);
-    if (tc_prepare_weights(c->layers, c->tensors, reinterpret_cast<const float*>(p), mode, &c->tc, &err))
+    if (tc_prepare_weights(c->layers, c->tensors, reinterpret_cast<const float*>(p), mode, c->sw.tc_conv, &c->tc, &err))
       return fail("tensor-core weight preparation: " + err);
   }
   c->pp.num_anchors = c->hdr.num_anchors;
@@ -247,17 +294,20 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   c->pp.max_total = c->hdr.max_total;
   c->pp.class_offset = c->hdr.class_offset;
   c->h_cams.assign(WB_MAX_CAMERAS, CameraCfg{});
-  c->cam_sat.assign(WB_MAX_CAMERAS, nullptr);
   c->cam_windows.assign(WB_MAX_CAMERAS, {});
   c->cam_merge_thr.assign(WB_MAX_CAMERAS, 0.5);
-  CK(cudaMalloc(&c->d_cams, sizeof(CameraCfg) * WB_MAX_CAMERAS));
+  CK(alloc(c->d_cams, sizeof(CameraCfg) * WB_MAX_CAMERAS));
   CK(cudaMemset(c->d_cams, 0, sizeof(CameraCfg) * WB_MAX_CAMERAS));
   for (int s = 0; s < WB_SLOTS; ++s)
     if (alloc_slot(c, c->slots[s])) return 1;
   c->frows_cap = WB_MAX_DETECTIONS * max_batch;
-  CK(cudaStreamCreateWithFlags(&c->fstream, cudaStreamNonBlocking));
-  CK(cudaMalloc(&c->d_frows, sizeof(wb_detection) * (size_t)c->frows_cap));
-  CK(cudaMalloc(&c->d_fverd, sizeof(uint32_t) * (size_t)c->frows_cap));
+  CK(create(c->fstream));
+  CK(alloc(c->d_frows, sizeof(wb_detection) * (size_t)c->frows_cap));
+  CK(alloc(c->d_fverd, sizeof(uint32_t) * (size_t)c->frows_cap));
+  CK(alloc(c->d_pre, sizeof(float) * (size_t)max_batch * c->hdr.input_h * c->hdr.input_w * 3));
+  CK(alloc(c->d_raw, sizeof(float) * (size_t)max_batch * WB_MAX_DETECTIONS * 6));
+  CK(alloc(c->h_raw, sizeof(float) * (size_t)max_batch * WB_MAX_DETECTIONS * 6));
+  CK(alloc(c->h_raw_num, sizeof(int) * max_batch));
   CK(cudaDeviceSynchronize());
   *out = guard.release();
   return 0;
@@ -269,46 +319,9 @@ int wb_destroy(wb_ctx* c) {
   cudaDeviceSynchronize();
   wb_comm_destroy(c);
   for (void* r : c->registered) cudaHostUnregister(r);
-  for (auto& s : c->slots) {
-    if (s.graph_exec) cudaGraphExecDestroy(s.graph_exec);
-    cudaFree(s.d_desc);
-    cudaFree(s.d_frames);
-    cudaFree(s.arena);
-    cudaFree(s.d_pre);
-    cudaFree(s.d_enc);
-    cudaFree(s.d_logits);
-    cudaFree(s.d_dec);
-    cudaFree(s.d_partial);
-    cudaFree(s.d_cand_count);
-    cudaFree(s.d_sel_count);
-    cudaFree(s.d_kept_hist);
-    cudaFree(s.d_cand);
-    cudaFree(s.d_sel);
-    cudaFree(s.d_out);
-    cudaFree(s.d_verdicts);
-    cudaFree(s.d_raw);
-    cudaFree(s.d_raw_num);
-    cudaFree(s.d_win);
-    cudaFree(s.d_wout);
-    cudaFree(s.d_wverd);
-    cudaFreeHost(s.h_win);
-    cudaFreeHost(s.h_desc);
-    cudaFreeHost(s.h_out);
-    cudaFreeHost(s.h_verdicts);
-    cudaFreeHost(s.h_raw);
-    cudaFreeHost(s.h_raw_num);
-    if (s.ev0) cudaEventDestroy(s.ev0);
-    if (s.ev1) cudaEventDestroy(s.ev1);
-    if (s.stream) cudaStreamDestroy(s.stream);
-  }
-  for (auto* p : c->cam_sat) cudaFree(p);
-  cudaFree(c->d_cams);
-  cudaFree(c->d_frows);
-  cudaFree(c->d_fverd);
-  if (c->fstream) cudaStreamDestroy(c->fstream);
-  cudaFree(c->d_weights);
+  for (auto& s : c->slots) s.graph_exec.reset();
   tc_free_weights(&c->tc);
-  delete c;
+  delete c;  // releases the owned buffers, streams and events
   return 0;
 }
 
@@ -380,23 +393,19 @@ int wb_set_camera(wb_ctx* c, int cam, int width, int height, int n_zones, const 
     cfg.has_zone_list[f.label] = f.has_zone_list ? 1 : 0;
     cfg.zone_bits[f.label] = f.zone_bits;
   }
-  if (c->cam_sat[cam]) {
-    CK(cudaFree(c->cam_sat[cam]));
-    c->cam_sat[cam] = nullptr;
-  }
+  CK(c->cam_sat[cam].reset());
   if (n_zones > 0) {
     size_t sat_elems = (size_t)n_zones * (height + 1) * (width + 1);
-    CK(cudaMalloc(&c->cam_sat[cam], sat_elems * sizeof(int32_t)));
-    uint8_t* d_r = nullptr;
+    CK(alloc(c->cam_sat[cam], sat_elems * sizeof(int32_t)));
+    DevBuf<uint8_t> d_r;
     size_t rb = (size_t)n_zones * height * width;
-    CK(cudaMalloc(&d_r, rb));
+    CK(alloc(d_r, rb));
     CK(cudaMemcpy(d_r, raster, rb, cudaMemcpyHostToDevice));
     int lcnt = 0;
     LaunchCtx lc{c->slots[0].stream, &lcnt};
     launch_build_sat(lc, d_r, n_zones, height, width, c->cam_sat[cam]);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(c->slots[0].stream));
-    CK(cudaFree(d_r));
     cfg.sat = c->cam_sat[cam];
   }
   c->h_cams[cam] = cfg;
@@ -462,6 +471,8 @@ enum SpanKind {
 struct Span {
   size_t last;  // last layer of the span
   SpanKind kind;
+  uint32_t out_off;        // arena offset the span's kernel writes: the output of layer `last`
+  long long residual_off;  // arena offset of the residual Add's other input (the shortcut), or -1: no Add
 };
 
 // a fused kernel reads the arena range of `reader`'s input while it writes that of `writer`'s output
@@ -478,41 +489,48 @@ static Span fused_span(const wb_ctx* c, size_t li, size_t end) {
   const wb_layer& L = Ls[li];
   // layer p + 1 is `Add(shortcut, output of p)` (fp32 modes: the shortcut can be added in an fp32 epilogue)
   auto residual_add_after = [&](size_t p) {
-    if (c->precision == 0 || c->precision == 1 || p + 1 >= end || getenv("WB_NO_FUSE_ADD") != nullptr) return false;
+    if (c->precision == 0 || c->precision == 1 || p + 1 >= end || !c->sw.fuse_add) return false;
     const wb_layer& P = Ls[p], &A = Ls[p + 1];
     return P.op == WB_OP_PW && P.act == WB_ACT_NONE && A.op == WB_OP_ADD &&
            (A.in_off == P.out_off || A.in2_off == P.out_off) && A.in_off != A.in2_off;
   };
-  if (L.op == WB_OP_DW && c->precision == 2 && li + 1 < end && getenv("WB_NO_FUSE") == nullptr) {
+  // layers [li, last]; a span ending in an Add adds the Add's other input to the output of layer last - 1
+  auto span = [&](size_t last, SpanKind kind) {
+    const wb_layer& A = Ls[last];
+    long long residual_off = -1;
+    if (kind == SPAN_DW_PW_ADD || kind == SPAN_PW_ADD) residual_off = A.in_off == Ls[last - 1].out_off ? A.in2_off : A.in_off;
+    return Span{last, kind, A.out_off, residual_off};
+  };
+  if (L.op == WB_OP_DW && c->precision == 2 && li + 1 < end && c->sw.fuse_dwpw) {
     const wb_layer& P = Ls[li + 1];
     if (P.in_off == L.out_off && fused_dwpw_supported(c->tc, (int)li + 1, L, P)) {
       if (residual_add_after(li + 1)) {
-        if (arena_disjoint(L, Ls[li + 2])) return {li + 2, SPAN_DW_PW_ADD};
+        if (arena_disjoint(L, Ls[li + 2])) return span(li + 2, SPAN_DW_PW_ADD);
       } else if (arena_disjoint(L, P)) {
-        return {li + 1, SPAN_DW_PW};
+        return span(li + 1, SPAN_DW_PW);
       }
     }
   }
-  if (L.op == WB_OP_PW && c->precision != 0 && tc_layer_supported(L, c->tc.mode) && residual_add_after(li) &&
-      arena_disjoint(L, Ls[li + 1]))
-    return {li + 1, SPAN_PW_ADD};
-  return {li, SPAN_ONE};
+  if (L.op == WB_OP_PW && c->tc_runs(L) && residual_add_after(li) && arena_disjoint(L, Ls[li + 1]))
+    return span(li + 1, SPAN_PW_ADD);
+  return span(li, SPAN_ONE);
 }
 
 // the layer program.  `pre` != NULL feeds an already pre-processed input (wb_backbone); otherwise the
-// fused stem samples the frames directly.  When `times` is given every launch is bracketed by events.
+// fused stem samples the frames directly.
 template <typename T>
 static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* pre, int first_layer,
                       int last_layer) {
   LaunchCtx lc{st, &s.launches};
-  T* arena = static_cast<T*>(s.arena);
+  // the n images' tensor at arena offset `off`
+  auto at = [&](long long off) { return static_cast<T*>(s.arena.h) + (size_t)off * n; };
   const int NA = c->hdr.num_anchors, C1 = c->hdr.num_classes + 1;
   const size_t end = last_layer < 0 ? c->layers.size() : (size_t)last_layer + 1;
   for (size_t li = (size_t)first_layer; li < end; ++li) {
     const wb_layer& L = c->layers[li];
-    const T* in = arena + (size_t)L.in_off * n;
-    const T* in2 = arena + (size_t)L.in2_off * n;
-    T* outp = arena + (size_t)L.out_off * n;
+    const T* in = at(L.in_off);
+    const T* in2 = at(L.in2_off);
+    T* outp = at(L.out_off);
     const float* w = L.w_tensor >= 0 ? c->tensor(L.w_tensor) : nullptr;
     const float* sc = L.scale_tensor >= 0 ? c->tensor(L.scale_tensor) : nullptr;
     const float* of = L.offset_tensor >= 0 ? c->tensor(L.offset_tensor) : nullptr;
@@ -525,15 +543,12 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
         const Span sp = fused_span(c, li, end);
         if (sp.kind == SPAN_DW_PW || sp.kind == SPAN_DW_PW_ADD) {
           const wb_layer& P = c->layers[li + 1];
-          const wb_layer& O = c->layers[sp.last];  // the layer whose output the kernel writes
-          const float* residual = nullptr;
-          if (sp.kind == SPAN_DW_PW_ADD)
-            residual = reinterpret_cast<const float*>(arena + (size_t)(O.in_off == P.out_off ? O.in2_off : O.in_off) * n);
+          const float* residual = sp.residual_off < 0 ? nullptr : reinterpret_cast<const float*>(at(sp.residual_off));
           std::string err;
           if (fused_launch_dwpw(lc, c->tc, (int)li + 1, n, L, P, static_cast<const void*>(in), w, sc, of,
                                 c->tensor(P.scale_tensor), c->tensor(P.offset_tensor), residual,
-                                static_cast<void*>(arena + (size_t)O.out_off * n), &err))
-            return fail("layers " + std::string(L.name) + " .. " + O.name + ": " + err);
+                                static_cast<void*>(at(sp.out_off)), &err))
+            return fail("layers " + std::string(L.name) + " .. " + c->layers[sp.last].name + ": " + err);
           li = sp.last;
           break;
         }
@@ -553,23 +568,16 @@ static int run_layers(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* p
       case WB_OP_PW:
       case WB_OP_CONV:
       case WB_OP_HEAD:
-        if (c->precision != 0 && tc_layer_supported(L, c->tc.mode)) {
+        if (c->tc_runs(L)) {
           // MobileNet-v2 bottleneck: a linear projection followed by `Add(shortcut, projection)` runs as one kernel,
           // the shortcut is added in the GEMM epilogue (fp32 modes) and the Add layer is skipped
-          const void* residual = nullptr;
-          void* dst = static_cast<void*>(outp);
-          const bool fuse_add = fused_span(c, li, end).kind == SPAN_PW_ADD;
-          if (fuse_add) {
-            const wb_layer& A = c->layers[li + 1];
-            const uint32_t other = A.in_off == L.out_off ? A.in2_off : A.in_off;
-            residual = static_cast<const void*>(arena + (size_t)other * n);
-            dst = static_cast<void*>(arena + (size_t)A.out_off * n);
-          }
+          const Span sp = fused_span(c, li, end);
+          const void* residual = sp.residual_off < 0 ? nullptr : static_cast<const void*>(at(sp.residual_off));
           std::string err;
-          if (tc_launch_gemm(lc, c->tc, (int)li, n, L, static_cast<const void*>(in), sc, of, dst, s.d_enc, s.d_logits, NA,
-                             C1, residual, &err))
+          if (tc_launch_gemm(lc, c->tc, (int)li, n, L, static_cast<const void*>(in), sc, of, static_cast<void*>(at(sp.out_off)),
+                             s.d_enc, s.d_logits, NA, C1, residual, c->sw.split_k, &err))
             return fail("layer " + std::string(L.name) + ": " + err);
-          if (fuse_add) ++li;  // the Add layer is done
+          li = sp.last;  // past the Add when it was fused
         } else {
           launch_gemm_cc<T>(lc, n, L, in, w, sc, of, outp, s.d_enc, s.d_logits, NA, C1, s.d_partial, s.partial_floats);
         }
@@ -589,22 +597,26 @@ static int run_post(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, 
   LaunchCtx lc{st, &s.launches};
   // the float boxes / scores / classes of `sess.run` are a test hook (wb_postprocess); the product path writes
   // Detection rows only
-  float* rb = want_raw ? s.d_raw : nullptr;
+  float* rb = want_raw ? c->d_raw.h : nullptr;
   float* rs = want_raw ? rb + (size_t)c->max_batch * WB_MAX_DETECTIONS * 4 : nullptr;
   float* rc = want_raw ? rs + (size_t)c->max_batch * WB_MAX_DETECTIONS : nullptr;
   launch_post(lc, n, c->pp, s.d_enc, s.d_logits, c->tensor(c->hdr.anchors_tensor), s.d_desc,
-              windowed ? nullptr : c->d_cams, flags, s.d_dec, s.d_cand_count, s.d_cand, s.d_sel_count, s.d_sel, s.d_out,
-              s.d_verdicts, rb, rs, rc, (want_raw || windowed) ? s.d_raw_num : nullptr, s.d_kept_hist);
+              windowed ? nullptr : c->d_cams.h, flags, s.d_dec, s.d_cand_count, s.d_cand, s.d_sel_count, s.d_sel, s.d_out,
+              s.d_verdicts, rb, rs, rc, (want_raw || windowed) ? s.d_raw_num.h : nullptr, s.d_kept_hist);
   if (windowed)
     launch_window_merge(lc, n_frames, c->pp, s.d_win, s.d_out, s.d_raw_num, c->d_cams, flags, s.d_wout, s.d_wverd);
   CK(cudaGetLastError());
   return 0;
 }
 
+// layers first..last (last < 0: to the end) in the engine's activation type
+static int run_program(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* pre, int first, int last) {
+  return c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, n, pre, first, last)
+                           : run_layers<float>(c, s, st, n, pre, first, last);
+}
+
 static int run_all(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, int n_frames, bool windowed) {
-  int rc = c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, n, nullptr, 0, -1)
-                             : run_layers<float>(c, s, st, n, nullptr, 0, -1);
-  if (rc) return rc;
+  if (int rc = run_program(c, s, st, n, nullptr, 0, -1)) return rc;
   return run_post(c, s, st, n, flags, false, n_frames, windowed);
 }
 
@@ -613,16 +625,13 @@ static int run_all(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, i
 // launch, so one graph serves RGB24 and 4:2:0 batches alike.
 static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, int n_frames, bool windowed) {
   const uint32_t gflags = flags & WB_F_FUSE_FILTERS;
-  if (!c->use_graph) {
+  if (!c->sw.graph) {
     s.launches = 0;
     return run_all(c, s, st, n, gflags, n_frames, windowed);
   }
   if (s.graph_exec == nullptr || s.graph_n != n || s.graph_flags != gflags || s.graph_frames != n_frames ||
       s.graph_windowed != windowed) {
-    if (s.graph_exec) {
-      cudaGraphExecDestroy(s.graph_exec);
-      s.graph_exec = nullptr;
-    }
+    s.graph_exec.reset();
     // warm-up run outside capture (sets function attributes, validates launches)
     s.launches = 0;
     if (int rc = run_all(c, s, st, n, gflags, n_frames, windowed)) return rc;
@@ -634,7 +643,7 @@ static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t 
     cudaError_t e = cudaStreamEndCapture(st, &graph);
     if (rc) return rc;
     if (e != cudaSuccess) return fail(std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e));
-    CK(cudaGraphInstantiate(&s.graph_exec, graph, 0));
+    CK(cudaGraphInstantiate(&s.graph_exec.h, graph, 0));
     CK(cudaGraphDestroy(graph));
     s.graph_n = n;
     s.graph_flags = gflags;
@@ -652,6 +661,26 @@ static int frame_format(uint32_t flags, int* fmt) {
   return 0;
 }
 
+// Copies n host frames of bytes[i] each to s.d_frames, 256-byte aligned, and points dev[i] at frame i's copy.  A buffer
+// that is too small is replaced, once the stream is done with it, by one with 25 % headroom.
+static int upload_frames(Slot& s, cudaStream_t st, int n, const uint8_t* const* frames, const size_t* bytes,
+                         const uint8_t** dev) {
+  size_t total = 0;
+  for (int i = 0; i < n; ++i) total += (bytes[i] + 255) / 256 * 256;
+  if (total > s.d_frames_cap) {
+    CK(cudaStreamSynchronize(st));
+    s.d_frames_cap = total + total / 4;
+    CK(alloc(s.d_frames, s.d_frames_cap));
+  }
+  size_t off = 0;
+  for (int i = 0; i < n; ++i) {
+    dev[i] = s.d_frames + off;
+    CK(cudaMemcpyAsync(s.d_frames + off, frames[i], bytes[i], cudaMemcpyHostToDevice, st));
+    off += (bytes[i] + 255) / 256 * 256;
+  }
+  return 0;
+}
+
 // One descriptor per model image.  With use_windows and at least one camera of the batch having detection windows, the
 // batch is windowed: every window of a frame is one image (a camera without windows: one full-frame window, camera
 // -1), and s.h_win / s.d_win describe the frames for k_window_merge.  Otherwise an image is a frame, as always.  A host
@@ -659,7 +688,7 @@ static int frame_format(uint32_t flags, int* fmt) {
 // caller's device frame).
 static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, const int32_t* cam_ids,
                      bool on_device, int fmt, cudaStream_t st, bool use_windows, int* n_images_out) {
-  size_t total = 0;
+  std::vector<size_t> bytes(n);
   bool windowed = false;
   int n_images = 0;
   for (int i = 0; i < n; ++i) {
@@ -671,7 +700,7 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
     REQUIRE(fmt == WB_FMT_RGB24 || (cc.width % 2 == 0 && cc.height % 2 == 0),
             "cam_id " + std::to_string(cam) + " is " + std::to_string(cc.width) + "x" + std::to_string(cc.height) +
                 ": 4:2:0 frames need an even width and height");
-    total += (frame_bytes(fmt, cc.width, cc.height) + 255) / 256 * 256;
+    bytes[i] = frame_bytes(fmt, cc.width, cc.height);
     const int nw = use_windows ? (int)c->cam_windows[cam].size() : 0;
     windowed |= nw > 0;
     n_images += std::max(nw, 1);
@@ -686,26 +715,17 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
   REQUIRE(n_images <= c->max_batch, "the batch's detection windows add up to " + std::to_string(n_images) +
                                         " model images, more than max_batch (" + std::to_string(c->max_batch) + ")");
   if (!windowed) n_images = n;
-  if (!on_device && frames != nullptr && total > s.d_frames_cap) {
-    CK(cudaStreamSynchronize(st));
-    if (s.d_frames) CK(cudaFree(s.d_frames));
-    s.d_frames_cap = total + total / 4;
-    CK(cudaMalloc(&s.d_frames, s.d_frames_cap));
+  std::vector<const uint8_t*> dev(n, nullptr);  // each frame on the device
+  if (frames != nullptr && on_device) {
+    dev.assign(frames, frames + n);
+  } else if (frames != nullptr) {
+    if (int rc = upload_frames(s, st, n, frames, bytes.data(), dev.data())) return rc;
   }
-  size_t off = 0;
   int img = 0;
   for (int i = 0; i < n; ++i) {
     const int cam = cam_ids[i];
     const CameraCfg& cc = c->h_cams[cam];
-    const size_t bytes = frame_bytes(fmt, cc.width, cc.height);
-    const uint8_t* base = nullptr;
-    if (frames != nullptr && on_device) {
-      base = frames[i];
-    } else if (frames != nullptr) {
-      base = s.d_frames + off;
-      CK(cudaMemcpyAsync(s.d_frames + off, frames[i], bytes, cudaMemcpyHostToDevice, st));
-      off += (bytes + 255) / 256 * 256;
-    }
+    const uint8_t* base = dev[i];
     const ChromaLayout cl = chroma_layout(fmt, cc.width, cc.height);
     const int bpp = fmt == WB_FMT_RGB24 ? 3 : 1;  // bytes per pixel of the RGB24 / luma plane
     const std::vector<int4>& wins = c->cam_windows[cam];
@@ -743,6 +763,23 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
   if (n_images_out) *n_images_out = n_images;
   return 0;
 }
+
+// The stage hooks (wb_preprocess, wb_backbone, wb_backbone_frames, wb_postprocess, wb_profile_layers) run
+// synchronously on slot 0 and hold the context lock throughout.  The guard takes the lock and makes the context's
+// device current; `rc` is non-zero when that fails, the batch of n images does not fit or slot 0 has a batch in flight.
+struct StageHook {
+  std::lock_guard<std::mutex> lock;
+  Slot& s;
+  cudaStream_t st;
+  int rc;
+  StageHook(wb_ctx* c, int n) : lock(c->mu), s(c->slots[0]), st(c->stream_of(0)), rc(enter(c, n)) {}
+  static int enter(wb_ctx* c, int n) {
+    REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range");
+    CK(cudaSetDevice(c->device));
+    REQUIRE(!c->slots[0].busy, "slot 0 is busy");
+    return 0;
+  }
+};
 
 extern "C" {
 
@@ -817,8 +854,8 @@ int wb_stream_fence(wb_ctx* c, uint64_t stream, int direction) {
   REQUIRE(direction == 0 || direction == 1, "direction must be 0 or 1");
   CK(cudaSetDevice(c->device));
   cudaStream_t user = reinterpret_cast<cudaStream_t>(stream);
-  cudaEvent_t ev;
-  CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  Event ev;
+  CK(cudaEventCreateWithFlags(&ev.h, cudaEventDisableTiming));
   if (direction == 0) {
     CK(cudaEventRecord(ev, user));
     for (auto& s : c->slots) CK(cudaStreamWaitEvent(s.stream, ev, 0));
@@ -828,7 +865,6 @@ int wb_stream_fence(wb_ctx* c, uint64_t stream, int direction) {
       CK(cudaStreamWaitEvent(user, ev, 0));
     }
   }
-  CK(cudaEventDestroy(ev));
   return 0;
 }
 
@@ -842,32 +878,22 @@ int wb_detect(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t* cam
 int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t* widths, const int32_t* heights,
                   float* out) {
   REQUIRE(c && frames && widths && heights && out, "NULL argument");
-  REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range");
-  std::lock_guard<std::mutex> lock(c->mu);
-  CK(cudaSetDevice(c->device));
-  Slot& s = c->slots[0];
-  REQUIRE(!s.busy, "slot 0 is busy");
-  cudaStream_t st = c->stream_of(0);
-  size_t total = 0;
-  for (int i = 0; i < n; ++i) total += (size_t)widths[i] * heights[i] * 3;
-  if (total > s.d_frames_cap) {
-    if (s.d_frames) CK(cudaFree(s.d_frames));
-    s.d_frames_cap = total;
-    CK(cudaMalloc(&s.d_frames, total));
-  }
-  size_t off = 0;
-  for (int i = 0; i < n; ++i) {
-    size_t bytes = (size_t)widths[i] * heights[i] * 3;
-    CK(cudaMemcpyAsync(s.d_frames + off, frames[i], bytes, cudaMemcpyHostToDevice, st));
-    s.h_desc[i] = FrameDesc{s.d_frames + off, s.d_frames + off + (size_t)widths[i] * heights[i], widths[i], heights[i],
-                            widths[i] * 3, -1, WB_FMT_RGB24, 0};
-    off += bytes;
-  }
+  StageHook h(c, n);
+  if (h.rc) return h.rc;
+  Slot& s = h.s;
+  cudaStream_t st = h.st;
+  std::vector<size_t> bytes(n);
+  for (int i = 0; i < n; ++i) bytes[i] = (size_t)widths[i] * heights[i] * 3;
+  std::vector<const uint8_t*> dev(n);
+  if (int rc = upload_frames(s, st, n, frames, bytes.data(), dev.data())) return rc;
+  for (int i = 0; i < n; ++i)
+    s.h_desc[i] = FrameDesc{dev[i], dev[i] + (size_t)widths[i] * heights[i], widths[i], heights[i], widths[i] * 3, -1,
+                            WB_FMT_RGB24, 0};
   CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n, cudaMemcpyHostToDevice, st));
   LaunchCtx lc{st, &s.launches};
-  launch_preprocess_f32(lc, s.d_desc, n, s.d_pre, c->hdr.input_h, c->hdr.input_w, c->hdr.pre_mul, c->hdr.pre_sub);
+  launch_preprocess_f32(lc, s.d_desc, n, c->d_pre, c->hdr.input_h, c->hdr.input_w, c->hdr.pre_mul, c->hdr.pre_sub);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, s.d_pre, sizeof(float) * (size_t)n * c->hdr.input_h * c->hdr.input_w * 3,
+  CK(cudaMemcpyAsync(out, c->d_pre, sizeof(float) * (size_t)n * c->hdr.input_h * c->hdr.input_w * 3,
                      cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return 0;
@@ -875,17 +901,25 @@ int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t*
 
 }  // extern "C"
 
-// the stage hooks' copy of layer `li`'s activation (n images, float32 NHWC; bf16 storage is widened) from slot s
-static int copy_layer_out(wb_ctx* c, Slot& s, int n, int li, float* layer_out, size_t layer_out_floats) {
-  const wb_layer& L = c->layers[li];
+// the backbone hooks' outputs from slot s (n images): the head buffers (enc and logits may be NULL) and, for
+// stop_layer >= 0 and a layer_out, that layer's activation (float32 NHWC; bf16 storage is widened)
+static int copy_backbone_out(wb_ctx* c, Slot& s, cudaStream_t st, int n, float* enc, float* logits, int stop_layer,
+                             float* layer_out, size_t layer_out_floats) {
+  if (enc) CK(cudaMemcpyAsync(enc, s.d_enc, sizeof(float) * (size_t)n * c->hdr.num_anchors * 4, cudaMemcpyDeviceToHost, st));
+  if (logits)
+    CK(cudaMemcpyAsync(logits, s.d_logits, sizeof(float) * (size_t)n * c->hdr.num_anchors * (c->hdr.num_classes + 1),
+                       cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (stop_layer < 0 || !layer_out) return 0;
+  const wb_layer& L = c->layers[stop_layer];
   REQUIRE(L.op != WB_OP_HEAD, "head layers have no activation output");
   size_t elems = (size_t)n * L.out_h * L.out_w * L.out_c;
   REQUIRE(layer_out_floats >= elems, "layer_out too small");
   if (c->elem_size() == 4) {
-    CK(cudaMemcpy(layer_out, static_cast<float*>(s.arena) + (size_t)L.out_off * n, elems * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(layer_out, static_cast<float*>(s.arena.h) + (size_t)L.out_off * n, elems * 4, cudaMemcpyDeviceToHost));
   } else {
     std::vector<uint16_t> tmp(elems);
-    CK(cudaMemcpy(tmp.data(), static_cast<uint16_t*>(s.arena) + (size_t)L.out_off * n, elems * 2, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(tmp.data(), static_cast<uint16_t*>(s.arena.h) + (size_t)L.out_off * n, elems * 2, cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < elems; ++i) {
       uint32_t u = (uint32_t)tmp[i] << 16;
       memcpy(&layer_out[i], &u, 4);
@@ -899,28 +933,18 @@ extern "C" {
 int wb_backbone(wb_ctx* c, int n, const float* pre, float* enc, float* logits, int stop_layer, float* layer_out,
                 size_t layer_out_floats) {
   REQUIRE(c && pre, "NULL argument");
-  REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range");
   REQUIRE(stop_layer < (int)c->layers.size(), "stop_layer out of range");
-  std::lock_guard<std::mutex> lock(c->mu);
-  CK(cudaSetDevice(c->device));
-  Slot& s = c->slots[0];
-  REQUIRE(!s.busy, "slot 0 is busy");
-  cudaStream_t st = c->stream_of(0);
+  StageHook h(c, n);
+  if (h.rc) return h.rc;
+  Slot& s = h.s;
+  cudaStream_t st = h.st;
   const size_t pre_floats = (size_t)n * c->hdr.input_h * c->hdr.input_w * 3;
-  CK(cudaMemcpyAsync(s.d_pre, pre, sizeof(float) * pre_floats, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(c->d_pre, pre, sizeof(float) * pre_floats, cudaMemcpyHostToDevice, st));
   CK(cudaMemsetAsync(s.d_enc, 0, sizeof(float) * (size_t)n * c->hdr.num_anchors * 4, st));
   CK(cudaMemsetAsync(s.d_logits, 0, sizeof(float) * (size_t)n * c->hdr.num_anchors * (c->hdr.num_classes + 1), st));
   s.launches = 0;
-  int rc = c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, n, s.d_pre, 0, stop_layer)
-                             : run_layers<float>(c, s, st, n, s.d_pre, 0, stop_layer);
-  if (rc) return rc;
-  if (enc) CK(cudaMemcpyAsync(enc, s.d_enc, sizeof(float) * (size_t)n * c->hdr.num_anchors * 4, cudaMemcpyDeviceToHost, st));
-  if (logits)
-    CK(cudaMemcpyAsync(logits, s.d_logits, sizeof(float) * (size_t)n * c->hdr.num_anchors * (c->hdr.num_classes + 1),
-                       cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (stop_layer >= 0 && layer_out)
-    if (int rc = copy_layer_out(c, s, n, stop_layer, layer_out, layer_out_floats)) return rc;
+  if (int rc = run_program(c, s, st, n, c->d_pre, 0, stop_layer)) return rc;
+  if (int rc = copy_backbone_out(c, s, st, n, enc, logits, stop_layer, layer_out, layer_out_floats)) return rc;
   c->last_launches = s.launches;
   return 0;
 }
@@ -929,35 +953,25 @@ int wb_backbone_frames(wb_ctx* c, int n, const uint8_t* const* frames, const int
                        float* enc, float* logits, int stop_layer, float* layer_out, size_t layer_out_floats,
                        int32_t* n_images) {
   REQUIRE(c && frames && cam_ids, "NULL argument");
-  REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range");
   REQUIRE(stop_layer >= -1 && stop_layer < (int)c->layers.size(), "stop_layer out of range");
   REQUIRE((flags & ~(WB_F_YUV420P | WB_F_NV12 | WB_F_FRAMES_ON_DEVICE | WB_F_FUSE_FILTERS)) == 0,
           "flags may only hold WB_F_YUV420P, WB_F_NV12, WB_F_FRAMES_ON_DEVICE and WB_F_FUSE_FILTERS");
-  std::lock_guard<std::mutex> lock(c->mu);
-  CK(cudaSetDevice(c->device));
-  Slot& s = c->slots[0];
-  REQUIRE(!s.busy, "slot 0 is busy");
-  cudaStream_t st = c->stream_of(0);
+  StageHook h(c, n);
+  if (h.rc) return h.rc;
+  Slot& s = h.s;
+  cudaStream_t st = h.st;
   int fmt = WB_FMT_RGB24;
   if (int rc = frame_format(flags, &fmt)) return rc;
   int ni = n;
   if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &ni)) return rc;
   if (stop_layer >= 0) {
     s.launches = 0;
-    int rc = c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, ni, nullptr, 0, stop_layer)
-                               : run_layers<float>(c, s, st, ni, nullptr, 0, stop_layer);
-    if (rc) return rc;
+    if (int rc = run_program(c, s, st, ni, nullptr, 0, stop_layer)) return rc;
   } else if (int rc = enqueue_kernels(c, s, st, ni, flags, n, s.windowed)) {
     return rc;
   }
   // the head buffers as the run left them: not cleared first, so a head row that no kernel wrote keeps stale values
-  if (enc) CK(cudaMemcpyAsync(enc, s.d_enc, sizeof(float) * (size_t)ni * c->hdr.num_anchors * 4, cudaMemcpyDeviceToHost, st));
-  if (logits)
-    CK(cudaMemcpyAsync(logits, s.d_logits, sizeof(float) * (size_t)ni * c->hdr.num_anchors * (c->hdr.num_classes + 1),
-                       cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (stop_layer >= 0 && layer_out)
-    if (int rc = copy_layer_out(c, s, ni, stop_layer, layer_out, layer_out_floats)) return rc;
+  if (int rc = copy_backbone_out(c, s, st, ni, enc, logits, stop_layer, layer_out, layer_out_floats)) return rc;
   if (n_images) *n_images = ni;
   c->last_launches = s.launches;
   return 0;
@@ -967,12 +981,10 @@ int wb_postprocess(wb_ctx* c, int n, const float* enc, const float* logits, cons
                    wb_detection* const* out, uint32_t* const* verdicts, float* boxes, float* scores, float* classes,
                    int32_t* num) {
   REQUIRE(c && enc && logits && cam_ids, "NULL argument");
-  REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range");
-  std::lock_guard<std::mutex> lock(c->mu);
-  CK(cudaSetDevice(c->device));
-  Slot& s = c->slots[0];
-  REQUIRE(!s.busy, "slot 0 is busy");
-  cudaStream_t st = c->stream_of(0);
+  StageHook h(c, n);
+  if (h.rc) return h.rc;
+  Slot& s = h.s;
+  cudaStream_t st = h.st;
   const int NA = c->hdr.num_anchors, C1 = c->hdr.num_classes + 1;
   CK(cudaMemcpyAsync(s.d_enc, enc, sizeof(float) * (size_t)n * NA * 4, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(s.d_logits, logits, sizeof(float) * (size_t)n * NA * C1, cudaMemcpyHostToDevice, st));
@@ -982,18 +994,18 @@ int wb_postprocess(wb_ctx* c, int n, const float* enc, const float* logits, cons
   const size_t B = c->max_batch;
   CK(cudaMemcpyAsync(s.h_out, s.d_out, sizeof(wb_detection) * (size_t)n * WB_MAX_DETECTIONS, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(s.h_verdicts, s.d_verdicts, sizeof(uint32_t) * (size_t)n * WB_MAX_DETECTIONS, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(s.h_raw, s.d_raw, sizeof(float) * B * WB_MAX_DETECTIONS * 6, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(s.h_raw_num, s.d_raw_num, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(c->h_raw, c->d_raw, sizeof(float) * B * WB_MAX_DETECTIONS * 6, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(c->h_raw_num, s.d_raw_num, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i) {
     if (out && out[i]) memcpy(out[i], s.h_out + (size_t)i * WB_MAX_DETECTIONS, sizeof(wb_detection) * WB_MAX_DETECTIONS);
     if (verdicts && verdicts[i])
       memcpy(verdicts[i], s.h_verdicts + (size_t)i * WB_MAX_DETECTIONS, sizeof(uint32_t) * WB_MAX_DETECTIONS);
   }
-  if (boxes) memcpy(boxes, s.h_raw, sizeof(float) * (size_t)n * WB_MAX_DETECTIONS * 4);
-  if (scores) memcpy(scores, s.h_raw + B * WB_MAX_DETECTIONS * 4, sizeof(float) * (size_t)n * WB_MAX_DETECTIONS);
-  if (classes) memcpy(classes, s.h_raw + B * WB_MAX_DETECTIONS * 5, sizeof(float) * (size_t)n * WB_MAX_DETECTIONS);
-  if (num) memcpy(num, s.h_raw_num, sizeof(int) * n);
+  if (boxes) memcpy(boxes, c->h_raw, sizeof(float) * (size_t)n * WB_MAX_DETECTIONS * 4);
+  if (scores) memcpy(scores, c->h_raw + B * WB_MAX_DETECTIONS * 4, sizeof(float) * (size_t)n * WB_MAX_DETECTIONS);
+  if (classes) memcpy(classes, c->h_raw + B * WB_MAX_DETECTIONS * 5, sizeof(float) * (size_t)n * WB_MAX_DETECTIONS);
+  if (num) memcpy(num, c->h_raw_num, sizeof(int) * n);
   c->last_launches = s.launches;
   return 0;
 }
@@ -1028,17 +1040,15 @@ int wb_last_launch_count(wb_ctx* c, int* launches) {
 int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, const int32_t* cam_ids,
                       float* ms, int32_t* kinds, int max_launches, int* n_out) {
   REQUIRE(c && device_frames && cam_ids && ms && kinds && n_out, "NULL argument");
-  REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range");
-  std::lock_guard<std::mutex> lock(c->mu);
-  CK(cudaSetDevice(c->device));
-  Slot& s = c->slots[0];
-  REQUIRE(!s.busy, "slot 0 is busy");
-  cudaStream_t st = c->stream_of(0);
+  StageHook h(c, n);
+  if (h.rc) return h.rc;
+  Slot& s = h.s;
+  cudaStream_t st = h.st;
   if (int rc = fill_desc(c, s, n, device_frames, cam_ids, true, WB_FMT_RGB24, st, false, nullptr)) return rc;
   const int nl = (int)c->layers.size();
   REQUIRE(max_launches >= nl + 1, "max_launches too small");
-  std::vector<cudaEvent_t> ev(nl + 2);
-  for (auto& e : ev) CK(cudaEventCreate(&e));
+  std::vector<Event> ev(nl + 2);  // entry i is timed from ev[i] to ev[i + 1]
+  for (auto& e : ev) CK(create(e));
   // every layer is launched REPS times back to back between two events (layers are idempotent: they
   // never write their own input), so host launch gaps do not leak into the per-kernel time
   const int REPS = 10;
@@ -1046,28 +1056,19 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
   if (int rc = run_all(c, s, st, n, 0, n, false)) return rc;  // warm-up, also fills every activation buffer
   s.launches = 0;
   CK(cudaEventRecord(ev[0], st));
-  for (int li = 0; li < nl; ++li) {
-    // a span the executor runs as one kernel is timed as a whole; its time is reported on the 1x1 (projection)
-    // entry and the span's other entries read 0
+  for (int li = 0; li < nl;) {
+    // time each span the executor runs as one kernel REPS times, and report its time on its 1x1 (projection) entry,
+    // or on its only layer; the span's other entries read 0
     const Span sp = fused_span(c, li, nl);
-    const int first = li, last = (int)sp.last;
+    const int last = (int)sp.last;
     const int timed = sp.kind == SPAN_DW_PW || sp.kind == SPAN_DW_PW_ADD ? li + 1 : li;
-    for (; li < timed; ++li) {
-      CK(cudaEventRecord(ev[li + 1], st));  // zero-length interval
-      kinds[li] = (int)c->layers[li].op;
+    for (int i = li; i <= last; ++i) {
+      for (int r = 0; i == timed && r < REPS; ++r)
+        if (int rc = run_program(c, s, st, n, nullptr, li, last)) return rc;
+      CK(cudaEventRecord(ev[i + 1], st));
+      kinds[i] = (int)c->layers[i].op;
     }
-    for (int r = 0; r < REPS; ++r) {
-      int rc = c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, n, nullptr, first, last)
-                                 : run_layers<float>(c, s, st, n, nullptr, first, last);
-      if (rc) return rc;
-    }
-    CK(cudaEventRecord(ev[li + 1], st));
-    kinds[li] = (int)c->layers[li].op;
-    while (li < last) {
-      ++li;
-      CK(cudaEventRecord(ev[li + 1], st));  // zero-length interval
-      kinds[li] = (int)c->layers[li].op;
-    }
+    li = last + 1;
   }
   for (int r = 0; r < REPS; ++r)
     if (int rc = run_post(c, s, st, n, 0)) return rc;
@@ -1079,7 +1080,6 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
   }
   s.launches /= REPS;
   kinds[nl] = 100;
-  for (auto& e : ev) cudaEventDestroy(e);
   *n_out = nl + 1;
   c->last_launches = s.launches;
   return 0;
@@ -1177,8 +1177,8 @@ int wb_comm_init(wb_ctx* c, int rank, int world, const uint8_t* id_bytes) {
   c->comm = comm;
   c->comm_rank = rank;
   c->comm_world = world;
-  CK(cudaStreamCreateWithFlags(&c->comm_stream, cudaStreamNonBlocking));
-  CK(cudaEventCreateWithFlags(&c->comm_ev, cudaEventDisableTiming));
+  CK(create(c->comm_stream));
+  CK(cudaEventCreateWithFlags(&c->comm_ev.h, cudaEventDisableTiming));
   return 0;
 }
 
@@ -1224,9 +1224,7 @@ int wb_comm_destroy(wb_ctx* c) {
   c->comm = nullptr;
   c->comm_rank = -1;
   c->comm_world = 0;
-  if (c->comm_ev) cudaEventDestroy(c->comm_ev);
-  if (c->comm_stream) cudaStreamDestroy(c->comm_stream);
-  c->comm_ev = nullptr;
-  c->comm_stream = nullptr;
+  c->comm_ev.reset();
+  c->comm_stream.reset();
   return 0;
 }
