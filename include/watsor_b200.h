@@ -75,7 +75,13 @@ int wb_device_count(int* count);
  * a compiled model blob (watsor_b200/model.py writes it from frozen_inference_graph.pb / cpu.pb).
  * precision: 0 = fp32 storage, dense convs on CUDA cores (FFMA); 1 = bf16 storage, bf16 wgmma (fast mode, not
  * a parity mode); 2 = fp32 storage, dense convs as 3xTF32 wgmma MMAs with fp32 accumulation (fp32-faithful: the
- * default of the Python host and what bench.py reports); 3 = single TF32 MMA (diagnostic). */
+ * default of the Python host and what bench.py reports); 3 = single TF32 MMA (diagnostic); 4 = fp16 storage, fp16
+ * wgmma (fast mode with 11 significant bits, the analogue of TensorRT's FP16 flag; not a parity mode).
+ * Precision 4's numerical policy: activations are stored as IEEE half, rounded to nearest even with subnormals kept,
+ * after a clamp to +-65504, so an activation that overflows saturates at +-65504 and never becomes inf.  Tensor-core
+ * weights are rounded to fp16 once, here; a model with a weight whose magnitude rounds beyond 65504 is refused, and
+ * wb_last_error names the layer.  Accumulation, folded BatchNorm, bias and the heads stay fp32; the stem, depthwise
+ * and CUDA-core GEMM weights stay fp32, as in precision 1. */
 int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_batch, int precision,
               wb_ctx** out);
 /* replaces __exit__ (tensorrt_gpu.py:59-63) */

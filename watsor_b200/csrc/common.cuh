@@ -1,6 +1,7 @@
 // common.cuh -- shared device-side types of libwatsor_b200 (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -58,7 +59,7 @@ struct PostParams {
   float class_offset;
 };
 
-// activation element type helpers (fp32 parity path / bf16 tensor-core path)
+// activation element type helpers (fp32 parity path / bf16 and fp16 tensor-core paths)
 template <typename T> struct ActIO;
 template <> struct ActIO<float> {
   static __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
@@ -83,6 +84,27 @@ template <> struct ActIO<__nv_bfloat16> {
   }
   static __device__ __forceinline__ float ld(const __nv_bfloat16* p) { return __bfloat162float(*p); }
   static __device__ __forceinline__ void st(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+};
+// fp16 storage (precision 4): round to nearest even, subnormals kept.  A value beyond the largest finite half is
+// clamped to +-65504 first, so an overflowing activation saturates instead of becoming +-inf and poisoning every layer
+// after it.  Only stores clamp: loads widen exactly.
+constexpr float FP16_MAX = 65504.0f;
+__device__ __forceinline__ float sat_fp16(float v) { return fminf(fmaxf(v, -FP16_MAX), FP16_MAX); }
+template <> struct ActIO<__half> {
+  static __device__ __forceinline__ float4 ld4(const __half* p) {
+    uint2 r = *reinterpret_cast<const uint2*>(p);
+    float2 fa = __half22float2(*reinterpret_cast<__half2*>(&r.x)), fb = __half22float2(*reinterpret_cast<__half2*>(&r.y));
+    return make_float4(fa.x, fa.y, fb.x, fb.y);
+  }
+  static __device__ __forceinline__ void st4(__half* p, float4 v) {
+    __half2 a = __floats2half2_rn(sat_fp16(v.x), sat_fp16(v.y)), b = __floats2half2_rn(sat_fp16(v.z), sat_fp16(v.w));
+    uint2 r;
+    r.x = *reinterpret_cast<uint32_t*>(&a);
+    r.y = *reinterpret_cast<uint32_t*>(&b);
+    *reinterpret_cast<uint2*>(p) = r;
+  }
+  static __device__ __forceinline__ float ld(const __half* p) { return __half2float(*p); }
+  static __device__ __forceinline__ void st(__half* p, float v) { *p = __float2half_rn(sat_fp16(v)); }
 };
 
 __device__ __forceinline__ float relu6f(float v) { return fminf(fmaxf(v, 0.0f), 6.0f); }

@@ -4,7 +4,7 @@
 // `BoxPredictor_i/{BoxEncodingPredictor,ClassPredictor}` (Conv2D + BiasAdd, Reshape, concat) of the
 // frozen graph run by watsor/detection/tensorflow_cpu.py:114.  All tensors are NHWC, TF `SAME`
 // padding (asymmetric).  The 1x1 / KxK dense convolutions are one tiled SGEMM with an optional
-// im2col row gather; the bf16 wgmma path lives in kernels_tc.cu.
+// im2col row gather; the wgmma path lives in kernels_tc.cu.
 #include <algorithm>
 
 #include "common.cuh"
@@ -87,6 +87,8 @@ template void launch_dw<float>(const LaunchCtx&, int, const wb_layer&, const flo
                                const float*, float*);
 template void launch_dw<__nv_bfloat16>(const LaunchCtx&, int, const wb_layer&, const __nv_bfloat16*, const float*,
                                        const float*, const float*, __nv_bfloat16*);
+template void launch_dw<__half>(const LaunchCtx&, int, const wb_layer&, const __half*, const float*, const float*,
+                                const float*, __half*);
 
 // residual add (MobileNet-v2 style bottlenecks)
 template <typename T>
@@ -104,6 +106,7 @@ void launch_add(const LaunchCtx& lc, size_t elems, const T* a, const T* b, T* ou
 }
 template void launch_add<float>(const LaunchCtx&, size_t, const float*, const float*, float*);
 template void launch_add<__nv_bfloat16>(const LaunchCtx&, size_t, const __nv_bfloat16*, const __nv_bfloat16*, __nv_bfloat16*);
+template void launch_add<__half>(const LaunchCtx&, size_t, const __half*, const __half*, __half*);
 
 // TF MaxPool / AvgPool with padding SAME (Inception modules): thread = (pixel, 4 channels).  The maximum ignores the
 // padding; the average is the fp32 sum of the in-image taps in (ky, kx) order divided by their count.
@@ -156,6 +159,7 @@ void launch_pool(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, T* 
 }
 template void launch_pool<float>(const LaunchCtx&, int, const wb_layer&, const float*, float*);
 template void launch_pool<__nv_bfloat16>(const LaunchCtx&, int, const wb_layer&, const __nv_bfloat16*, __nv_bfloat16*);
+template void launch_pool<__half>(const LaunchCtx&, int, const wb_layer&, const __half*, __half*);
 
 // ConcatV2 along channels, one input: [n*h*w][in_c] -> channels [row_off, row_off + in_c) of [n*h*w][out_c]
 template <typename T>
@@ -177,6 +181,7 @@ void launch_copy_channels(const LaunchCtx& lc, int n, const wb_layer& L, const T
 }
 template void launch_copy_channels<float>(const LaunchCtx&, int, const wb_layer&, const float*, float*);
 template void launch_copy_channels<__nv_bfloat16>(const LaunchCtx&, int, const wb_layer&, const __nv_bfloat16*, __nv_bfloat16*);
+template void launch_copy_channels<__half>(const LaunchCtx&, int, const wb_layer&, const __half*, __half*);
 
 // ---------------------------------------------------------------------------------------------------
 // SGEMM  C[M,N] = A[M,K] * W[K,N]  (+ per-column affine, ReLU6)
@@ -383,8 +388,7 @@ struct SplitKReduceArgs {
   const float* partial;  // [splits][M][ld] raw accumulators
   const float* scale;
   const float* offset;
-  void* out;  // fp32 or bf16 [M][N]
-  int out_is_bf16;
+  void* out;  // T [M][N]
   float* enc;
   float* logits;
   int M, N, ld, splits, act;
@@ -392,7 +396,8 @@ struct SplitKReduceArgs {
 };
 
 // sums the split-K partial tiles in split order and applies the layer epilogue (affine, ReLU6, store
-// or head scatter).  One thread per 4 output columns.
+// or head scatter) with the activation type T.  One thread per 4 output columns.
+template <typename T>
 __global__ void __launch_bounds__(256) k_splitk_reduce(SplitKReduceArgs r) {
   const int n4 = r.ld >> 2;
   size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -425,16 +430,15 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(SplitKReduceArgs r) {
       else
         r.logits[row * r.ncp1 + (nn - r.n_box)] = v[j];
     }
-  } else if (r.out_is_bf16) {
-    ActIO<__nv_bfloat16>::st4(reinterpret_cast<__nv_bfloat16*>(r.out) + (size_t)m * r.N + n, make_float4(v[0], v[1], v[2], v[3]));
   } else {
-    *reinterpret_cast<float4*>(reinterpret_cast<float*>(r.out) + (size_t)m * r.N + n) = make_float4(v[0], v[1], v[2], v[3]);
+    ActIO<T>::st4(reinterpret_cast<T*>(r.out) + (size_t)m * r.N + n, make_float4(v[0], v[1], v[2], v[3]));
   }
 }
 
+template <typename T>
 void launch_splitk_reduce(const LaunchCtx& lc, const SplitKReduceArgs& r) {
   size_t total = (size_t)r.M * (r.ld >> 2);
-  k_splitk_reduce<<<(unsigned)((total + 255) / 256), 256, 0, lc.stream>>>(r);
+  k_splitk_reduce<T><<<(unsigned)((total + 255) / 256), 256, 0, lc.stream>>>(r);
   ++*lc.launch_counter;
 }
 
@@ -513,7 +517,6 @@ void launch_gemm_cc(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, 
     r.scale = scale;
     r.offset = offset;
     r.out = out;
-    r.out_is_bf16 = sizeof(T) == 2;
     r.enc = enc;
     r.logits = logits;
     r.M = g.M;
@@ -528,7 +531,7 @@ void launch_gemm_cc(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, 
     r.num_anchors = g.num_anchors;
     r.ncp1 = g.ncp1;
     r.hw = g.out_h * g.out_w;
-    launch_splitk_reduce(lc, r);
+    launch_splitk_reduce<T>(lc, r);
   }
 }
 
@@ -537,3 +540,5 @@ template void launch_gemm_cc<float>(const LaunchCtx&, int, const wb_layer&, cons
 template void launch_gemm_cc<__nv_bfloat16>(const LaunchCtx&, int, const wb_layer&, const __nv_bfloat16*, const float*,
                                             const float*, const float*, __nv_bfloat16*, float*, float*, int, int, float*,
                                             size_t);
+template void launch_gemm_cc<__half>(const LaunchCtx&, int, const wb_layer&, const __half*, const float*, const float*,
+                                     const float*, __half*, float*, float*, int, int, float*, size_t);

@@ -354,14 +354,14 @@ int fused_launch_dwpw(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_ind
     unsigned long long st[3] = {(unsigned long long)dw.in_c * 4, (unsigned long long)dw.in_w * dw.in_c * 4,
                                 (unsigned long long)dw.in_h * dw.in_w * dw.in_c * 4};
     unsigned box[4] = {32, (unsigned)p.tw_in, (unsigned)p.th_in, 1};
-    if (!tc_encode_map(&map_in, in, 4, 4, dims, st, box, false, err)) return 1;
+    if (!tc_encode_map(&map_in, in, TC_TF32X3, 4, dims, st, box, false, err)) return 1;
   }
   {
     unsigned long long dims[2] = {(unsigned long long)w.k, (unsigned long long)w.n_pad};
     unsigned long long st[1] = {(unsigned long long)w.k * 4};
     unsigned box[2] = {32, (unsigned)p.block_n};
-    if (!tc_encode_map(&map_b, w.w, 4, 2, dims, st, box, true, err)) return 1;
-    if (!tc_encode_map(&map_b_lo, w.w_lo, 4, 2, dims, st, box, true, err)) return 1;
+    if (!tc_encode_map(&map_b, w.w, TC_TF32X3, 2, dims, st, box, true, err)) return 1;
+    if (!tc_encode_map(&map_b_lo, w.w_lo, TC_TF32X3, 2, dims, st, box, true, err)) return 1;
   }
   static PerDeviceFlag attr_done[4];
   static int ctas = 0;

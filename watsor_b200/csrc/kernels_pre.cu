@@ -370,3 +370,5 @@ template void launch_stem<float>(const LaunchCtx&, const FrameDesc*, const float
 template void launch_stem<__nv_bfloat16>(const LaunchCtx&, const FrameDesc*, const float*, int,
                                          const wb_layer&, int, int, float, float, const float*, const float*,
                                          const float*, __nv_bfloat16*);
+template void launch_stem<__half>(const LaunchCtx&, const FrameDesc*, const float*, int, const wb_layer&, int, int,
+                                  float, float, const float*, const float*, const float*, __half*);

@@ -2,8 +2,9 @@
 // TMA (cp.async.bulk.tensor) -> 128B-swizzled shared memory -> wgmma with the fp32 accumulators in registers ->
 // staging tile -> epilogue (folded BatchNorm / bias, ReLU6) -> global.  sm_90a.
 //
-// Three operand modes share one warp-specialised kernel:
+// Four operand modes share one warp-specialised kernel:
 //   TC_BF16    A, W in bf16, bf16 activations out                        -- "fast" mode
+//   TC_FP16    A, W in fp16, fp16 activations out (saturated at +-65504) -- "fast" mode, 3 more significant bits
 //   TC_TF32X1  A, W in fp32, one TF32 MMA per product                     -- diagnostic
 //   TC_TF32X3  A, W in fp32, every product formed as three TF32 MMAs
 //              (A_hi*W_hi + A_lo*W_hi + A_hi*W_lo, fp32 accumulate)      -- fp32-faithful "parity" mode
@@ -16,6 +17,7 @@
 #include <cuda.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
@@ -28,7 +30,7 @@ namespace {
 struct TcArgs {
   const float* scale;
   const float* offset;
-  void* out;  // bf16 or fp32 [M][N]
+  void* out;  // [M][N] activations: fp32, bf16 or fp16 by mode
   float* enc;
   float* logits;
   int M, N, n_pad, K;  // K in elements
@@ -63,8 +65,8 @@ __device__ __forceinline__ float4 ld_dsmem128(uint32_t addr, uint32_t rank) {
 // One output row of the tile from the staging tile(s) to global memory, lanes along the columns (coalesced).
 // The row's raw accumulators are this CTA's own (members == 1) or, in a split-K cluster, the sum of the members'
 // partial rows in rank order; then folded BN / bias, ReLU6, the optional bottleneck shortcut, and the store: dense
-// [M][N], or the head scatter into the concatenated box-encoding / class-logit tensors.
-template <bool TF32>
+// [M][N] of OutT (float in the TF32 modes), or the head scatter into the concatenated box-encoding / class-logit tensors.
+template <typename OutT>
 __device__ __forceinline__ void copy_out_row(const TcArgs& g, const uint8_t* smem, int pitch, int r, int m0, int n0,
                                              int lane, int members) {
   const int mm = m0 + r;
@@ -103,14 +105,14 @@ __device__ __forceinline__ void copy_out_row(const TcArgs& g, const uint8_t* sme
         else
           g.logits[hr * g.ncp1 + (c - g.n_box)] = ys[e];
       }
-    } else if (TF32) {
+    } else if (std::is_same<OutT, float>::value) {
       if (g.residual != nullptr) {
         const float4 rr = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(g.residual) + (size_t)mm * g.N + nn);
         y = make_float4(__fadd_rn(y.x, rr.x), __fadd_rn(y.y, rr.y), __fadd_rn(y.z, rr.z), __fadd_rn(y.w, rr.w));
       }
       *reinterpret_cast<float4*>(reinterpret_cast<float*>(g.out) + (size_t)mm * g.N + nn) = y;
     } else {
-      ActIO<__nv_bfloat16>::st4(reinterpret_cast<__nv_bfloat16*>(g.out) + (size_t)mm * g.N + nn, y);
+      ActIO<OutT>::st4(reinterpret_cast<OutT*>(g.out) + (size_t)mm * g.N + nn, y);
     }
   }
 }
@@ -118,13 +120,16 @@ __device__ __forceinline__ void copy_out_row(const TcArgs& g, const uint8_t* sme
 constexpr int GEMM_THREADS = 288;
 constexpr int GEMM_PRODUCER_WARP = 8;
 
-// MODE 0: bf16 operands; MODE 1: tf32 single product (diagnostic); MODE 2: tf32 x3 split.  BN: N tile (32 / 64 / 128).
+// MODE 0: bf16 operands; MODE 1: tf32 single product (diagnostic); MODE 2: tf32 x3 split; MODE 3: fp16 operands.
+// BN: N tile (32 / 64 / 128).
 template <int MODE, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     k_gemm_tc(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
               const __grid_constant__ CUtensorMap map_b_lo, TcArgs g) {
-  constexpr bool TF32 = MODE != 0;
+  constexpr bool TF32 = MODE == 1 || MODE == 2;
   constexpr bool X3 = MODE == 2;
+  // activation type: the MMAs' operand type and the dense output's element type
+  using ActT = typename std::conditional<TF32, float, typename std::conditional<MODE == 3, __half, __nv_bfloat16>::type>::type;
   constexpr int ELEM = TF32 ? 4 : 2;
   constexpr int K_PER_BLOCK = ROW_BYTES / ELEM;
   constexpr int B_TILE_BYTES = BN * ROW_BYTES;
@@ -199,7 +204,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         wg_x3_kblock_sum<BN>(acc, part, a_hi, a_lo, b_hi, b_lo);
       } else {
         wgmma_fence();
-        wg_mma_kblock<TF32, false, BN>(acc, a_hi, a_lo, b_hi, b_lo, 1u);
+        wg_mma_kblock<ActT, false, BN>(acc, a_hi, a_lo, b_hi, b_lo, 1u);
         wgmma_commit();
         wgmma_wait_all();
       }
@@ -237,18 +242,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     cluster_sync_all();
     const int z = (int)cluster_ctarank();
     for (int r = z + g.splits * warp; r < rows; r += n_warps * g.splits)
-      copy_out_row<TF32>(g, smem, pitch, r, m0, n0, lane, g.splits);
+      copy_out_row<ActT>(g, smem, pitch, r, m0, n0, lane, g.splits);
     __syncwarp();
     cluster_sync_all();  // nobody exits while a peer still reads its staging tile
   } else if (g.is_head) {
-    for (int r = warp; r < rows; r += n_warps) copy_out_row<TF32>(g, smem, pitch, r, m0, n0, lane, 1);
+    for (int r = warp; r < rows; r += n_warps) copy_out_row<ActT>(g, smem, pitch, r, m0, n0, lane, 1);
   } else {
     // dense [M][N] output: the thread count is a multiple of the row's BN / 4 float4 columns, so a thread keeps its 4
     // columns and walks down the rows -- folded BN / bias in registers, pointers advanced by a constant, ~20
     // instructions per float4 (this phase is issue bound: 2.5 warps per scheduler)
     static_assert(GEMM_THREADS % (BN / 4) == 0, "every thread of the dense epilogue keeps its 4 columns");
     constexpr int C4N = BN / 4, ROW_STEP = GEMM_THREADS / C4N;
-    using OutT = typename std::conditional<TF32, float, __nv_bfloat16>::type;
     const int r_it = (int)threadIdx.x / C4N, c_it = (int)threadIdx.x % C4N;
     const int nn = n0 + c_it * 4;
     if (nn < g.N && r_it < rows) {
@@ -256,7 +260,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       const bool relu = g.act == WB_ACT_RELU6;
       uint32_t sp = smem_u32(smem) + (uint32_t)((r_it * pitch + c_it * 4) * 4);
       constexpr uint32_t sstep = (uint32_t)(ROW_STEP * pitch * 4);
-      OutT* op = reinterpret_cast<OutT*>(g.out) + (size_t)(m0 + r_it) * g.N + nn;
+      ActT* op = reinterpret_cast<ActT*>(g.out) + (size_t)(m0 + r_it) * g.N + nn;
       // the bottleneck shortcut is fused in the fp32 modes only
       const float* rp = TF32 && g.residual != nullptr ? reinterpret_cast<const float*>(g.residual) + (size_t)(m0 + r_it) * g.N + nn : nullptr;
       const size_t gstep = (size_t)ROW_STEP * g.N;
@@ -274,7 +278,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                                  affine_rn(y[u].w, sc.w, of.w));
           if (relu) v = make_float4(relu6f(v.x), relu6f(v.y), relu6f(v.z), relu6f(v.w));
           if (rp != nullptr) v = make_float4(__fadd_rn(v.x, rs[u].x), __fadd_rn(v.y, rs[u].y), __fadd_rn(v.z, rs[u].z), __fadd_rn(v.w, rs[u].w));
-          ActIO<OutT>::st4(op + u * gstep, v);
+          ActIO<ActT>::st4(op + u * gstep, v);
         }
         sp += 4 * sstep;
         op += 4 * gstep;
@@ -289,7 +293,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           v = make_float4(__fadd_rn(v.x, r4.x), __fadd_rn(v.y, r4.y), __fadd_rn(v.z, r4.z), __fadd_rn(v.w, r4.w));
           rp += gstep;
         }
-        ActIO<OutT>::st4(op, v);
+        ActIO<ActT>::st4(op, v);
         sp += sstep;
         op += gstep;
       }
@@ -315,18 +319,24 @@ EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// 2-D K-major matrix [rows][k] -> tensor map with a (128 B x box_rows) box, 128B swizzle
-bool make_map(CUtensorMap* map, const void* base, int elem_bytes, int rows, int k, int box_rows, std::string* err) {
+CUtensorMapDataType map_dtype(int mode) {
+  return mode == TC_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                         : (mode == TC_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
+}
+
+// 2-D K-major matrix [rows][k] of operand mode `mode` -> tensor map with a (128 B x box_rows) box, 128B swizzle
+bool make_map(CUtensorMap* map, const void* base, int mode, int rows, int k, int box_rows, std::string* err) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) {
     *err = "cuTensorMapEncodeTiled is not available from the driver";
     return false;
   }
+  const int elem_bytes = tc_elem_bytes(mode);
   cuuint64_t dims[2] = {(cuuint64_t)k, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)k * elem_bytes};
   cuuint32_t box[2] = {(cuuint32_t)(ROW_BYTES / elem_bytes), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+  CUresult r = fn(map, map_dtype(mode), 2,
                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -339,7 +349,7 @@ bool make_map(CUtensorMap* map, const void* base, int elem_bytes, int rows, int 
 
 }  // namespace
 
-bool tc_encode_map(void* map, const void* base, int elem_bytes, int rank, const unsigned long long* dims,
+bool tc_encode_map(void* map, const void* base, int mode, int rank, const unsigned long long* dims,
                    const unsigned long long* strides_bytes, const unsigned* box, bool swizzle128, std::string* err,
                    const unsigned* elem_strides) {
   EncodeTiledFn fn = encode_fn();
@@ -355,8 +365,7 @@ bool tc_encode_map(void* map, const void* base, int elem_bytes, int rank, const 
     es[i] = elem_strides ? elem_strides[i] : 1;
     if (i + 1 < rank) st[i] = strides_bytes[i];
   }
-  CUresult r = fn(reinterpret_cast<CUtensorMap*>(map),
-                  elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank,
+  CUresult r = fn(reinterpret_cast<CUtensorMap*>(map), map_dtype(mode), (cuuint32_t)rank,
                   const_cast<void*>(base), d, st, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -388,11 +397,11 @@ int pick_block_n(int n_pad) { return n_pad <= 32 ? 32 : (n_pad <= 64 ? 64 : 128)
 
 bool tc_layer_supported(const wb_layer& L, int mode, bool conv) {
   // 1x1: the activation and weight rows are K-major tensor maps, whose row stride must be a multiple of 16 bytes
-  // (K % 4 in fp32, K % 8 in bf16)
-  const int elem = mode == TC_BF16 ? 2 : 4;
+  // (K % 4 in fp32, K % 8 in bf16 / fp16)
+  const int elem = tc_elem_bytes(mode);
   if ((L.op == WB_OP_PW || L.op == WB_OP_HEAD) && L.kh == 1 && L.kw == 1 && L.stride == 1 && (L.in_c * elem) % 16 == 0)
     return true;
-  // KxK / strided dense convolutions (the SSD extra layers): implicit GEMM, one filter tap x 32 (64 bf16) channels
+  // KxK / strided dense convolutions (the SSD extra layers): implicit GEMM, one filter tap x 32 (64 bf16 / fp16) channels
   // per k-block; a CTA's tile is a whole number of output images, so the maps must be small (<= 128 pixels)
   return L.op == WB_OP_CONV && L.in_c % 64 == 0 && L.out_h * L.out_w <= (uint32_t)BLOCK_M && L.stride <= 8 && conv;
 }
@@ -410,7 +419,7 @@ int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb
     w.k = K;
     w.n_pad = NP;
     w.block_n = pick_block_n(NP);
-    const int elem = mode == TC_BF16 ? 2 : 4;
+    const int elem = tc_elem_bytes(mode);
     const size_t bytes = (size_t)NP * K * elem;
     std::vector<uint8_t> hi(bytes), lo(mode == TC_TF32X3 ? bytes : 0);
     for (int n = 0; n < NP; ++n)
@@ -419,6 +428,15 @@ int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb
         if (mode == TC_BF16) {
           __nv_bfloat16 b = __float2bfloat16_rn(v);
           memcpy(&hi[((size_t)n * K + k) * 2], &b, 2);
+        } else if (mode == TC_FP16) {
+          // round to nearest even, subnormals kept; a weight that rounds beyond 65504 would become inf
+          __half h = __float2half_rn(v);
+          if (std::isinf(__half2float(h))) {
+            *err = std::string("layer ") + L.name + ": weight " + std::to_string(v) +
+                   " is outside the fp16 range (|w| <= 65504); run this model in bf16 or an fp32 mode";
+            return 1;
+          }
+          memcpy(&hi[((size_t)n * K + k) * 2], &h, 2);
         } else {
           uint32_t u;
           memcpy(&u, &v, 4);
@@ -439,14 +457,14 @@ int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb
       *err = "cudaMalloc/cudaMemcpy of tensor-core weights failed";
       return 1;
     }
-    if (!make_map(reinterpret_cast<CUtensorMap*>(w.tmap_b), w.w, elem, NP, K, w.block_n, err)) return 1;
+    if (!make_map(reinterpret_cast<CUtensorMap*>(w.tmap_b), w.w, mode, NP, K, w.block_n, err)) return 1;
     if (mode == TC_TF32X3) {
       if (cudaMalloc(&w.w_lo, bytes) != cudaSuccess ||
           cudaMemcpy(w.w_lo, lo.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
         *err = "cudaMalloc/cudaMemcpy of tensor-core weights failed";
         return 1;
       }
-      if (!make_map(reinterpret_cast<CUtensorMap*>(w.tmap_b_lo), w.w_lo, elem, NP, K, w.block_n, err)) return 1;
+      if (!make_map(reinterpret_cast<CUtensorMap*>(w.tmap_b_lo), w.w_lo, mode, NP, K, w.block_n, err)) return 1;
     } else {
       memcpy(w.tmap_b_lo, w.tmap_b, sizeof(w.tmap_b));
     }
@@ -472,7 +490,7 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
     return 1;
   }
   const int mode = tw.mode;
-  const int elem = mode == TC_BF16 ? 2 : 4;
+  const int elem = tc_elem_bytes(mode);
   TcArgs g;
   g.scale = scale;
   g.offset = offset;
@@ -484,15 +502,15 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
   g.n_pad = L.n_pad;
   g.K = L.kh * L.kw * L.in_c;
   g.block_n = w.block_n;
-  g.residual = mode == TC_BF16 ? nullptr : residual;
+  g.residual = elem == 2 ? nullptr : residual;
   g.conv = L.op == WB_OP_CONV;
   g.cpb = (L.in_c * elem) / ROW_BYTES;
   g.conv_kw = L.kw;
   g.conv_pad_t = L.pad_t;
   g.conv_pad_l = L.pad_l;
   g.rows_per_tile = g.conv ? (BLOCK_M / (int)(L.out_h * L.out_w)) * (int)(L.out_h * L.out_w) : BLOCK_M;
-  if (mode == TC_BF16 && residual != nullptr) {
-    *err = "residual fusion is not available in bf16 mode";
+  if (elem == 2 && residual != nullptr) {
+    *err = "residual fusion is not available in the 16-bit modes";
     return 1;
   }
   g.k_blocks = (g.K * elem + ROW_BYTES - 1) / ROW_BYTES;
@@ -540,8 +558,8 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
     unsigned box[4] = {(unsigned)(ROW_BYTES / elem), (unsigned)((L.out_w - 1) * L.stride + 1),
                        (unsigned)((L.out_h - 1) * L.stride + 1), (unsigned)imgs};
     unsigned es[4] = {1, L.stride, L.stride, 1};
-    if (!tc_encode_map(&map_a, in, elem, 4, dims, st, box, true, err, es)) return 1;
-  } else if (!make_map(&map_a, in, elem, g.M, g.K, BLOCK_M, err)) {
+    if (!tc_encode_map(&map_a, in, mode, 4, dims, st, box, true, err, es)) return 1;
+  } else if (!make_map(&map_a, in, mode, g.M, g.K, BLOCK_M, err)) {
     return 1;
   }
   CUtensorMap map_b, map_b_lo;
@@ -568,12 +586,15 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
     cfg.numAttrs = g.splits > 1 ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, map_a, map_b, map_b_lo, g);
   };
-  static PerDeviceFlag attr_done[3][3];
+  static PerDeviceFlag attr_done[4][3];
   const int bi = g.block_n == 32 ? 0 : (g.block_n == 64 ? 1 : 2);
   cudaError_t e;
   if (mode == TC_BF16) {
     e = bi == 0 ? launch(k_gemm_tc<0, 32>, attr_done[0][0])
                 : (bi == 1 ? launch(k_gemm_tc<0, 64>, attr_done[0][1]) : launch(k_gemm_tc<0, 128>, attr_done[0][2]));
+  } else if (mode == TC_FP16) {
+    e = bi == 0 ? launch(k_gemm_tc<3, 32>, attr_done[3][0])
+                : (bi == 1 ? launch(k_gemm_tc<3, 64>, attr_done[3][1]) : launch(k_gemm_tc<3, 128>, attr_done[3][2]));
   } else if (mode == TC_TF32X1) {
     e = bi == 0 ? launch(k_gemm_tc<1, 32>, attr_done[1][0])
                 : (bi == 1 ? launch(k_gemm_tc<1, 64>, attr_done[1][1]) : launch(k_gemm_tc<1, 128>, attr_done[1][2]));

@@ -5,10 +5,12 @@
 
 #include "common.cuh"
 
-enum TcMode { TC_BF16 = 0, TC_TF32X1 = 1, TC_TF32X3 = 2 };
+enum TcMode { TC_BF16 = 0, TC_TF32X1 = 1, TC_TF32X3 = 2, TC_FP16 = 3 };
+// bytes per operand element: 2 in the 16-bit modes, 4 (fp32 read as TF32) otherwise
+inline int tc_elem_bytes(int mode) { return mode == TC_BF16 || mode == TC_FP16 ? 2 : 4; }
 
 struct TcLayerWeights {
-  void* w = nullptr;     // [n_pad][K] K-major (bf16, or fp32 "hi" part), device
+  void* w = nullptr;     // [n_pad][K] K-major (bf16, fp16, or fp32 "hi" part), device
   void* w_lo = nullptr;  // fp32 "lo" part (TF32X3)
   int n_pad = 0, k = 0, block_n = 0;
   bool ready = false;
@@ -31,8 +33,9 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
                    const float* scale, const float* offset, void* out, float* enc, float* logits, int num_anchors,
                    int num_classes_p1, const void* residual, bool split_k, std::string* err);
 
-// generic tiled tensor-map encoder (rank <= 5); `map` points to 128 bytes aligned to 64
-bool tc_encode_map(void* map, const void* base, int elem_bytes, int rank, const unsigned long long* dims,
+// generic tiled tensor-map encoder (rank <= 5) of elements of operand mode `mode` (TcMode); `map` points to 128 bytes
+// aligned to 64
+bool tc_encode_map(void* map, const void* base, int mode, int rank, const unsigned long long* dims,
                    const unsigned long long* strides_bytes, const unsigned* box, bool swizzle128, std::string* err,
                    const unsigned* elem_strides = nullptr);
 

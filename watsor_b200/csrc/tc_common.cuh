@@ -95,11 +95,11 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
 // D[64 x N] (+)= A[64 x K] * B[N x K]^T, both operands K-major in shared memory, fp32 accumulators in registers.
-// TF32: k = 8 per instruction; BF16: k = 16.  Either way one instruction covers 32 bytes of a 128-byte row.
+// Op: the operand type, float (read as TF32: k = 8 per instruction), __nv_bfloat16 or __half (k = 16).  Either way one instruction covers 32 bytes of a 128-byte row.
 // Accumulator i of a thread holds row 16 * (warp % 4) + lane / 4 + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (lane % 4) + i % 2.
 // scale_d = 0 overwrites D instead of adding to it.
-template <bool TF32, int N> struct Wgmma;
-template <> struct Wgmma<true, 32> {
+template <typename Op, int N> struct Wgmma;
+template <> struct Wgmma<float, 32> {
   static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
@@ -108,7 +108,7 @@ template <> struct Wgmma<true, 32> {
         : "l"(da), "l"(db), "r"(scale_d));
   }
 };
-template <> struct Wgmma<true, 64> {
+template <> struct Wgmma<float, 64> {
   static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
@@ -117,7 +117,7 @@ template <> struct Wgmma<true, 64> {
         : "l"(da), "l"(db), "r"(scale_d));
   }
 };
-template <> struct Wgmma<true, 128> {
+template <> struct Wgmma<float, 128> {
   static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
@@ -126,54 +126,59 @@ template <> struct Wgmma<true, 128> {
         : "l"(da), "l"(db), "r"(scale_d));
   }
 };
-template <> struct Wgmma<false, 32> {
-  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(da), "l"(db), "r"(scale_d));
-  }
-};
-template <> struct Wgmma<false, 64> {
-  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(da), "l"(db), "r"(scale_d));
-  }
-};
-template <> struct Wgmma<false, 128> {
-  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(da), "l"(db), "r"(scale_d));
-  }
-};
+// The bf16 and f16 forms differ only in the operand type's PTX name.
+#define WB_WGMMA_16BIT(OP, PTX_T) \
+  template <> struct Wgmma<OP, 32> { \
+    static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) { \
+      asm volatile( \
+          "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n" \
+          "wgmma.mma_async.sync.aligned.m64n32k16.f32." PTX_T "." PTX_T " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n" \
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+          : "l"(da), "l"(db), "r"(scale_d)); \
+    } \
+  }; \
+  template <> struct Wgmma<OP, 64> { \
+    static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) { \
+      asm volatile( \
+          "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n" \
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32." PTX_T "." PTX_T " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n" \
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+          : "l"(da), "l"(db), "r"(scale_d)); \
+    } \
+  }; \
+  template <> struct Wgmma<OP, 128> { \
+    static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) { \
+      asm volatile( \
+          "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n" \
+          "wgmma.mma_async.sync.aligned.m64n128k16.f32." PTX_T "." PTX_T " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n" \
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+          : "l"(da), "l"(db), "r"(scale_d)); \
+    } \
+  };
+WB_WGMMA_16BIT(__nv_bfloat16, "bf16")
+WB_WGMMA_16BIT(__half, "f16")
+#undef WB_WGMMA_16BIT
 
-// One 128-byte k-block (32 fp32 / 64 bf16 along K) of a warpgroup's 64 x N tile: four k-steps.  X3 (3xTF32) issues
+// One 128-byte k-block (32 fp32 / 64 bf16 or fp16 along K) of a warpgroup's 64 x N tile: four k-steps.  X3 (3xTF32) issues
 // the small correction products lo(A)*hi(B) and hi(A)*lo(B) of all four k-steps first and the hi(A)*hi(B) products
 // last: the tensor core's accumulation rounds toward zero, and this order leaves four such roundings at the magnitude
 // of the k-block's partial sum instead of twelve.  The GEMM and the fused depthwise kernel both issue their MMAs
 // through here, so equal inputs give bit-equal outputs.
-template <bool TF32, bool X3, int N>
+template <typename Op, bool X3, int N>
 __device__ __forceinline__ void wg_mma_kblock(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
                                               uint32_t scale_first) {
   if (X3) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const uint32_t koff = (uint32_t)(k * 32);
-      Wgmma<TF32, N>::mma(d, make_sw128_desc(a_lo + koff), make_sw128_desc(b_hi + koff), k == 0 ? scale_first : 1u);
-      Wgmma<TF32, N>::mma(d, make_sw128_desc(a_hi + koff), make_sw128_desc(b_lo + koff), 1u);
+      Wgmma<Op, N>::mma(d, make_sw128_desc(a_lo + koff), make_sw128_desc(b_hi + koff), k == 0 ? scale_first : 1u);
+      Wgmma<Op, N>::mma(d, make_sw128_desc(a_hi + koff), make_sw128_desc(b_lo + koff), 1u);
     }
   }
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const uint32_t koff = (uint32_t)(k * 32);
-    Wgmma<TF32, N>::mma(d, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), (X3 || k > 0) ? 1u : scale_first);
+    Wgmma<Op, N>::mma(d, make_sw128_desc(a_hi + koff), make_sw128_desc(b_hi + koff), (X3 || k > 0) ? 1u : scale_first);
   }
 }
 
@@ -183,7 +188,7 @@ template <int N>
 __device__ __forceinline__ void wg_x3_kblock_sum(float* acc, float* part, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
                                                  uint32_t b_lo) {
   wgmma_fence();
-  wg_mma_kblock<true, true, N>(part, a_hi, a_lo, b_hi, b_lo, 0u);
+  wg_mma_kblock<float, true, N>(part, a_hi, a_lo, b_hi, b_lo, 0u);
   wgmma_commit();
   wgmma_wait_all();
 #pragma unroll
@@ -208,7 +213,7 @@ __device__ __forceinline__ void split_tf32(uint32_t hi_addr, uint32_t lo_addr) {
 }
 
 constexpr int BLOCK_M = 128;
-constexpr int ROW_BYTES = 128;                     // one swizzle row = 64 bf16 or 32 fp32 along K
+constexpr int ROW_BYTES = 128;                     // one swizzle row = 64 bf16 / fp16 or 32 fp32 along K
 constexpr int A_TILE_BYTES = BLOCK_M * ROW_BYTES;  // 16 KB
 
 

@@ -124,7 +124,7 @@ struct wb_ctx {
   std::vector<wb_layer> layers;
   std::vector<wb_tensor_entry> tensors;
   DevBuf<float> d_weights;
-  TcWeights tc;  // bf16 copies of the GEMM weights (precision 1)
+  TcWeights tc;  // the GEMM weights in the tensor cores' operand format (precision != 0)
   PostParams pp;
   DevBuf<CameraCfg> d_cams;
   std::vector<CameraCfg> h_cams;
@@ -156,7 +156,9 @@ struct wb_ctx {
   PinnedBuf<int> h_raw_num;
 
   const float* tensor(int idx) const { return d_weights + tensors[idx].offset; }
-  size_t elem_size() const { return precision == 1 ? 2 : 4; }
+  // the 16-bit activation modes: 1 (bf16), 4 (fp16)
+  bool half_acts() const { return precision == 1 || precision == 4; }
+  size_t elem_size() const { return half_acts() ? 2 : 4; }
   cudaStream_t stream_of(int s) { return has_user_stream ? user_stream : slots[s].stream; }
   // whether layer L runs on the tensor-core GEMM
   bool tc_runs(const wb_layer& L) const { return precision != 0 && tc_layer_supported(L, tc.mode, sw.tc_conv); }
@@ -215,8 +217,9 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   REQUIRE(out != nullptr && model_blob != nullptr, "NULL argument");
   REQUIRE(blob_bytes >= sizeof(wb_model_header), "model blob too small");
   REQUIRE(max_batch >= 1 && max_batch <= 4096, "max_batch out of range");
-  REQUIRE(precision >= 0 && precision <= 3,
-          "precision must be 0 (fp32 CUDA cores), 1 (bf16 wgmma), 2 (fp32 via 3xTF32 wgmma) or 3 (1xTF32, diagnostic)");
+  REQUIRE(precision >= 0 && precision <= 4,
+          "precision must be 0 (fp32 CUDA cores), 1 (bf16 wgmma), 2 (fp32 via 3xTF32 wgmma), 3 (1xTF32, diagnostic) or "
+          "4 (fp16 wgmma)");
   CK(cudaSetDevice(device));
   struct CtxFree {
     void operator()(wb_ctx* p) const { wb_destroy(p); }
@@ -277,7 +280,7 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   CK(cudaMemcpy(c->d_weights, p, floats * sizeof(float), cudaMemcpyHostToDevice));
   if (precision != 0) {
     std::string err;
-    const int mode = precision == 1 ? TC_BF16 : (precision == 2 ? TC_TF32X3 : TC_TF32X1);
+    const int mode = precision == 1 ? TC_BF16 : (precision == 2 ? TC_TF32X3 : (precision == 4 ? TC_FP16 : TC_TF32X1));
     if (tc_prepare_weights(c->layers, c->tensors, reinterpret_cast<const float*>(p), mode, c->sw.tc_conv, &c->tc, &err))
       return fail("tensor-core weight preparation: " + err);
   }
@@ -328,7 +331,11 @@ int wb_destroy(wb_ctx* c) {
 int wb_device_name(wb_ctx* c, char* buf, size_t n) {
   REQUIRE(c && buf && n > 0, "NULL argument");
   snprintf(buf, n, "%s (cuda:%d, sm_%d%d, %s)", c->prop.name, c->device, c->prop.major, c->prop.minor,
-           c->precision == 1 ? "bf16 wgmma" : (c->precision == 2 ? "fp32 3xTF32 wgmma" : (c->precision == 3 ? "tf32 wgmma" : "fp32")));
+           c->precision == 1   ? "bf16 wgmma"
+           : c->precision == 2 ? "fp32 3xTF32 wgmma"
+           : c->precision == 3 ? "tf32 wgmma"
+           : c->precision == 4 ? "fp16 wgmma"
+                               : "fp32");
   return 0;
 }
 
@@ -489,7 +496,7 @@ static Span fused_span(const wb_ctx* c, size_t li, size_t end) {
   const wb_layer& L = Ls[li];
   // layer p + 1 is `Add(shortcut, output of p)` (fp32 modes: the shortcut can be added in an fp32 epilogue)
   auto residual_add_after = [&](size_t p) {
-    if (c->precision == 0 || c->precision == 1 || p + 1 >= end || !c->sw.fuse_add) return false;
+    if (c->precision == 0 || c->half_acts() || p + 1 >= end || !c->sw.fuse_add) return false;
     const wb_layer& P = Ls[p], &A = Ls[p + 1];
     return P.op == WB_OP_PW && P.act == WB_ACT_NONE && A.op == WB_OP_ADD &&
            (A.in_off == P.out_off || A.in2_off == P.out_off) && A.in_off != A.in2_off;
@@ -611,8 +618,9 @@ static int run_post(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, 
 
 // layers first..last (last < 0: to the end) in the engine's activation type
 static int run_program(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* pre, int first, int last) {
-  return c->precision == 1 ? run_layers<__nv_bfloat16>(c, s, st, n, pre, first, last)
-                           : run_layers<float>(c, s, st, n, pre, first, last);
+  if (c->precision == 1) return run_layers<__nv_bfloat16>(c, s, st, n, pre, first, last);
+  if (c->precision == 4) return run_layers<__half>(c, s, st, n, pre, first, last);
+  return run_layers<float>(c, s, st, n, pre, first, last);
 }
 
 static int run_all(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, int n_frames, bool windowed) {
@@ -902,7 +910,7 @@ int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t*
 }  // extern "C"
 
 // the backbone hooks' outputs from slot s (n images): the head buffers (enc and logits may be NULL) and, for
-// stop_layer >= 0 and a layer_out, that layer's activation (float32 NHWC; bf16 storage is widened)
+// stop_layer >= 0 and a layer_out, that layer's activation (float32 NHWC; bf16 / fp16 storage is widened exactly)
 static int copy_backbone_out(wb_ctx* c, Slot& s, cudaStream_t st, int n, float* enc, float* logits, int stop_layer,
                              float* layer_out, size_t layer_out_floats) {
   if (enc) CK(cudaMemcpyAsync(enc, s.d_enc, sizeof(float) * (size_t)n * c->hdr.num_anchors * 4, cudaMemcpyDeviceToHost, st));
@@ -920,9 +928,17 @@ static int copy_backbone_out(wb_ctx* c, Slot& s, cudaStream_t st, int n, float* 
   } else {
     std::vector<uint16_t> tmp(elems);
     CK(cudaMemcpy(tmp.data(), static_cast<uint16_t*>(s.arena.h) + (size_t)L.out_off * n, elems * 2, cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < elems; ++i) {
-      uint32_t u = (uint32_t)tmp[i] << 16;
-      memcpy(&layer_out[i], &u, 4);
+    if (c->precision == 4) {
+      for (size_t i = 0; i < elems; ++i) {
+        __half h;
+        memcpy(&h, &tmp[i], 2);
+        layer_out[i] = __half2float(h);
+      }
+    } else {
+      for (size_t i = 0; i < elems; ++i) {
+        uint32_t u = (uint32_t)tmp[i] << 16;
+        memcpy(&layer_out[i], &u, 4);
+      }
     }
   }
   return 0;

@@ -13,8 +13,9 @@ from ._lib import ClassFilter, check
 from .windows import check_windows
 from .stream.share import MAX_DETECTIONS, Detection
 
-# 0: fp32 CUDA-core convs; 1: bf16 wgmma; 2: fp32 storage, dense convs as 3xTF32 wgmma (fp32-faithful)
-PRECISION_FP32, PRECISION_BF16_TC, PRECISION_TF32X3 = 0, 1, 2
+# 0: fp32 CUDA-core convs; 1: bf16 wgmma; 2: fp32 storage, dense convs as 3xTF32 wgmma (fp32-faithful);
+# 4: fp16 wgmma, activations saturated at +-65504 (include/watsor_b200.h, wb_create)
+PRECISION_FP32, PRECISION_BF16_TC, PRECISION_TF32X3, PRECISION_FP16_TC = 0, 1, 2, 4
 
 # frame layouts the hot path reads, by ffmpeg's -pix_fmt names -> wb_detect / wb_submit flag
 PIXEL_FORMATS = {'rgb24': 0, 'yuv420p': _lib.WB_F_YUV420P, 'nv12': _lib.WB_F_NV12}
