@@ -156,9 +156,8 @@ void launch_gemm_cc(const LaunchCtx& lc, int n, const wb_layer& L, const T* in, 
                     int num_anchors, int num_classes_p1, float* partial, size_t partial_floats);
 void launch_post(const LaunchCtx& lc, int n, const PostParams& pp, const float* enc, const float* logits,
                  const float* anchors, const FrameDesc* frames, const CameraCfg* cams, uint32_t flags,
-                 float* dec_boxes, int* cand_count, unsigned long long* cand, int* sel_count,
-                 unsigned long long* sel, wb_detection* out, uint32_t* verdicts, float* raw_boxes,
-                 float* raw_scores, float* raw_classes, int* raw_num, int* kept_hist);
+                 int* sel_count, unsigned long long* sel_key, float4* sel_box, wb_detection* out, uint32_t* verdicts,
+                 float* raw_boxes, float* raw_scores, float* raw_classes, int* raw_num, int* kept_hist);
 void launch_window_merge(const LaunchCtx& lc, int n_frames, const PostParams& pp, const WindowFrame* win,
                          const wb_detection* rows, const int* raw_num, const CameraCfg* cams, uint32_t flags,
                          wb_detection* out, uint32_t* verdicts);

@@ -1,5 +1,5 @@
-// kernels_post.cu -- K7 (anchor decode + sigmoid), K8 (per-class NMS, global top-100),
-// K9 (integer conversion + confidence / area / mask-zone predicates -> Detection[100]).
+// kernels_post.cu -- K8 (per-class sigmoid scores, anchor decode and NMS), K9 (global top-100, integer conversion +
+// confidence / area / mask-zone predicates -> Detection[100]).
 //
 // Restates `Postprocessor/Decode/*`, `Postprocessor/convert_scores`, `Postprocessor/Slice`,
 // `Postprocessor/BatchMultiClassNonMaxSuppression/*` and the final `add` of the frozen graph
@@ -13,7 +13,7 @@
 
 #include "common.cuh"
 
-// ------------------------------------------------------------------------------------------- K7
+// `Postprocessor/Decode/*` for one anchor
 __device__ __forceinline__ float4 decode_box(float4 e, float4 a, const PostParams& pp) {
   // anchors are corner boxes [ymin,xmin,ymax,xmax]  (get_center_coordinates_and_sizes)
   float wa = __fsub_rn(a.w, a.y), ha = __fsub_rn(a.z, a.x);
@@ -29,62 +29,10 @@ __device__ __forceinline__ float4 decode_box(float4 e, float4 a, const PostParam
                      __fadd_rn(xcenter, hw));
 }
 
+// `Postprocessor/convert_scores`
 __device__ __forceinline__ float sigmoid_score(float logit, float logit_scale) {
   float z = __fdiv_rn(logit, logit_scale);
   return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-z)));
-}
-
-constexpr int DEC_TILE = 64;
-
-// grid (ceil(N/DEC_TILE), frames).  Decodes DEC_TILE boxes, then sweeps the [DEC_TILE][C+1] logit tile
-// with coalesced loads; every (anchor, class) with score > threshold becomes a candidate key
-// score_bits << 32 | ~anchor  (sorting keys descending gives "score descending, lower anchor index first",
-// the pop order of TF's NonMaxSuppressionV5).  Appends are aggregated per block: positions inside the
-// block come from shared-memory counters, one global atomicAdd per (block, class) reserves the range
-// (90 classes x 1917 anchors would otherwise be 172 k global atomics per frame on 90 addresses).
-__global__ void __launch_bounds__(256)
-    k_decode_scores(PostParams pp, const float* __restrict__ enc, const float* __restrict__ logits,
-                    const float* __restrict__ anchors, float4* __restrict__ dec, int* __restrict__ cand_count,
-                    unsigned long long* __restrict__ cand) {
-  extern __shared__ unsigned char s_dec_raw[];
-  const int f = blockIdx.y, a0 = blockIdx.x * DEC_TILE;
-  const int N = pp.num_anchors, C = pp.num_classes, C1 = C + 1;
-  const int na = min(DEC_TILE, N - a0);
-  const int total = na * C1;
-  float* s_score = reinterpret_cast<float*>(s_dec_raw);                         // [DEC_TILE*C1]
-  int* s_cnt = reinterpret_cast<int*>(s_score + DEC_TILE * C1);                 // [C] then base [C]
-  int* s_base = s_cnt + C;
-  short* s_pos = reinterpret_cast<short*>(s_base + C);                          // [DEC_TILE*C1]
-  for (int c = threadIdx.x; c < C; c += blockDim.x) s_cnt[c] = 0;
-  if ((int)threadIdx.x < na) {
-    int i = a0 + threadIdx.x;
-    float4 e = reinterpret_cast<const float4*>(enc)[(size_t)f * N + i];
-    float4 a = reinterpret_cast<const float4*>(anchors)[i];
-    dec[(size_t)f * N + i] = decode_box(e, a, pp);
-  }
-  __syncthreads();
-  const float* lt = logits + ((size_t)f * N + a0) * C1;
-  for (int e = threadIdx.x; e < total; e += blockDim.x) {
-    int il = e / C1, c = e - il * C1;
-    short pos = -1;
-    if (c != 0) {  // `Postprocessor/Slice`: background column dropped after the sigmoid
-      float sc = sigmoid_score(lt[e], pp.logit_scale);
-      s_score[e] = sc;
-      if (sc > pp.score_thr) pos = (short)atomicAdd(&s_cnt[c - 1], 1);
-    }
-    s_pos[e] = pos;
-  }
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x)
-    s_base[c] = s_cnt[c] > 0 ? atomicAdd(&cand_count[f * C + c], s_cnt[c]) : 0;
-  __syncthreads();
-  for (int e = threadIdx.x; e < total; e += blockDim.x) {
-    const short pos = s_pos[e];
-    if (pos < 0) continue;
-    int il = e / C1, c = e - il * C1;
-    cand[((size_t)f * C + (c - 1)) * N + s_base[c - 1] + pos] =
-        ((unsigned long long)__float_as_uint(s_score[e]) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)(a0 + il));
-  }
 }
 
 // ------------------------------------------------------------------------------------------- K8
@@ -136,20 +84,26 @@ __device__ __forceinline__ void bitonic_desc(unsigned long long* a, int P) {
 }
 
 // grid (classes, frames), 256 threads.  Per (frame, class):
+//  0. scores: the block reads its class's column of the frame's logits (the heads' [N][C+1] output, L2-resident) and
+//     keeps every anchor's sigmoid score in shared memory; anchors at or below the score threshold are marked as no
+//     candidate.  A candidate's key  score_bits << 32 | ~anchor  is formed only when it is gathered (sorting keys
+//     descending gives "score descending, lower anchor index first", the pop order of TF's NonMaxSuppressionV5).
 //  1. candidate keys -> shared memory, in CHUNKS of descending score.  With many candidates (score threshold 1e-8
 //     makes every anchor one) only the head of the order is ever visited before max_per_class boxes are kept or the
 //     early exit fires (most classes stop after two rounds), so the keys are never sorted as a whole: a score
-//     histogram (sign, exponent and 5 mantissa bits of the float: 32 bins per octave) is built once, and each chunk
-//     is "the highest remaining bins that hold >= want keys" (96 for the first chunk, 384 after), gathered from the
-//     L2-resident key list and sorted (bitonic).  A chunk is a whole number of bins and every key of a higher bin is
-//     larger than every key of a lower one, so the visiting order is exactly the descending key order.
-//  2. greedy suppression with exact sequential semantics, 32 candidates per round:
+//     histogram (sign, exponent and 5 mantissa bits of the float: 32 bins per octave), built in the score pass, and
+//     each chunk is "the highest remaining bins that hold >= want keys" (96 for the first chunk, 384 after), gathered
+//     from the scores in shared memory and sorted (bitonic).  A chunk is a whole number of bins and every key of a
+//     higher bin is larger than every key of a lower one, so the visiting order is exactly the descending key order.
+//     A class with at most NMS_PREFILTER_MIN candidates is one chunk of every bin.
+//  2. greedy suppression with exact sequential semantics, 32 candidates per round; warp 0 decodes the round's
+//     candidate boxes from the box encodings and the anchors:
 //     phase 1 (all 8 warps): candidate i vs every box kept in EARLIER rounds (warp w takes candidates
 //     4w..4w+3, lanes stride over the kept list, a ballot decides);
 //     phase 2 (warp 0): walk the 32 candidates in order; a surviving candidate is kept and immediately
 //     suppresses the later candidates of the same round that it overlaps.
 // Output: merge keys  score_bits << 32 | (0xFFFF - class) << 16 | (0xFFFF - rank)  for the kept boxes whose
-// window-clipped area is positive (0 otherwise), plus the anchor index of every kept box.
+// window-clipped area is positive (0 otherwise), plus the decoded corners of every kept box.
 constexpr int KEPT_BINS = 1024;
 // monotone non-decreasing in the score (scores are sigmoid outputs in [0, 1]); resolution 1/1024
 __device__ __forceinline__ int score_bin(unsigned score_bits) {
@@ -164,116 +118,134 @@ constexpr int NMS_BINS = 1024;
 __device__ __forceinline__ int nms_bin(unsigned long long key) {
   return min(NMS_BINS - 1, max(0, (int)(key >> 50) - (100 << 5)));
 }
+__device__ __forceinline__ unsigned long long nms_key(unsigned score_bits, int anchor) {
+  return ((unsigned long long)score_bits << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)anchor);
+}
+constexpr unsigned NMS_NO_CAND = 0xFFFFFFFFu;  // score slot of an anchor that is no candidate (a NaN: never > thr)
+constexpr int NMS_LOADS = 4;  // logits in flight per thread in the score pass (8 would spill at 40 registers)
 
-__global__ void __launch_bounds__(256)
-    k_nms(PostParams pp, const float4* __restrict__ dec, const int* __restrict__ cand_count,
-          const unsigned long long* __restrict__ cand, int sort_cap, int* __restrict__ sel_count,
-          unsigned long long* __restrict__ sel_key, int* __restrict__ sel_idx, int* __restrict__ kept_hist) {
-  extern __shared__ unsigned long long s_a[];  // [sort_cap]: the current chunk, sorted
+// 720 blocks (8 frames x 90 classes) are one wave on 132 SMs at 6 blocks per SM: at most 40 registers per thread
+__global__ void __launch_bounds__(256, 6)
+    k_nms(PostParams pp, const float* __restrict__ enc, const float* __restrict__ logits,
+          const float* __restrict__ anchors, int sort_cap, int* __restrict__ sel_count,
+          unsigned long long* __restrict__ sel_key, float4* __restrict__ sel_box, int* __restrict__ kept_hist) {
+  extern __shared__ unsigned long long s_a[];  // [sort_cap]: the current chunk, sorted; then the scores
+  unsigned* s_score = reinterpret_cast<unsigned*>(s_a + sort_cap);  // [N]: score bits by anchor, or NMS_NO_CAND
   __shared__ float4 s_kept[128];  // normalised corners of the kept boxes
   __shared__ float s_karea[128];
   __shared__ float4 s_cbox[32];  // normalised corners of the round's candidates
   __shared__ float s_carea[32];
-  __shared__ float4 s_craw[32];  // as decoded (for the clipped-area test)
+  __shared__ float4 s_craw[32];  // as decoded (for the clipped-area test and the output)
   __shared__ unsigned s_alive;   // bit i: candidate i of the round survived phase 1
-  __shared__ int s_nkept_sh, s_na, s_cut;
+  __shared__ int s_nkept_sh, s_na, s_cut, s_n;
   __shared__ int s_hist[NMS_BINS];
   __shared__ int s_above[8];
   int* fhist = kept_hist + (size_t)blockIdx.y * KEPT_BINS;  // this frame's histogram of kept, selectable scores
   const int c = blockIdx.x, f = blockIdx.y, C = pp.num_classes, N = pp.num_anchors;
-  const int n = min(cand_count[f * C + c], N);
   const int max_out = min(pp.max_per_class, N);
   unsigned long long* out_key = sel_key + ((size_t)f * C + c) * pp.max_per_class;
-  int* out_idx = sel_idx + ((size_t)f * C + c) * pp.max_per_class;
+  float4* out_box = sel_box + ((size_t)f * C + c) * pp.max_per_class;
   for (int i = threadIdx.x; i < pp.max_per_class; i += blockDim.x) out_key[i] = 0ull;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < NMS_BINS; i += blockDim.x) s_hist[i] = 0;
+  if (threadIdx.x == 0) {
+    s_n = 0;
+    s_nkept_sh = 0;
+  }
+  __syncthreads();
+  // `Postprocessor/convert_scores` + `Postprocessor/Slice` (background column 0 dropped after the sigmoid) for column
+  // c + 1: strided 4-byte loads, all of a thread's issued before any is used
+  const float* col = logits + (size_t)f * N * (C + 1) + (c + 1);
+  int ncand = 0;
+  for (int a0 = 0; a0 < N; a0 += NMS_LOADS * blockDim.x) {
+    float lg[NMS_LOADS];
+#pragma unroll
+    for (int k = 0; k < NMS_LOADS; ++k) {
+      const int a = a0 + k * blockDim.x + threadIdx.x;
+      lg[k] = a < N ? __ldg(col + (size_t)a * (C + 1)) : 0.f;
+    }
+#pragma unroll
+    for (int k = 0; k < NMS_LOADS; ++k) {
+      const int a = a0 + k * blockDim.x + threadIdx.x;
+      const unsigned sb = __float_as_uint(sigmoid_score(lg[k], pp.logit_scale));
+      const bool cand = a < N && __uint_as_float(sb) > pp.score_thr;
+      if (a < N) s_score[a] = cand ? sb : NMS_NO_CAND;
+      // scores of one class crowd into few bins: aggregate equal bins inside the warp (__match_any_sync) so that one
+      // lane per distinct bin issues the shared-memory atomic
+      const int bin = cand ? nms_bin(nms_key(sb, a)) : -1;
+      const unsigned peers = __match_any_sync(0xffffffffu, bin);
+      if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(&s_hist[bin], __popc(peers));
+      ncand += cand;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) ncand += __shfl_xor_sync(0xffffffffu, ncand, o);
+  if (lane == 0 && ncand > 0) atomicAdd(&s_n, ncand);
+  __syncthreads();
+  const int n = s_n;
   if (n == 0) {
     if (threadIdx.x == 0) sel_count[f * C + c] = 0;
     return;
   }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const unsigned long long* ck = cand + ((size_t)f * C + c) * N;
   const bool chunked = n > NMS_PREFILTER_MIN;
-  if (chunked) {
-    for (int i = threadIdx.x; i < NMS_BINS; i += blockDim.x) s_hist[i] = 0;
-    __syncthreads();
-    for (int i0 = 0; i0 < n; i0 += blockDim.x) {
-      // scores of one class crowd into few bins: aggregate equal bins inside the warp (__match_any_sync) so that one
-      // lane per distinct bin issues the shared-memory atomic
-      const int i = i0 + threadIdx.x;
-      const int bin = i < n ? nms_bin(ck[i]) : -1;
-      const unsigned peers = __match_any_sync(0xffffffffu, bin);
-      if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(&s_hist[bin], __popc(peers));
-    }
-  }
-  const float4* fdec = dec + (size_t)f * N;
-  if (threadIdx.x == 0) s_nkept_sh = 0;
-  __syncthreads();
+  const float4* fenc = reinterpret_cast<const float4*>(enc) + (size_t)f * N;
+  const float4* anc = reinterpret_cast<const float4*>(anchors);
 
   bool stop = false;
   int hi_bin = NMS_BINS;  // bins >= hi_bin have been visited
   for (int chunk = 0; !stop; ++chunk) {
-    int count;
-    if (!chunked) {
-      if (chunk > 0) break;
-      int P = 32;
-      while (P < n) P <<= 1;
-      for (int i = threadIdx.x; i < P; i += blockDim.x) s_a[i] = i < n ? ck[i] : 0ull;
-      __syncthreads();
-      bitonic_desc(s_a, P);
-      count = n;
-    } else {
-      if (hi_bin <= 0 || s_nkept_sh >= max_out) break;  // uniform: both were published before a barrier
-      const int want = chunk == 0 ? NMS_CHUNK0 : NMS_CHUNK;
-      if (warp == 0) {  // highest remaining bins first until `want` keys are covered (or nothing is left: cut = 0)
-        int acc = 0, cut = 0;
-        for (int top = hi_bin - 1; top >= 0 && acc < want; top -= 32) {
-          const int b = top - lane;
-          const int v = b >= 0 ? s_hist[b] : 0;
-          int incl = v;  // inclusive prefix over lanes (lane 0 = highest bin)
+    if (hi_bin <= 0 || s_nkept_sh >= max_out) break;  // uniform: both were published before a barrier
+    const int want = chunk == 0 ? NMS_CHUNK0 : NMS_CHUNK;
+    if (warp == 0) {  // highest remaining bins first until `want` keys are covered (or nothing is left: cut = 0)
+      int acc = 0, cut = 0;
+      for (int top = hi_bin - 1; chunked && top >= 0 && acc < want; top -= 32) {
+        const int b = top - lane;
+        const int v = b >= 0 ? s_hist[b] : 0;
+        int incl = v;  // inclusive prefix over lanes (lane 0 = highest bin)
 #pragma unroll
-          for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-          }
-          const unsigned reach = __ballot_sync(0xffffffffu, acc + incl >= want);
-          if (reach) {
-            const int l = __ffs(reach) - 1;
-            cut = top - l;
-            acc += __shfl_sync(0xffffffffu, incl, l);
-            break;
-          }
-          acc += __shfl_sync(0xffffffffu, incl, 31);
-          cut = max(top - 31, 0);
+        for (int o = 1; o < 32; o <<= 1) {
+          const int t = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += t;
         }
-        if (lane == 0) {
-          s_cut = cut;
-          s_na = 0;
+        const unsigned reach = __ballot_sync(0xffffffffu, acc + incl >= want);
+        if (reach) {
+          const int l = __ffs(reach) - 1;
+          cut = top - l;
+          acc += __shfl_sync(0xffffffffu, incl, l);
+          break;
         }
+        acc += __shfl_sync(0xffffffffu, incl, 31);
+        cut = max(top - 31, 0);
       }
-      __syncthreads();
-      const int cut = s_cut;
-      for (int i0 = 0; i0 < n; i0 += blockDim.x) {  // pass over the L2-resident keys: bins [cut, hi_bin)
-        const int i = i0 + threadIdx.x;
-        const unsigned long long k = i < n ? ck[i] : 0ull;
-        const int bin = nms_bin(k);
-        const bool in = i < n && bin >= cut && bin < hi_bin;
-        // warp-aggregated append: one shared-memory atomic per warp instead of one per key
-        const unsigned m = __ballot_sync(0xffffffffu, in);
-        int base_pos = 0;
-        if (lane == 0 && m) base_pos = atomicAdd(&s_na, __popc(m));
-        base_pos = __shfl_sync(0xffffffffu, base_pos, 0);
-        if (in) s_a[base_pos + __popc(m & ((1u << lane) - 1u))] = k;
+      if (lane == 0) {
+        s_cut = cut;
+        s_na = 0;
       }
-      __syncthreads();
-      count = s_na;
-      hi_bin = cut;
-      if (count == 0) continue;  // uniform; an empty range can only be the last one (cut == 0)
-      int P = 32;
-      while (P < count) P <<= 1;
-      for (int i = count + threadIdx.x; i < P; i += blockDim.x) s_a[i] = 0ull;
-      __syncthreads();
-      bitonic_desc(s_a, P);
     }
+    __syncthreads();
+    const int cut = s_cut;
+    for (int i0 = 0; i0 < N; i0 += blockDim.x) {  // pass over the scores: the candidates in bins [cut, hi_bin)
+      const int i = i0 + threadIdx.x;
+      const unsigned sb = i < N ? s_score[i] : NMS_NO_CAND;
+      const unsigned long long k = nms_key(sb, i);
+      const int bin = nms_bin(k);
+      const bool in = sb != NMS_NO_CAND && bin >= cut && bin < hi_bin;
+      // warp-aggregated append: one shared-memory atomic per warp instead of one per key
+      const unsigned m = __ballot_sync(0xffffffffu, in);
+      int base_pos = 0;
+      if (lane == 0 && m) base_pos = atomicAdd(&s_na, __popc(m));
+      base_pos = __shfl_sync(0xffffffffu, base_pos, 0);
+      if (in) s_a[base_pos + __popc(m & ((1u << lane) - 1u))] = k;
+    }
+    __syncthreads();
+    const int count = s_na;
+    hi_bin = cut;
+    if (count == 0) continue;  // uniform; an empty range can only be the last one (cut == 0)
+    int P = 32;
+    while (P < count) P <<= 1;
+    for (int i = count + threadIdx.x; i < P; i += blockDim.x) s_a[i] = 0ull;
+    __syncthreads();
+    bitonic_desc(s_a, P);
     const unsigned long long* sorted = s_a;
     for (int base = 0; base < count; base += 32) {
       const int nkept = s_nkept_sh;
@@ -306,7 +278,7 @@ __global__ void __launch_bounds__(256)
       if (threadIdx.x < 32) {
         if (lane < cnt) {
           const unsigned idx = 0xFFFFFFFFu - (unsigned)(sorted[base + lane] & 0xFFFFFFFFull);
-          const float4 raw = fdec[idx];
+          const float4 raw = decode_box(__ldg(fenc + idx), __ldg(anc + idx), pp);
           const NBox nb = normalise_box(raw);
           s_craw[lane] = raw;
           s_cbox[lane] = nb.c;
@@ -346,7 +318,7 @@ __global__ void __launch_bounds__(256)
             s_karea[nk] = barea;
             float4 cb = clip_unit(s_craw[t]);
             float area = __fmul_rn(__fsub_rn(cb.z, cb.x), __fsub_rn(cb.w, cb.y));
-            out_idx[nk] = (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull));
+            out_box[nk] = s_craw[t];
             out_key[nk] = area > 0.f ? ((key & 0xFFFFFFFF00000000ull) | ((unsigned long long)(0xFFFFu - (unsigned)c) << 16) |
                                         (unsigned long long)(0xFFFFu - (unsigned)nk))
                                      : 0ull;
@@ -444,8 +416,8 @@ constexpr int MERGE_BINS = 2048;   // sign + exponent + 2 mantissa bits of the s
 constexpr int MERGE_CAP = 4096;    // gathered keys that fit the fast path (ties in the cut bin can exceed max_total)
 
 __global__ void __launch_bounds__(MERGE_THREADS)
-    k_merge_filter(PostParams pp, const float4* __restrict__ dec, const int* __restrict__ sel_count,
-                   const unsigned long long* __restrict__ sel_key, const int* __restrict__ sel_idx,
+    k_merge_filter(PostParams pp, const int* __restrict__ sel_count, const unsigned long long* __restrict__ sel_key,
+                   const float4* __restrict__ sel_box,
                    const FrameDesc* __restrict__ frames, const CameraCfg* __restrict__ cams, uint32_t flags,
                    wb_detection* __restrict__ out, uint32_t* __restrict__ verdicts, float* __restrict__ raw_boxes,
                    float* __restrict__ raw_scores, float* __restrict__ raw_classes, int* __restrict__ raw_num) {
@@ -453,7 +425,7 @@ __global__ void __launch_bounds__(MERGE_THREADS)
   __shared__ int s_hist[MERGE_BINS];
   __shared__ unsigned long long s_win[128];
   __shared__ int s_nvalid, s_cut, s_n;
-  const int f = blockIdx.x, C = pp.num_classes, MP = pp.max_per_class, N = pp.num_anchors;
+  const int f = blockIdx.x, C = pp.num_classes, MP = pp.max_per_class;
   const unsigned long long* keys = sel_key + (size_t)f * C * MP;
   const int total = C * MP;
   const int want = min(pp.max_total, 128);
@@ -546,8 +518,7 @@ __global__ void __launch_bounds__(MERGE_THREADS)
     int c = 0xFFFF - (int)((k >> 16) & 0xFFFFull), rank = 0xFFFF - (int)(k & 0xFFFFull);
     score = __uint_as_float((unsigned)(k >> 32));
     cls = (float)c;
-    int idx = sel_idx[((size_t)f * C + c) * MP + rank];
-    box = clip_unit(dec[(size_t)f * N + idx]);
+    box = clip_unit(sel_box[((size_t)f * C + c) * MP + rank]);
   }
   cls = __fadd_rn(cls, pp.class_offset);  // graph node `add` (+1 also on the zero padding)
   if (raw_boxes) {
@@ -574,39 +545,30 @@ __global__ void __launch_bounds__(MERGE_THREADS)
 
 void launch_post(const LaunchCtx& lc, int n, const PostParams& pp, const float* enc, const float* logits,
                  const float* anchors, const FrameDesc* frames, const CameraCfg* cams, uint32_t flags,
-                 float* dec_boxes, int* cand_count, unsigned long long* cand, int* sel_count,
-                 unsigned long long* sel, wb_detection* out, uint32_t* verdicts, float* raw_boxes,
-                 float* raw_scores, float* raw_classes, int* raw_num, int* kept_hist) {
+                 int* sel_count, unsigned long long* sel_key, float4* sel_box, wb_detection* out, uint32_t* verdicts,
+                 float* raw_boxes, float* raw_scores, float* raw_classes, int* raw_num, int* kept_hist) {
   const int C = pp.num_classes, N = pp.num_anchors;
-  cudaMemsetAsync(cand_count, 0, sizeof(int) * (size_t)n * C, lc.stream);
   cudaMemsetAsync(kept_hist, 0, sizeof(int) * (size_t)n * KEPT_BINS, lc.stream);
-  dim3 g1((N + DEC_TILE - 1) / DEC_TILE, n);
-  const size_t dec_smem = (size_t)DEC_TILE * (C + 1) * (sizeof(float) + sizeof(short)) + 2 * sizeof(int) * C + 16;
-  k_decode_scores<<<g1, 256, dec_smem, lc.stream>>>(pp, enc, logits, anchors, reinterpret_cast<float4*>(dec_boxes),
-                                                    cand_count, cand);
-  ++*lc.launch_counter;
   int sort_cap = 32;
   while (sort_cap < N) sort_cap <<= 1;
-  // sel holds keys [n][C][max_per_class] followed by anchor indices (int) of the same shape
-  unsigned long long* sel_key = sel;
-  int* sel_idx = reinterpret_cast<int*>(sel + (size_t)n * C * pp.max_per_class);
   static PerDeviceFlag attr_done;
   if (!attr_done.get()) {
-    cudaFuncSetAttribute(k_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, 132 * 1024);
-    cudaFuncSetAttribute(k_decode_scores, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    cudaFuncSetAttribute(k_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(k_merge_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
     attr_done.set();
   }
-  k_nms<<<dim3(C, n), 256, sizeof(unsigned long long) * sort_cap, lc.stream>>>(
-      pp, reinterpret_cast<const float4*>(dec_boxes), cand_count, cand, sort_cap, sel_count, sel_key, sel_idx, kept_hist);
+  // the chunk buffer (every key may land in one chunk) and the scores: 23.5 KB for 1917 anchors
+  const size_t nms_smem = sizeof(unsigned long long) * sort_cap + sizeof(unsigned) * (size_t)N;
+  k_nms<<<dim3(C, n), 256, nms_smem, lc.stream>>>(pp, enc, logits, anchors, sort_cap, sel_count, sel_key, sel_box,
+                                                  kept_hist);
   ++*lc.launch_counter;
   {
     int P = 32;
     while (P < C * pp.max_per_class) P <<= 1;
     const size_t merge_smem = sizeof(unsigned long long) * (size_t)std::max(P, MERGE_CAP);
-    k_merge_filter<<<n, MERGE_THREADS, merge_smem, lc.stream>>>(
-        pp, reinterpret_cast<const float4*>(dec_boxes), sel_count, sel_key, sel_idx, frames, cams, flags, out,
-        verdicts, raw_boxes, raw_scores, raw_classes, raw_num);
+    k_merge_filter<<<n, MERGE_THREADS, merge_smem, lc.stream>>>(pp, sel_count, sel_key, sel_box, frames, cams, flags,
+                                                                out, verdicts, raw_boxes, raw_scores, raw_classes,
+                                                                raw_num);
   }
   ++*lc.launch_counter;
 }

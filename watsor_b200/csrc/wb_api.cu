@@ -76,12 +76,13 @@ struct Slot {
   DevBuf<uint8_t> d_frames;
   size_t d_frames_cap = 0;
   DevBuf<void> arena;
-  DevBuf<float> d_enc, d_logits, d_dec;
+  DevBuf<float> d_enc, d_logits;
   DevBuf<float> d_partial;  // split-K scratch
   size_t partial_floats = 0;
-  DevBuf<int> d_cand_count, d_sel_count;
+  DevBuf<int> d_sel_count;
   DevBuf<int> d_kept_hist;  // [B][1024] per-frame histogram of kept scores (exact NMS early exit)
-  DevBuf<unsigned long long> d_cand, d_sel;
+  DevBuf<unsigned long long> d_sel;  // [B][C][max_per_class] merge keys of the kept boxes
+  DevBuf<float4> d_sel_box;          // ... and their decoded corners
   DevBuf<wb_detection> d_out;
   PinnedBuf<wb_detection> h_out;
   DevBuf<uint32_t> d_verdicts;
@@ -191,14 +192,12 @@ static int alloc_slot(wb_ctx* c, Slot& s) {
   CK(alloc(s.arena, (size_t)B * c->hdr.arena_elems * c->elem_size() + 1024));
   CK(alloc(s.d_enc, sizeof(float) * (size_t)B * N * 4));
   CK(alloc(s.d_logits, sizeof(float) * (size_t)B * N * (C + 1)));
-  CK(alloc(s.d_dec, sizeof(float) * (size_t)B * N * 4));
   s.partial_floats = (size_t)4 * 1024 * 1024 + (size_t)B * 512 * 1024;
   CK(alloc(s.d_partial, sizeof(float) * s.partial_floats));
-  CK(alloc(s.d_cand_count, sizeof(int) * (size_t)B * C));
   CK(alloc(s.d_sel_count, sizeof(int) * (size_t)B * C));
   CK(alloc(s.d_kept_hist, sizeof(int) * (size_t)B * 1024));
-  CK(alloc(s.d_cand, sizeof(unsigned long long) * (size_t)B * C * N));
-  CK(alloc(s.d_sel, (sizeof(unsigned long long) + sizeof(int)) * (size_t)B * C * MP));
+  CK(alloc(s.d_sel, sizeof(unsigned long long) * (size_t)B * C * MP));
+  CK(alloc(s.d_sel_box, sizeof(float4) * (size_t)B * C * MP));
   CK(alloc(s.d_out, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
   CK(alloc(s.h_out, sizeof(wb_detection) * (size_t)B * WB_MAX_DETECTIONS));
   CK(alloc(s.d_verdicts, sizeof(uint32_t) * (size_t)B * WB_MAX_DETECTIONS));
@@ -608,7 +607,7 @@ static int run_post(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, 
   float* rs = want_raw ? rb + (size_t)c->max_batch * WB_MAX_DETECTIONS * 4 : nullptr;
   float* rc = want_raw ? rs + (size_t)c->max_batch * WB_MAX_DETECTIONS : nullptr;
   launch_post(lc, n, c->pp, s.d_enc, s.d_logits, c->tensor(c->hdr.anchors_tensor), s.d_desc,
-              windowed ? nullptr : c->d_cams.h, flags, s.d_dec, s.d_cand_count, s.d_cand, s.d_sel_count, s.d_sel, s.d_out,
+              windowed ? nullptr : c->d_cams.h, flags, s.d_sel_count, s.d_sel, s.d_sel_box, s.d_out,
               s.d_verdicts, rb, rs, rc, (want_raw || windowed) ? s.d_raw_num.h : nullptr, s.d_kept_hist);
   if (windowed)
     launch_window_merge(lc, n_frames, c->pp, s.d_win, s.d_out, s.d_raw_num, c->d_cams, flags, s.d_wout, s.d_wverd);
