@@ -1,6 +1,7 @@
 """Float64 restatement of the backbone layer operations, per-element error bounds for the CUDA kernels that run them,
 bit-exact float32 restatements where a kernel's order of operations is defined, and `plan()`, the kernel dispatch of
-csrc/ restated so that a test can prove which branch a layer reaches.
+csrc/ restated so that a test can prove which branch a layer reaches.  Everything that depends on the precision mode
+reads its row of `PRECISIONS`.
 
 Everything is numpy on NHWC arrays.  The reference operations follow the TensorFlow op definitions (Conv2D,
 DepthwiseConv2dNative, MaxPool, AvgPool with padding SAME; ConcatV2; Add; the box-predictor Reshape + concat), not the
@@ -15,8 +16,8 @@ range cannot hide behind that range:
     |ŷ - y| <= B_acc·|s| + (epilogue roundings),     B_acc = (c_mode + steps·t_step + γ_n) · P + 1e-30
 
 with u = 2^-24 and γ_n = n·u / (1 - n·u).  The epilogue `fl(fl(ẑ·s) + o)` adds u·|ẑ·s| and u·|ẑ·s + o|; ReLU6 is
-1-Lipschitz, so the bound passes through it; bf16 storage adds the final rounding to 8 significant bits, at most
-2^-8 of the stored value.  The mode terms:
+1-Lipschitz, so the bound passes through it; 16-bit storage adds the final rounding of the stored value (below).
+Heads write fp32 in every mode.  The mode terms:
 
 * fp32 FFMA (precision 0, `k_gemm_cc`, the stem, depthwise): every product enters an fmaf chain (split-K: chains
   of a split, then an ordered sum of the splits), one rounding per step and at most K + splits steps:
@@ -33,12 +34,26 @@ with u = 2^-24 and γ_n = n·u / (1 - n·u).  The epilogue `fl(fl(ẑ·s) + o)` 
 * tf32x1 (precision 3, diagnostic): the tensor core reads the fp32 operands as TF32 (each within 2^-10 relative):
   c = 2^-9 + 2^-20; the accumulator runs across the whole k range of a split: steps = 4 per k-block; n = splits.
 * bf16 (precision 1): the same truncating chain (`wgmma.k16`: 17 addends, t_step = 17·2^-23, 4 steps per 64-value
-  k-block) on the bf16-rounded activations and weights, c = 0, n = splits; then one bf16 rounding of the output.
-  Heads write fp32 in every mode.
+  k-block) on the bf16-rounded activations and weights, c = 0, n = splits; then one bf16 rounding of the output, at
+  most 2^-8 of the stored value.
+* fp16 (precision 4, `k_gemm_tc<3>`) runs bf16's MMA sequence on fp16 operands (`wgmma.k16.f32.f16.f16`): bf16's chain
+  constants.  A product of two fp16 values (11 × 11 significant bits) is exact in fp32, and so is a product with a
+  subnormal fp16 factor (at least 2^-48, far above fp32's normal range floor): the chain needs no absolute term as long
+  as the tensor core keeps subnormal operands (tests/test_gpu_fp16.py checks a 1x1 whose weights are all fp16
+  subnormals against this bound).  The output rounding to fp16 (round to nearest even, subnormals kept) errs by at
+  most 2^-11·|y| for a normal result and by half the subnormal spacing, 2^-25, for a subnormal one: 2^-11·|y| + 2^-25.
+  That holds below the clamp (|y| <= 65504); above it the store saturates at ±65504 by design.
 
-The depthwise kernels are fmaf chains of at most 9 terms; they are bounded like the fp32 GEMM (γ_9), not emulated,
-because float64 cannot reproduce a fused multiply-add's single rounding without double rounding.
+The CUDA-core kernels (stem, depthwise, `k_gemm_cc`) keep their fp32 arithmetic in every mode and only store the
+mode's type: their bound is the fp32 one plus the output rounding.  The depthwise kernels are fmaf chains of at most 9
+terms; they are bounded like the fp32 GEMM (γ_9), not emulated, because float64 cannot reproduce a fused multiply-add's
+single rounding without double rounding.
+
+Dispatch: fp16 and bf16 elements are both 2 bytes, which is all the tensor-core gate and the GEMM's k-block count
+depend on, and both modes refuse residual and dw→1×1 fusion, so precision 4's plan is bf16's but for the GEMM's MODE.
 """
+from collections import namedtuple
+
 import numpy as np
 
 from watsor_b200.model import (ACT_RELU6, OP_ADD, OP_AVGPOOL, OP_CONV, OP_COPY, OP_DW, OP_HEAD, OP_MAXPOOL, OP_PW,
@@ -46,9 +61,13 @@ from watsor_b200.model import (ACT_RELU6, OP_ADD, OP_AVGPOOL, OP_CONV, OP_COPY, 
 
 U = 2.0 ** -24            # fp32 unit roundoff
 U_BF16 = 2.0 ** -8        # bf16 unit roundoff (8 significant bits)
+U_FP16 = 2.0 ** -11       # fp16 unit roundoff (11 significant bits)
+FP16_SUB_HALF = 2.0 ** -25  # half the spacing of fp16 subnormals: the absolute rounding error of a subnormal result
+FP16_MAX = 65504.0        # largest finite fp16: the activation stores clamp to it
 TINY = 1e-30              # absolute floor: products of subnormal TF32 halves may be flushed to zero
 
-# (c, truncating steps per k-block, t_step): see the module docstring
+# (c, truncating steps per k-block, t_step) of a tensor-core accumulation chain, by PRECISIONS' `chain` key; 0 is the
+# fp32 FFMA chain of the CUDA-core kernels: see the module docstring
 MODE_CONSTANTS = {
     0: (0.0, 0, 0.0),
     2: (3.01 * 2.0 ** -20, 12, 9 * 2.0 ** -23),
@@ -148,15 +167,19 @@ def head_scatter(y, anchors_per_loc, n_box, row_off, enc, logits):
 
 
 # ------------------------------------------------------------------------------------------------- error bounds
-def dense_bound(P, zs, y_ref, scale, offset, mode, k_blocks=1, splits=1, kb_per=None, K=None, bf16_out=False):
-    """Per-element bound on |kernel - reference| of a dense layer (module docstring).  P = Σ|a|·|w|, zs = the exact
-    z·s and y_ref = act(z·s + o), all broadcast to the output's shape.  K: length of the fp32 chain (mode 0);
-    k_blocks / kb_per: tensor-core k-blocks of the layer / of one split."""
-    c, steps, t_step = MODE_CONSTANTS[mode]
+def dense_bound(P, zs, y_ref, scale, offset, precision, k_blocks=1, splits=1, kb_per=None, K=None, tc=True, head=False):
+    """Per-element bound on |kernel - reference| of a dense layer of a `precision` engine (module docstring).  P =
+    Σ|a|·|w|, zs = the exact z·s and y_ref = act(z·s + o), all broadcast to the output's shape.  tc: the layer runs on
+    the tensor-core GEMM (else on the CUDA cores' fp32 chain); K: length of the fp32 chain; k_blocks / kb_per:
+    tensor-core k-blocks of the layer / of one split; head: the output is written as fp32, not stored as an
+    activation."""
+    mode = PRECISIONS[precision]
+    chain = mode.chain if tc else 0
+    c, steps, t_step = MODE_CONSTANTS[chain]
     kb_per = k_blocks if kb_per is None else kb_per
-    if mode == 0:
+    if chain == 0:
         rel = gamma(K + splits)
-    elif mode == 2:
+    elif chain == 2:
         rel = c + steps * t_step + gamma(k_blocks + splits)
     else:
         rel = c + steps * kb_per * t_step + gamma(splits)
@@ -164,14 +187,15 @@ def dense_bound(P, zs, y_ref, scale, offset, mode, k_blocks=1, splits=1, kb_per=
     b = rel * P * s + TINY
     b = b + U * (np.abs(zs) + b)                                             # fl(ẑ·s)
     b = b + U * (np.abs(zs + np.asarray(offset, np.float64)) + b)           # fl(· + o)
-    if bf16_out:
-        b = b + U_BF16 * (np.abs(y_ref) + b)
+    if mode.out_round and not head:
+        rel_out, abs_out = mode.out_round
+        b = b + rel_out * (np.abs(y_ref) + b) + abs_out
     return b
 
 
-def chain_bound(P, zs, y_ref, scale, offset, terms, bf16_out=False):
-    """An fmaf chain of `terms` products (stem, depthwise), then the affine epilogue."""
-    return dense_bound(P, zs, y_ref, scale, offset, 0, K=terms - 1, splits=1, bf16_out=bf16_out)
+def chain_bound(P, zs, y_ref, scale, offset, terms, precision=0):
+    """An fmaf chain of `terms` products (stem, depthwise), the affine epilogue, then the store of `precision`."""
+    return dense_bound(P, zs, y_ref, scale, offset, precision, K=terms - 1, splits=1, tc=False)
 
 
 # -------------------------------------------------------------------------------------- bit-exact restatements
@@ -182,23 +206,57 @@ def bf16_round(x):
     return u.astype(np.uint32).view(np.float32)
 
 
-def _store(x, bf16):
-    return bf16_round(x) if bf16 else x.astype(np.float32)
+def fp16_round(x):
+    """float32 -> fp16 (round to nearest even, subnormals kept) -> float32, as __float2half_rn (no NaN inputs here).
+    Magnitudes from 65520 up become inf, as they do there; the activation stores clamp first (fp16_store)."""
+    x = np.asarray(x, np.float32).astype(np.float64)
+    a = np.abs(x)
+    _, ex = np.frexp(a)                             # a = m·2^ex with m in [0.5, 1): exponent ex - 1
+    q = 2.0 ** (np.maximum(ex - 1, -14) - 10)       # the fp16 spacing at a: 2^(e - 10), 2^-24 among the subnormals
+    r = np.round(a / q) * q                         # a / q is exact; np.round rounds half to even
+    r = np.where(r > FP16_MAX, np.inf, r)
+    return np.copysign(r, x).astype(np.float32)
 
 
-def add_f32(a, b, bf16=False):
+def fp16_store(x):
+    """ActIO<__half>::st / st4: clamp to ±65504, then round to fp16."""
+    return fp16_round(np.clip(np.asarray(x, np.float32), -FP16_MAX, FP16_MAX))
+
+
+def f32_store(x):
+    return np.asarray(x, np.float32)
+
+
+# The precision modes by wb_create's number; csrc/wb_api.cu has the same table for the library.
+#   name: in test IDs.  storage: the activation type in kernel names.  store: its bit-exact store.
+#   out_round: (relative, absolute) rounding of a stored activation, or None.
+#   tc_bytes, tc_mode, tc_round: the tensor-core GEMM's operand bytes, k_gemm_tc MODE and the host rounding of its
+#   weights, or None: no tensor cores.  chain: the MODE_CONSTANTS key of its accumulation.
+#   fuse_add: a linear 1x1 -> residual Add runs as one GEMM (fp32 storage: the shortcut is added in the epilogue).
+Precision = namedtuple('Precision', 'name storage store out_round tc_bytes tc_mode tc_round chain fuse_add')
+PRECISIONS = [
+    Precision('fp32', 'float', f32_store, None, None, None, None, 0, False),
+    Precision('bf16', '__nv_bfloat16', bf16_round, (U_BF16, 0.0), 2, 0, bf16_round, 1, False),
+    Precision('tf32x3', 'float', f32_store, None, 4, 2, f32_store, 2, True),
+    Precision('tf32x1', 'float', f32_store, None, 4, 1, f32_store, 3, True),
+    Precision('fp16', '__half', fp16_store, (U_FP16, FP16_SUB_HALF), 2, 3, fp16_round, 1, False),
+]
+
+
+def add_f32(a, b, precision=0):
     """k_add: one float32 addition per element, stored as T."""
-    return _store(np.asarray(a, np.float32) + np.asarray(b, np.float32), bf16)
+    return PRECISIONS[precision].store(np.asarray(a, np.float32) + np.asarray(b, np.float32))
 
 
-def copy_channels_f32(parts, row_offs, total_c, bf16=False):
-    """k_copy_channels: a copy (bf16 storage holds bf16 values already)."""
-    return _store(concat([np.asarray(p, np.float32) for p in parts], row_offs, total_c), bf16)
+def copy_channels_f32(parts, row_offs, total_c, precision=0):
+    """k_copy_channels: a copy (16-bit storage holds 16-bit values already)."""
+    return PRECISIONS[precision].store(concat([np.asarray(p, np.float32) for p in parts], row_offs, total_c))
 
 
-def pool_f32(x, k, stride, kind, bf16=False):
+def pool_f32(x, k, stride, kind, precision=0):
     """k_pool: the max of the in-image taps, or their __fadd_rn sum in (ky, kx) order from +0, then __fdiv_rn by the
-    number of in-image taps."""
+    number of in-image taps, stored as T."""
+    store = PRECISIONS[precision].store
     x = np.asarray(x, np.float32)
     xp, oh, ow = _same_padded(x, k, k, stride)
     mp, _, _ = _same_padded(np.ones(x.shape[:3] + (1,), np.float32), k, k, stride)
@@ -207,13 +265,13 @@ def pool_f32(x, k, stride, kind, bf16=False):
         acc = np.full(x.shape[:1] + (oh, ow, x.shape[3]), -np.inf, np.float32)
         for (_, _, xs), (_, _, ms) in taps:
             acc = np.where(ms > 0, np.maximum(acc, xs), acc)
-        return _store(acc, bf16)
+        return store(acc)
     acc = np.zeros(x.shape[:1] + (oh, ow, x.shape[3]), np.float32)
     cnt = np.zeros(x.shape[:1] + (oh, ow, 1), np.float32)
     for (_, _, xs), (_, _, ms) in taps:
         acc = np.where(ms > 0, (acc + xs).astype(np.float32), acc)
         cnt = cnt + ms
-    return _store((acc / cnt).astype(np.float32), bf16)
+    return store((acc / cnt).astype(np.float32))
 
 
 # ----------------------------------------------------------------------------------------------------- dispatch
@@ -236,8 +294,9 @@ PARTIAL_FLOATS_MIN = 4 * 1024 * 1024
 
 
 def tc_supported(L, precision, env=()):
-    """tc_layer_supported (csrc/kernels_tc.cu): a 1x1 needs K-major rows of a multiple of 16 bytes."""
-    elem = 2 if precision == 1 else 4
+    """tc_layer_supported (csrc/kernels_tc.cu) in a mode with tensor cores: a 1x1 needs K-major rows of a multiple of
+    16 bytes."""
+    elem = PRECISIONS[precision].tc_bytes
     if L.op in (OP_PW, OP_HEAD) and L.kh == 1 and L.kw == 1 and L.stride == 1 and L.in_c * elem % 16 == 0:
         return True
     return (L.op == OP_CONV and L.in_c % 64 == 0 and L.out_h * L.out_w <= BLOCK_M and L.stride <= 8 and
@@ -271,9 +330,10 @@ def plan(L, n, precision, sms, env=(), fuse_add_next=False):
     if L.op == OP_COPY:
         return dict(kernel='k_copy_channels', launches=1, branches={'copy'})
     M, K = n * L.out_h * L.out_w, L.kh * L.kw * L.in_c
-    if precision != 0 and tc_supported(L, precision, env):
+    mode = PRECISIONS[precision]
+    if mode.tc_mode is not None and tc_supported(L, precision, env):
         conv = L.op == OP_CONV
-        elem = 2 if precision == 1 else 4
+        elem = mode.tc_bytes
         hw = L.out_h * L.out_w
         rpt = (BLOCK_M // hw) * hw if conv else BLOCK_M
         bn = pick_block_n(L.n_pad)
@@ -292,15 +352,15 @@ def plan(L, n, precision, sms, env=(), fuse_add_next=False):
             kb_per = _ceil(kb, min(sms // tiles, kb // 8, 8))
             splits = _ceil(kb, kb_per)
             br.add('tc:split%d' % splits)
-        fused = fuse_add_next and precision in (2, 3) and L.op == OP_PW and L.act != ACT_RELU6 and \
+        fused = fuse_add_next and mode.fuse_add and L.op == OP_PW and L.act != ACT_RELU6 and \
             'WB_NO_FUSE_ADD' not in env
         if fuse_add_next:
             br.add('fuse_add:yes' if fused else 'fuse_add:no')
-        return dict(kernel='k_gemm_tc', mode={1: 0, 3: 1, 2: 2}[precision], bn=bn, tiles=tiles, k_blocks=kb,
+        return dict(kernel='k_gemm_tc', mode=mode.tc_mode, bn=bn, tiles=tiles, k_blocks=kb,
                     kb_per=kb_per, splits=splits, rows_per_tile=rpt, launches=1 + (fuse_add_next and not fused),
                     fused_add=fused, branches=br)
     br = set()
-    if precision != 0:
+    if mode.tc_mode is not None:
         br.add('tc:unsupported_conv' if L.op == OP_CONV else 'tc:unsupported_1x1')
     if fuse_add_next:
         br.add('fuse_add:no')
@@ -326,9 +386,9 @@ def plan(L, n, precision, sms, env=(), fuse_add_next=False):
     return dict(kernel='k_gemm_cc', tile=64, splits=splits, launches=1 + (splits > 1) + fuse_add_next, branches=br)
 
 
-def kernel_name_pattern(p, bf16):
+def kernel_name_pattern(p, precision):
     """Substring of the demangled name of the kernel plan() names (as torch.profiler reports it)."""
-    t = '__nv_bfloat16' if bf16 else 'float'
+    t = PRECISIONS[precision].storage
     k = p['kernel']
     if k == 'k_gemm_tc':
         return 'k_gemm_tc<%d, %d>' % (p['mode'], p['bn'])

@@ -1,53 +1,29 @@
 """The fp16 mode (precision 4) on the GPU: every backbone kernel that runs in bf16 runs again in fp16 against the float64
-restatement of tests/layer_reference.py (fp16 storage, bounds and dispatch: tests/fp16_reference.py), the stem on
-camera frames, the frame path's bit-identity with the stage path, saturation of overflowing activations at ±65504,
-the refusal of weights beyond the fp16 range, and the whole-network error of fp16 against bf16's on the configs[2]
-model."""
+restatement of tests/layer_reference.py, the stem on camera frames, the frame path's bit-identity with the stage path,
+saturation of overflowing activations at ±65504, the refusal of weights beyond the fp16 range, and the whole-network
+error of fp16 against bf16's on the configs[2] model."""
 import numpy as np
 import pytest
 
-from tests import fp16_reference as F
 from tests import layer_reference as R
 from tests import test_gpu_frame_path as FP
 from tests import test_gpu_layer_kernels as LK
 from tests import workload
 from tests.artist import artist_frame
 from tests.test_gpu_frame_path import batches  # noqa: F401  (the frame batches fixture, shared with that module)
+from tests.test_gpu_layer_kernels import report  # noqa: F401  (the largest error / bound per family)
 from watsor_b200._lib import WatsorB200Error
 from watsor_b200.engine import PRECISION_BF16_TC, PRECISION_FP16_TC, Engine
 from watsor_b200.model import ACT_NONE, ACT_RELU6, OP_HEAD, Model, _Emitter
 
 pytestmark = pytest.mark.gpu
 FP16 = PRECISION_FP16_TC
-WORST = {}          # family -> largest error / bound
-
-
-@pytest.fixture(scope='module', autouse=True)
-def report():
-    yield
-    if WORST:
-        print('\nfp16: largest error / bound per family:')
-        for fam, r in sorted(WORST.items()):
-            print('  %-18s %.3g' % (fam, r))
-
-
-def _record(family, err, bound):
-    ratio = float(np.max(err / bound))
-    WORST[family] = max(WORST.get(family, 0.0), ratio)
-    return ratio
 
 
 # --------------------------------------------------------------------------------------- (1) every kernel vs float64
-# every case that runs in bf16, and a 1x1 whose weights are all fp16 subnormals (|w| < 2^-14): the bound has no
-# absolute term for the product chain, so a tensor core that flushed subnormal operands would fail it
-SUBNORMAL = LK.case('pw_subnormal_weights_K64_N64_10_n2', 'tc_pw', ('gemm', 10, 64, 64, 1, 1, ACT_NONE), 2, (FP16,),
-                    {'all': {'kernel': 'k_gemm_tc', 'splits': 1}})
-CASES = [c for c in LK.CASES if 1 in c.precisions] + [SUBNORMAL]
-
-
-def _subnormal_weights(m, L, seed):
+def _subnormal_weights(m, L):
     """the tested 1x1's weights -> fp16 subnormals of both signs, scale 1, offset 0: y = z exactly"""
-    rng = np.random.default_rng(seed)
+    rng = np.random.default_rng(7)
     w = m.tensors[L.w_tensor]
     m.tensors[L.w_tensor] = (rng.choice([-1.0, 1.0], w.shape) * rng.uniform(2.0 ** -24, 2.0 ** -15, w.shape)).astype(np.float32)
     m.tensors[L.scale_tensor] = np.ones_like(m.tensors[L.scale_tensor])
@@ -55,149 +31,23 @@ def _subnormal_weights(m, L, seed):
     assert np.all(np.abs(m.tensors[L.w_tensor]) < 2.0 ** -14)
 
 
-def _weights(m, L, tc):
-    K = L.kh * L.kw * L.in_c
-    w = np.asarray(m.tensors[L.w_tensor], np.float32).reshape(K, L.n_pad)[:, :L.out_c]
-    if tc:
-        w = F.fp16_round(w)             # the tensor-core weights are rounded to fp16 once on the host
-    return w.astype(np.float64).reshape(L.kh, L.kw, L.in_c, L.out_c)
+# every case that runs in bf16, and a 1x1 whose weights are all fp16 subnormals (|w| < 2^-14): the bound has no
+# absolute term for the product chain, so a tensor core that flushed subnormal operands would fail it
+SUBNORMAL = LK.case('pw_subnormal_weights_K64_N64_10_n2', 'subnormal_w', ('gemm', 10, 64, 64, 1, 1, ACT_NONE), 2,
+                    (FP16,), {'all': {'kernel': 'k_gemm_tc', 'splits': 1}}, prepare=_subnormal_weights)
+CASES = [c for c in LK.CASES if 1 in c.precisions] + [SUBNORMAL]
 
 
 @pytest.mark.parametrize('c', CASES, ids=lambda c: c.name + '-fp16')
 def test_layer_kernel_fp16(c):
-    m, li, inputs, (h, w) = LK.build(c.spec, seed=len(c.name))
-    L = m.layers[li]
-    if c is SUBNORMAL:
-        _subnormal_weights(m, L, 7)
-    sms = LK._sms()
-    pre = np.random.default_rng(c.n).standard_normal((c.n, h, w, 3)).astype(np.float32)
-    xs, (enc, lg, y), launches, kernels = LK._run(m, li, inputs, pre, FP16, c.env)
-
-    # ---- the branch: plan(), launch count, kernel name (+ cluster split); the claims are bf16's (same plan)
-    plans = [F.plan(Li, c.n, sms, c.env) for Li in m.layers[:li + 1]]
-    p = plans[-1]
-    want = LK.claim_for(c, 1 if 1 in c.precisions else FP16)
-    assert {k: p[k] for k in want} == want, (p, want)
-    assert launches == sum(q['launches'] for q in plans), (launches, plans)
-    names = [k for k, _ in kernels]
-    assert len(names) == launches, names
-    last = len(kernels) - 1
-    if p['kernel'] == 'k_gemm_cc' and p['splits'] > 1:
-        assert 'k_splitk_reduce<__half>' in names[last], names
-        last -= 1
-    tested = kernels[last]
-    assert F.kernel_name_pattern(p) in tested[0], (tested, p, names)
-    if p['kernel'] == 'k_gemm_tc' and tested[1] is not None:
-        assert tested[1][2] == p['splits'], (tested, p)
-
-    # ---- the arithmetic
-    kind = c.spec[0]
-    f64 = [np.asarray(x, np.float64) for x in xs]
-    if kind in ('pool', 'add', 'concat'):
-        if kind == 'pool':
-            want_y = F.pool_f32(xs[0], L.kh, L.stride, c.spec[5])
-        elif kind == 'add':
-            want_y = F.add_f32(xs[0], xs[1])
-        else:
-            cl = [m.layers[i] for i in range(li - 2, li + 1)]
-            want_y = F.copy_channels_f32(xs, [q.row_off for q in cl], L.out_c)
-        assert np.array_equal(y, want_y)
-        assert np.abs(y).max() > 0
-        return
-    sc = np.asarray(m.tensors[L.scale_tensor], np.float64)[:L.out_c]
-    of = np.asarray(m.tensors[L.offset_tensor], np.float64)[:L.out_c]
-    if kind in ('stem', 'dw'):
-        if kind == 'stem':
-            a, wt, terms = pre.astype(np.float64), _weights(m, L, False), L.kh * L.kw * 3
-            z, P = R.conv2d(a, wt, L.stride), R.conv2d(np.abs(a), np.abs(wt), L.stride)
-        else:
-            wt, terms = np.asarray(m.tensors[L.w_tensor], np.float64).reshape(3, 3, L.out_c), 9
-            z, P = R.depthwise(f64[0], wt, L.stride), R.depthwise(np.abs(f64[0]), np.abs(wt), L.stride)
-        yr = R.affine(z, sc, of, L.act)
-        bound = F.chain_bound(P, z * sc, yr, sc, of, terms)
-        err = np.abs(y - yr)
-        _record(c.family, err, bound)
-        assert np.all(err <= bound)
-        return
-    tc = p['kernel'] == 'k_gemm_tc'
-    mode = FP16 if tc else 0
-
-    def bound_for(q, P, z, sc, of, yr, is_head):
-        if mode == 0:
-            return F.dense_bound(P, z * sc, yr, sc, of, 0, K=L.kh * L.kw * L.in_c, splits=q['splits'], fp16_out=not is_head)
-        return F.dense_bound(P, z * sc, yr, sc, of, mode, k_blocks=q['k_blocks'], splits=q['splits'], kb_per=q['kb_per'],
-                             fp16_out=not is_head)
-
-    if L.op == OP_HEAD:
-        ref, bnd = [np.zeros(enc.shape), np.zeros(lg.shape)], [np.zeros(enc.shape), np.zeros(lg.shape)]
-        for hl in (q for q in m.layers if q.op == OP_HEAD):
-            hw_t = _weights(m, hl, tc)
-            hsc = np.asarray(m.tensors[hl.scale_tensor], np.float64)[:hl.out_c]
-            hof = np.asarray(m.tensors[hl.offset_tensor], np.float64)[:hl.out_c]
-            z, P = R.conv2d(f64[0], hw_t, 1), R.conv2d(np.abs(f64[0]), np.abs(hw_t), 1)
-            yr = R.affine(z, hsc, hof, hl.act)
-            hq = F.plan(hl, c.n, sms, c.env)
-            R.head_scatter(yr, hl.anchors_per_loc, hl.n_box, hl.row_off, *ref)
-            R.head_scatter(bound_for(hq, P, z, hsc, hof, yr, True), hl.anchors_per_loc, hl.n_box, hl.row_off, *bnd)
-        err = np.concatenate([np.abs(enc - ref[0]).ravel(), np.abs(lg - ref[1]).ravel()])
-        yr = np.concatenate([r.ravel() for r in ref])
-        bound = np.concatenate([b.ravel() for b in bnd])
-    else:
-        wt = _weights(m, L, tc)
-        z, P = R.conv2d(f64[0], wt, L.stride), R.conv2d(np.abs(f64[0]), np.abs(wt), L.stride)
-        yr = R.affine(z, sc, of, L.act)
-        err = np.abs(y - yr)
-        bound = bound_for(p, P, z, sc, of, yr, False)
-    ratio = _record('subnormal_w' if c is SUBNORMAL else c.family, err, bound)
-    assert np.all(err <= bound), (ratio, float(err.max()))
-    assert np.abs(yr).max() > 0
+    LK.check_layer(c, FP16)
 
 
 # ------------------------------------------------------------------------------------------- (2) stem on frames
 @pytest.mark.parametrize('group', FP.GROUPS)
 @pytest.mark.parametrize('stem', list(FP.STEMS))
 def test_stem_on_frames_fp16(batches, stem, group):  # noqa: F811
-    """test_gpu_frame_path (a) in fp16: bit-identical to the stem on preprocess() of the same RGB images, and within
-    the float64 bound on oracle.preprocess, for both stem kernels."""
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    m = FP._stem_model(stem)
-    L = m.layers[0]
-    shape = (L.out_h, L.out_w, L.out_c)
-    plan = F.plan(L, 1, torch.cuda.get_device_properties(0).multi_processor_count)
-    with Engine(m.to_blob(), device=0, max_batch=FP.MAX_IMAGES, precision=FP16) as e:
-        runs = []
-        for fmt, cams, frames, images in batches[group]:
-            FP._configure(e, cams)
-            runs += [(fmt, cams, frames, images, False, frames), (fmt, cams, frames, images, True, FP._to_device(frames))]
-        for _ in range(3):
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                got = []
-                for fmt, cams, _, images, on_dev, src in runs:
-                    ptrs = [t.data_ptr() for t in src] if on_dev else src
-                    _, _, y, n_img = e.backbone_frames(ptrs, list(cams), stop_layer=0, layer_shape=shape,
-                                                       pixel_format=fmt, frames_on_device=on_dev)
-                    assert n_img == len(images) and e.last_launch_count() == 1
-                    got.append(y)
-                torch.cuda.synchronize()
-            kernels = [k for k, _ in LK._kernels(prof)]
-            if len(kernels) == len(runs):
-                break
-        assert len(kernels) == len(runs), kernels
-        assert all(F.kernel_name_pattern(plan) in k for k in kernels), (plan['kernel'], kernels)
-        for b, (fmt, cams, frames, images) in enumerate(batches[group]):
-            want = e.backbone(e.preprocess(images), stop_layer=0, layer_shape=shape)[2]
-            for on_dev in (False, True):
-                assert np.array_equal(got[2 * b + on_dev], want), (fmt, list(cams.values()), on_dev)
-            key = (stem, group, b)
-            if key not in FP.REFS:
-                FP.REFS[key] = FP._stem_reference(m, images)
-            zs, P, yr, sc, of = FP.REFS[key]
-            bound = F.chain_bound(P, zs, yr, sc, of, L.kh * L.kw * 3)
-            err = np.abs(got[2 * b] - yr)
-            _record('frames:' + plan['kernel'], err, bound)
-            assert np.all(err <= bound), (fmt, list(cams.values()), float(np.max(err / bound)))
-            assert np.abs(yr).max() > 0
+    FP.test_stem_on_frames(batches, stem, FP16, group)
 
 
 # ------------------------------------------------------------------------------------------------ (3) frame path
@@ -287,10 +137,10 @@ def test_saturation(kind):
             if names:
                 break
         assert any(pattern in k for k in names), names
-        over = np.abs(exact) > F.FP16_MAX
-        assert np.array_equal(y[over], np.sign(exact[over]) * F.FP16_MAX)    # exactly ±65504, with the sign
+        over = np.abs(exact) > R.FP16_MAX
+        assert np.array_equal(y[over], np.sign(exact[over]) * R.FP16_MAX)    # exactly ±65504, with the sign
         assert np.any(y[over] > 0) and np.any(y[over] < 0)
-        assert np.array_equal(y, F.fp16_store(exact.astype(np.float32)))      # and the rest rounded as usual
+        assert np.array_equal(y, R.fp16_store(exact.astype(np.float32)))      # and the rest rounded as usual
         enc, lg, _ = e.backbone(pre)
         assert np.all(np.isfinite(enc)) and np.all(np.isfinite(lg))
         assert np.abs(enc).max() > 0
@@ -336,5 +186,5 @@ def test_configs2_layer_error_fp16_vs_bf16():
                     worst[precision] = max(worst[precision], float(np.abs(got - w).max()) / max(1.0, float(np.abs(w).max())))
     print('configs[2] worst per-layer error / range: bf16 %.3g, fp16 %.3g (ratio %.3g); largest |activation| %.4g'
           % (worst[PRECISION_BF16_TC], worst[FP16], worst[FP16] / worst[PRECISION_BF16_TC], peak))
-    assert peak < F.FP16_MAX, 'the fp32 oracle activations leave the fp16 range: the comparison would measure the clamp'
+    assert peak < R.FP16_MAX, 'the fp32 oracle activations leave the fp16 range: the comparison would measure the clamp'
     assert worst[FP16] <= worst[PRECISION_BF16_TC] / 4

@@ -26,7 +26,8 @@ from tests import workload
 from tests.artist import artist_frame
 from tests.conftest import PORCH_CONFIG, load_golden_frame
 from tests.gpu_util import new_rows, rows_bytes
-from tests.test_gpu_layer_kernels import NAMES, _kernels, build
+from tests.test_gpu_layer_kernels import _kernels, build, record
+from tests.test_gpu_layer_kernels import report  # noqa: F401  (the largest error / bound per family)
 from tests.yuv_emulation import cv2_rgb, random_frame
 from watsor_b200 import _lib
 from watsor_b200.detection.b200 import B200ObjectDetector
@@ -98,16 +99,6 @@ def batches():
 
 
 REFS = {}           # (stem, group, batch) -> float64 (z·s, P, y) of the stem on oracle.preprocess of the batch's images
-WORST = {}          # (kernel, precision) -> largest error / bound
-
-
-@pytest.fixture(scope='module', autouse=True)
-def report():
-    yield
-    if WORST:
-        print('\nstem on frames: largest error / bound per kernel and precision:')
-        for (k, p), r in sorted(WORST.items()):
-            print('  %-18s %-7s %.3g' % (k, NAMES[p], r))
 
 
 def _stem_model(name):
@@ -144,7 +135,7 @@ def _configure(e, cams):
 
 
 @pytest.mark.parametrize('group', GROUPS)
-@pytest.mark.parametrize('precision', [0, 2, 1], ids=lambda p: NAMES[p])
+@pytest.mark.parametrize('precision', [0, 2, 1], ids=lambda p: R.PRECISIONS[p].name)
 @pytest.mark.parametrize('stem', list(STEMS))
 def test_stem_on_frames(batches, stem, precision, group):
     import torch
@@ -152,7 +143,6 @@ def test_stem_on_frames(batches, stem, precision, group):
     m = _stem_model(stem)
     L = m.layers[0]
     shape = (L.out_h, L.out_w, L.out_c)
-    bf16 = precision == 1
     plan = R.plan(L, 1, precision, torch.cuda.get_device_properties(0).multi_processor_count)
     with Engine(m.to_blob(), device=0, max_batch=MAX_IMAGES, precision=precision) as e:
         runs = []
@@ -181,7 +171,7 @@ def test_stem_on_frames(batches, stem, precision, group):
             if len(kernels) == len(runs):
                 break
         assert len(kernels) == len(runs), kernels
-        assert all(R.kernel_name_pattern(plan, bf16) in k for k in kernels), (plan['kernel'], kernels)
+        assert all(R.kernel_name_pattern(plan, precision) in k for k in kernels), (plan['kernel'], kernels)
 
         for b, (fmt, cams, frames, images) in enumerate(batches[group]):
             # (1) the stage path on the same RGB images, as one batch of the same image count
@@ -194,11 +184,9 @@ def test_stem_on_frames(batches, stem, precision, group):
             if key not in REFS:
                 REFS[key] = _stem_reference(m, images)
             zs, P, yr, sc, of = REFS[key]
-            bound = R.chain_bound(P, zs, yr, sc, of, L.kh * L.kw * 3, bf16_out=bf16)
+            bound = R.chain_bound(P, zs, yr, sc, of, L.kh * L.kw * 3, precision)
             err = np.abs(got[2 * b] - yr)
-            ratio = float(np.max(err / bound))
-            wk = (plan['kernel'], precision)
-            WORST[wk] = max(WORST.get(wk, 0.0), ratio)
+            ratio = record('frames:' + plan['kernel'], precision, err, bound)
             assert np.all(err <= bound), (fmt, list(cams.values()), ratio)
             assert np.abs(yr).max() > 0
 
@@ -237,7 +225,7 @@ def _detect(det, frames, cams, **kw):
     return [rows_bytes(r) for r in rows], verd
 
 
-@pytest.mark.parametrize('precision', [0, 1, 2, 3], ids=lambda p: NAMES[p])
+@pytest.mark.parametrize('precision', [0, 1, 2, 3], ids=lambda p: R.PRECISIONS[p].name)
 @pytest.mark.parametrize('net', list(NETWORKS))
 def test_network_frames_equal_stage_path(request, net, precision):
     m, cams, frames, stale = NETWORKS[net](request)
@@ -290,7 +278,7 @@ SEQUENCE = [((640, 480), (640, 480), 'rgb24', False, 'l1'),
 
 
 @pytest.mark.parametrize('windowed', [False, True], ids=['frames', 'windows'])
-@pytest.mark.parametrize('precision', [2, 1], ids=lambda p: NAMES[p])
+@pytest.mark.parametrize('precision', [2, 1], ids=lambda p: R.PRECISIONS[p].name)
 def test_graph_replay_depends_only_on_its_key(precision, windowed):
     blob = workload.v2_coco_model().to_blob()
     os.environ['WB_NO_GRAPH'] = '1'

@@ -20,17 +20,17 @@ from watsor_b200.model import ACT_NONE, ACT_RELU6, OP_HEAD, Model, _Emitter
 
 pytestmark = pytest.mark.gpu
 
-Case = namedtuple('Case', 'name family spec n precisions claim env')
-NAMES = {0: 'fp32', 1: 'bf16', 2: 'tf32x3', 3: 'tf32x1'}
+Case = namedtuple('Case', 'name family spec n precisions claim env prepare')
 
 
-def case(name, family, spec, n, precisions, claim, env=()):
-    """claim: plan() entries the tested layer must show, per precision ('all', or 0 / 1 / 'tf32' for 2 and 3)."""
-    return Case(name, family, spec, n, tuple(precisions), claim, tuple(env))
+def case(name, family, spec, n, precisions, claim, env=(), prepare=None):
+    """claim: plan() entries the tested layer must show, per precision ('all', or 0 / 1 / 'tf32' for 2 and 3; fp16
+    runs bf16's plan and claims 1's).  prepare(m, L): rewrites the model's weights after build()."""
+    return Case(name, family, spec, n, tuple(precisions), claim, tuple(env), prepare)
 
 
 def claim_for(c, precision):
-    key = 'tf32' if precision in (2, 3) else precision
+    key = {2: 'tf32', 3: 'tf32', 4: 1}.get(precision, precision)
     return c.claim.get(key, c.claim.get('all', {}))
 
 
@@ -274,15 +274,19 @@ WORST = {}          # (family, precision) -> largest error / bound
 
 @pytest.fixture(scope='module', autouse=True)
 def report():
+    """At the end of each module that uses it (test_gpu_frame_path and test_gpu_fp16 import it), the largest error /
+    bound its tests recorded."""
     yield
-    print('\nlargest error / bound per family and precision:')
-    for (fam, p), r in sorted(WORST.items()):
-        print('  %-10s %-7s %.3g' % (fam, NAMES[p], r))
+    if WORST:
+        print('\nlargest error / bound per family and precision:')
+        for (fam, p), r in sorted(WORST.items()):
+            print('  %-18s %-7s %.3g' % (fam, R.PRECISIONS[p].name, r))
+        WORST.clear()
 
 
-def _record(c, precision, err, bound):
+def record(family, precision, err, bound):
     ratio = float(np.max(err / bound))
-    key = (c.family, precision)
+    key = (family, precision)
     WORST[key] = max(WORST.get(key, 0.0), ratio)
     return ratio
 
@@ -290,18 +294,25 @@ def _record(c, precision, err, bound):
 def _weights(m, L, precision, tc):
     K = L.kh * L.kw * L.in_c
     w = np.asarray(m.tensors[L.w_tensor], np.float32).reshape(K, L.n_pad)[:, :L.out_c]
-    if precision == 1 and tc:
-        w = R.bf16_round(w)             # the tensor-core weights are rounded to bf16 once on the host
+    if tc:
+        w = R.PRECISIONS[precision].tc_round(w)     # the tensor-core weights are rounded once on the host
     return w.astype(np.float64).reshape(L.kh, L.kw, L.in_c, L.out_c)
 
 
-PARAMS = [pytest.param(c, p, id='%s-%s' % (c.name, NAMES[p])) for c in CASES for p in c.precisions]
+PARAMS = [pytest.param(c, p, id='%s-%s' % (c.name, R.PRECISIONS[p].name)) for c in CASES for p in c.precisions]
 
 
 @pytest.mark.parametrize('c,precision', PARAMS)
 def test_layer_kernel(c, precision):
+    check_layer(c, precision)
+
+
+def check_layer(c, precision):
+    """Case c in a `precision` engine: the branch it claims, and its arithmetic against float64 (module docstring)."""
     m, li, inputs, (h, w) = build(c.spec, seed=len(c.name))
     L = m.layers[li]
+    if c.prepare:
+        c.prepare(m, L)
     sms = _sms()
     pre = np.random.default_rng(c.n).standard_normal((c.n, h, w, 3)).astype(np.float32)
     xs, (enc, lg, y), launches, kernels = _run(m, li, inputs, pre, precision, c.env)
@@ -319,16 +330,15 @@ def test_layer_kernel(c, precision):
     assert launches == sum(q['launches'] for q in plans), (launches, plans)
     names = [k for k, _ in kernels]
     assert len(names) == launches, names
-    bf16 = precision == 1
     last = len(kernels) - 1
     if pair and not p.get('fused_add', False):
         assert 'k_add<' in names[last], names
         last -= 1
     if p['kernel'] == 'k_gemm_cc' and p['splits'] > 1:
-        assert 'k_splitk_reduce' in names[last], names
+        assert 'k_splitk_reduce<%s>' % R.PRECISIONS[precision].storage in names[last], names
         last -= 1
     tested = kernels[last]
-    assert R.kernel_name_pattern(p, bf16) in tested[0], (tested, p, names)
+    assert R.kernel_name_pattern(p, precision) in tested[0], (tested, p, names)
     if p['kernel'] == 'k_gemm_tc' and tested[1] is not None:
         assert tested[1][2] == p['splits'], (tested, p)
 
@@ -337,12 +347,12 @@ def test_layer_kernel(c, precision):
     f64 = [np.asarray(x, np.float64) for x in xs]
     if kind in ('pool', 'add', 'concat'):
         if kind == 'pool':
-            want_y = R.pool_f32(xs[0], L.kh, L.stride, c.spec[5], bf16)
+            want_y = R.pool_f32(xs[0], L.kh, L.stride, c.spec[5], precision)
         elif kind == 'add':
-            want_y = R.add_f32(xs[0], xs[1], bf16)
+            want_y = R.add_f32(xs[0], xs[1], precision)
         else:
             cl = [m.layers[i] for i in range(li - 2, li + 1)]
-            want_y = R.copy_channels_f32(xs, [q.row_off for q in cl], L.out_c, bf16)
+            want_y = R.copy_channels_f32(xs, [q.row_off for q in cl], L.out_c, precision)
         assert np.array_equal(y, want_y)
         assert np.abs(y).max() > 0
         return
@@ -353,18 +363,18 @@ def test_layer_kernel(c, precision):
         wt = _weights(m, L, precision, False)
         z, P = R.conv2d(a, wt, L.stride), R.conv2d(np.abs(a), np.abs(wt), L.stride)
         yr = R.affine(z, sc, of, L.act)
-        bound = R.chain_bound(P, z * sc, yr, sc, of, L.kh * L.kw * 3, bf16_out=bf16)
+        bound = R.chain_bound(P, z * sc, yr, sc, of, L.kh * L.kw * 3, precision)
         err = np.abs(y - yr)
-        _record(c, precision, err, bound)
+        record(c.family, precision, err, bound)
         assert np.all(err <= bound)
         return
     if kind == 'dw':
         wt = np.asarray(m.tensors[L.w_tensor], np.float64).reshape(3, 3, L.out_c)
         z, P = R.depthwise(f64[0], wt, L.stride), R.depthwise(np.abs(f64[0]), np.abs(wt), L.stride)
         yr = R.affine(z, sc, of, L.act)
-        bound = R.chain_bound(P, z * sc, yr, sc, of, 9, bf16_out=bf16)
+        bound = R.chain_bound(P, z * sc, yr, sc, of, 9, precision)
         err = np.abs(y - yr)
-        _record(c, precision, err, bound)
+        record(c.family, precision, err, bound)
         assert np.all(err <= bound)
         return
     G = m.layers[li - 1] if kind == 'pw_add' else L           # the GEMM layer
@@ -377,18 +387,15 @@ def test_layer_kernel(c, precision):
     yr = R.affine(z, sc, of, G.act)
     K = G.kh * G.kw * G.in_c
 
-    def bound_for(mode, q):
-        is_head = G.op == OP_HEAD
-        if mode == 0:
-            return R.dense_bound(P, z * sc, yr, sc, of, 0, K=K, splits=q['splits'], bf16_out=bf16 and not is_head)
-        return R.dense_bound(P, z * sc, yr, sc, of, mode, k_blocks=q['k_blocks'], splits=q['splits'],
-                             kb_per=q['kb_per'], bf16_out=bf16 and not is_head)
+    def bound_for(bp, q):
+        """the bound of the layer's kernel in a `bp` engine (2: the tf32x3 bar)"""
+        return R.dense_bound(P, z * sc, yr, sc, of, bp, k_blocks=q.get('k_blocks', 1), splits=q['splits'],
+                             kb_per=q.get('kb_per'), K=K, tc=tc, head=G.op == OP_HEAD)
 
-    mode = precision if tc else 0
     if G.op == OP_HEAD:
         # every head of the model, scattered into the whole enc / logits arrays: a row written twice or not at all fails
         ref = [np.zeros(enc.shape), np.zeros(lg.shape)]
-        bnd = {md: [np.zeros(enc.shape), np.zeros(lg.shape)] for md in {mode, 2 if tc else mode}}
+        bnd = {bp: [np.zeros(enc.shape), np.zeros(lg.shape)] for bp in {precision, 2 if tc else precision}}
         for hl in (q for q in m.layers if q.op == OP_HEAD):
             hw_t = _weights(m, hl, precision, tc)
             sc = np.asarray(m.tensors[hl.scale_tensor], np.float64)[:hl.out_c]
@@ -397,21 +404,21 @@ def test_layer_kernel(c, precision):
             yr = R.affine(z, sc, of, hl.act)
             hq = R.plan(hl, c.n, precision, sms, c.env)
             R.head_scatter(yr, hl.anchors_per_loc, hl.n_box, hl.row_off, *ref)
-            for md, arrs in bnd.items():
-                R.head_scatter(bound_for(md, hq), hl.anchors_per_loc, hl.n_box, hl.row_off, *arrs)
+            for bp, arrs in bnd.items():
+                R.head_scatter(bound_for(bp, hq), hl.anchors_per_loc, hl.n_box, hl.row_off, *arrs)
         err = np.concatenate([np.abs(enc - ref[0]).ravel(), np.abs(lg - ref[1]).ravel()])
         yr = np.concatenate([r.ravel() for r in ref])
-        bound, bound3 = (np.concatenate([b.ravel() for b in bnd[md]]) for md in (mode, 2 if tc else mode))
+        bound, bound3 = (np.concatenate([b.ravel() for b in bnd[bp]]) for bp in (precision, 2 if tc else precision))
     else:
         err = np.abs(y - yr)
-        bound = bound_for(mode, gp)
+        bound = bound_for(precision, gp)
         bound3 = bound_for(2, gp) if tc else None
     if kind == 'pw_add':
         # Add(x, p): one more fp32 rounding, fused or not
         yr = yr + f64[0]
         err = np.abs(y - yr)
         bound, bound3 = (None if b is None else b + R.U * (np.abs(yr) + b) for b in (bound, bound3))
-    ratio = _record(c, precision, err, bound)
+    ratio = record(c.family, precision, err, bound)
     assert np.all(err <= bound), (ratio, float(err.max()))
     assert np.abs(yr).max() > 0
     if precision == 3 and K >= 256:

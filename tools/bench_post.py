@@ -28,9 +28,9 @@ from tests import workload  # noqa: E402
 from tests.artist import artist_frame  # noqa: E402
 from tools.bench_yuv import card  # noqa: E402
 from watsor_b200.detection.b200 import B200ObjectDetector  # noqa: E402
-from watsor_b200.engine import PRECISION_BF16_TC, PRECISION_FP16_TC, PRECISION_TF32X3  # noqa: E402
+from watsor_b200.engine import PRECISIONS  # noqa: E402
 
-MODES = {'fp32': 0, 'bf16': PRECISION_BF16_TC, 'fp16': PRECISION_FP16_TC, 'tf32x3': PRECISION_TF32X3}
+MODES = {m: PRECISIONS[m] for m in ('fp32', 'bf16', 'fp16', 'tf32x3')}
 CAMS, W, H, RING, SLOTS = 8, 640, 480, 8, 6
 POST_KERNELS = ('k_decode_scores', 'k_nms', 'k_merge_filter')
 

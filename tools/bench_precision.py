@@ -31,10 +31,10 @@ from tests.artist import artist_frame  # noqa: E402
 from tests.gpu_util import new_rows, rows_to_tuples  # noqa: E402
 from tools.bench_yuv import card  # noqa: E402
 from watsor_b200.detection.b200 import B200ObjectDetector  # noqa: E402
-from watsor_b200.engine import PRECISION_BF16_TC, PRECISION_FP16_TC, PRECISION_TF32X3  # noqa: E402
+from watsor_b200.engine import PRECISIONS  # noqa: E402
 from watsor_b200.model import OP_HEAD  # noqa: E402
 
-MODES = {'bf16': PRECISION_BF16_TC, 'fp16': PRECISION_FP16_TC, 'tf32x3': PRECISION_TF32X3}
+MODES = {m: PRECISIONS[m] for m in ('bf16', 'fp16', 'tf32x3')}
 CAMS, W, H, RING = 8, 640, 480, 4
 
 

@@ -586,22 +586,19 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
     cfg.numAttrs = g.splits > 1 ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, map_a, map_b, map_b_lo, g);
   };
-  static PerDeviceFlag attr_done[4][3];
-  const int bi = g.block_n == 32 ? 0 : (g.block_n == 64 ? 1 : 2);
-  cudaError_t e;
-  if (mode == TC_BF16) {
-    e = bi == 0 ? launch(k_gemm_tc<0, 32>, attr_done[0][0])
-                : (bi == 1 ? launch(k_gemm_tc<0, 64>, attr_done[0][1]) : launch(k_gemm_tc<0, 128>, attr_done[0][2]));
-  } else if (mode == TC_FP16) {
-    e = bi == 0 ? launch(k_gemm_tc<3, 32>, attr_done[3][0])
-                : (bi == 1 ? launch(k_gemm_tc<3, 64>, attr_done[3][1]) : launch(k_gemm_tc<3, 128>, attr_done[3][2]));
-  } else if (mode == TC_TF32X1) {
-    e = bi == 0 ? launch(k_gemm_tc<1, 32>, attr_done[1][0])
-                : (bi == 1 ? launch(k_gemm_tc<1, 64>, attr_done[1][1]) : launch(k_gemm_tc<1, 128>, attr_done[1][2]));
-  } else {
-    e = bi == 0 ? launch(k_gemm_tc<2, 32>, attr_done[2][0])
-                : (bi == 1 ? launch(k_gemm_tc<2, 64>, attr_done[2][1]) : launch(k_gemm_tc<2, 128>, attr_done[2][2]));
-  }
+  // the instantiations by [TcMode][block_n 32 / 64 / 128]
+  struct Instance {
+    void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, TcArgs);
+    PerDeviceFlag attr_done;
+  };
+  static Instance instances[4][3] = {
+      {{k_gemm_tc<TC_BF16, 32>}, {k_gemm_tc<TC_BF16, 64>}, {k_gemm_tc<TC_BF16, 128>}},
+      {{k_gemm_tc<TC_TF32X1, 32>}, {k_gemm_tc<TC_TF32X1, 64>}, {k_gemm_tc<TC_TF32X1, 128>}},
+      {{k_gemm_tc<TC_TF32X3, 32>}, {k_gemm_tc<TC_TF32X3, 64>}, {k_gemm_tc<TC_TF32X3, 128>}},
+      {{k_gemm_tc<TC_FP16, 32>}, {k_gemm_tc<TC_FP16, 64>}, {k_gemm_tc<TC_FP16, 128>}},
+  };
+  Instance& k = instances[mode][g.block_n == 32 ? 0 : (g.block_n == 64 ? 1 : 2)];
+  const cudaError_t e = launch(k.kern, k.attr_done);
   if (e != cudaSuccess) {
     *err = std::string("tensor-core GEMM launch: ") + cudaGetErrorString(e);
     return 1;

@@ -68,6 +68,22 @@ static cudaError_t alloc(Owned<T*, Release>& b, size_t bytes) {
 static cudaError_t create(Stream& s) { return cudaStreamCreateWithFlags(&s.h, cudaStreamNonBlocking); }
 static cudaError_t create(Event& e) { return cudaEventCreate(&e.h); }
 
+// The precision modes, indexed by wb_create's `precision` (include/watsor_b200.h).  Every precision-dependent choice of
+// the executor reads the mode's row: the activation storage type and the tensor-core GEMMs' operand mode.
+enum class Storage { F32, BF16, F16 };
+struct PrecisionMode {
+  const char* name;  // wb_device_name
+  Storage storage;   // activations in the arena
+  int tc_mode;       // TcMode of the dense layers that the tensor-core GEMM takes, or -1: CUDA cores only
+};
+static const PrecisionMode PRECISIONS[] = {
+    {"fp32", Storage::F32, -1},
+    {"bf16 wgmma", Storage::BF16, TC_BF16},
+    {"fp32 3xTF32 wgmma", Storage::F32, TC_TF32X3},
+    {"tf32 wgmma", Storage::F32, TC_TF32X1},
+    {"fp16 wgmma", Storage::F16, TC_FP16},
+};
+
 struct Slot {
   Stream stream;
   Event ev0, ev1;
@@ -109,7 +125,7 @@ struct Slot {
 struct wb_ctx {
   int device = 0;
   int max_batch = 0;
-  int precision = 0;
+  int precision = 0;  // index into PRECISIONS
   // path switches (INTEGRATION.md §4), read from the environment once, in wb_create: an engine keeps the paths it was
   // created with, and routes to the tensor cores exactly the layers whose weights it prepared for them
   struct {
@@ -125,7 +141,7 @@ struct wb_ctx {
   std::vector<wb_layer> layers;
   std::vector<wb_tensor_entry> tensors;
   DevBuf<float> d_weights;
-  TcWeights tc;  // the GEMM weights in the tensor cores' operand format (precision != 0)
+  TcWeights tc;  // the GEMM weights in the tensor cores' operand format (modes with a tc_mode)
   PostParams pp;
   DevBuf<CameraCfg> d_cams;
   std::vector<CameraCfg> h_cams;
@@ -157,12 +173,11 @@ struct wb_ctx {
   PinnedBuf<int> h_raw_num;
 
   const float* tensor(int idx) const { return d_weights + tensors[idx].offset; }
-  // the 16-bit activation modes: 1 (bf16), 4 (fp16)
-  bool half_acts() const { return precision == 1 || precision == 4; }
-  size_t elem_size() const { return half_acts() ? 2 : 4; }
+  const PrecisionMode& mode() const { return PRECISIONS[precision]; }
+  size_t elem_size() const { return mode().storage == Storage::F32 ? 4 : 2; }
   cudaStream_t stream_of(int s) { return has_user_stream ? user_stream : slots[s].stream; }
   // whether layer L runs on the tensor-core GEMM
-  bool tc_runs(const wb_layer& L) const { return precision != 0 && tc_layer_supported(L, tc.mode, sw.tc_conv); }
+  bool tc_runs(const wb_layer& L) const { return mode().tc_mode >= 0 && tc_layer_supported(L, tc.mode, sw.tc_conv); }
 };
 
 extern "C" {
@@ -216,7 +231,7 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   REQUIRE(out != nullptr && model_blob != nullptr, "NULL argument");
   REQUIRE(blob_bytes >= sizeof(wb_model_header), "model blob too small");
   REQUIRE(max_batch >= 1 && max_batch <= 4096, "max_batch out of range");
-  REQUIRE(precision >= 0 && precision <= 4,
+  REQUIRE(precision >= 0 && precision < (int)std::size(PRECISIONS),
           "precision must be 0 (fp32 CUDA cores), 1 (bf16 wgmma), 2 (fp32 via 3xTF32 wgmma), 3 (1xTF32, diagnostic) or "
           "4 (fp16 wgmma)");
   CK(cudaSetDevice(device));
@@ -277,10 +292,10 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   }
   CK(alloc(c->d_weights, floats * sizeof(float)));
   CK(cudaMemcpy(c->d_weights, p, floats * sizeof(float), cudaMemcpyHostToDevice));
-  if (precision != 0) {
+  if (c->mode().tc_mode >= 0) {
     std::string err;
-    const int mode = precision == 1 ? TC_BF16 : (precision == 2 ? TC_TF32X3 : (precision == 4 ? TC_FP16 : TC_TF32X1));
-    if (tc_prepare_weights(c->layers, c->tensors, reinterpret_cast<const float*>(p), mode, c->sw.tc_conv, &c->tc, &err))
+    if (tc_prepare_weights(c->layers, c->tensors, reinterpret_cast<const float*>(p), c->mode().tc_mode, c->sw.tc_conv,
+                           &c->tc, &err))
       return fail("tensor-core weight preparation: " + err);
   }
   c->pp.num_anchors = c->hdr.num_anchors;
@@ -330,11 +345,7 @@ int wb_destroy(wb_ctx* c) {
 int wb_device_name(wb_ctx* c, char* buf, size_t n) {
   REQUIRE(c && buf && n > 0, "NULL argument");
   snprintf(buf, n, "%s (cuda:%d, sm_%d%d, %s)", c->prop.name, c->device, c->prop.major, c->prop.minor,
-           c->precision == 1   ? "bf16 wgmma"
-           : c->precision == 2 ? "fp32 3xTF32 wgmma"
-           : c->precision == 3 ? "tf32 wgmma"
-           : c->precision == 4 ? "fp16 wgmma"
-                               : "fp32");
+           c->mode().name);
   return 0;
 }
 
@@ -493,9 +504,10 @@ static bool arena_disjoint(const wb_layer& reader, const wb_layer& writer) {
 static Span fused_span(const wb_ctx* c, size_t li, size_t end) {
   const std::vector<wb_layer>& Ls = c->layers;
   const wb_layer& L = Ls[li];
-  // layer p + 1 is `Add(shortcut, output of p)` (fp32 modes: the shortcut can be added in an fp32 epilogue)
+  // layer p + 1 is `Add(shortcut, output of p)` (tensor-core modes with fp32 storage: the shortcut can be added in an
+  // fp32 epilogue)
   auto residual_add_after = [&](size_t p) {
-    if (c->precision == 0 || c->half_acts() || p + 1 >= end || !c->sw.fuse_add) return false;
+    if (c->mode().tc_mode < 0 || c->mode().storage != Storage::F32 || p + 1 >= end || !c->sw.fuse_add) return false;
     const wb_layer& P = Ls[p], &A = Ls[p + 1];
     return P.op == WB_OP_PW && P.act == WB_ACT_NONE && A.op == WB_OP_ADD &&
            (A.in_off == P.out_off || A.in2_off == P.out_off) && A.in_off != A.in2_off;
@@ -507,7 +519,7 @@ static Span fused_span(const wb_ctx* c, size_t li, size_t end) {
     if (kind == SPAN_DW_PW_ADD || kind == SPAN_PW_ADD) residual_off = A.in_off == Ls[last - 1].out_off ? A.in2_off : A.in_off;
     return Span{last, kind, A.out_off, residual_off};
   };
-  if (L.op == WB_OP_DW && c->precision == 2 && li + 1 < end && c->sw.fuse_dwpw) {
+  if (L.op == WB_OP_DW && li + 1 < end && c->sw.fuse_dwpw) {
     const wb_layer& P = Ls[li + 1];
     if (P.in_off == L.out_off && fused_dwpw_supported(c->tc, (int)li + 1, L, P)) {
       if (residual_add_after(li + 1)) {
@@ -617,8 +629,8 @@ static int run_post(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, 
 
 // layers first..last (last < 0: to the end) in the engine's activation type
 static int run_program(wb_ctx* c, Slot& s, cudaStream_t st, int n, const float* pre, int first, int last) {
-  if (c->precision == 1) return run_layers<__nv_bfloat16>(c, s, st, n, pre, first, last);
-  if (c->precision == 4) return run_layers<__half>(c, s, st, n, pre, first, last);
+  if (c->mode().storage == Storage::BF16) return run_layers<__nv_bfloat16>(c, s, st, n, pre, first, last);
+  if (c->mode().storage == Storage::F16) return run_layers<__half>(c, s, st, n, pre, first, last);
   return run_layers<float>(c, s, st, n, pre, first, last);
 }
 
@@ -922,12 +934,12 @@ static int copy_backbone_out(wb_ctx* c, Slot& s, cudaStream_t st, int n, float* 
   REQUIRE(L.op != WB_OP_HEAD, "head layers have no activation output");
   size_t elems = (size_t)n * L.out_h * L.out_w * L.out_c;
   REQUIRE(layer_out_floats >= elems, "layer_out too small");
-  if (c->elem_size() == 4) {
+  if (c->mode().storage == Storage::F32) {
     CK(cudaMemcpy(layer_out, static_cast<float*>(s.arena.h) + (size_t)L.out_off * n, elems * 4, cudaMemcpyDeviceToHost));
   } else {
     std::vector<uint16_t> tmp(elems);
     CK(cudaMemcpy(tmp.data(), static_cast<uint16_t*>(s.arena.h) + (size_t)L.out_off * n, elems * 2, cudaMemcpyDeviceToHost));
-    if (c->precision == 4) {
+    if (c->mode().storage == Storage::F16) {
       for (size_t i = 0; i < elems; ++i) {
         __half h;
         memcpy(&h, &tmp[i], 2);

@@ -18,7 +18,7 @@ import os
 import numpy as np
 
 from .. import _lib
-from ..engine import PRECISION_BF16_TC, PRECISION_FP16_TC, PRECISION_FP32, PRECISION_TF32X3, Engine
+from ..engine import PRECISION_BF16_TC, PRECISION_FP16_TC, PRECISION_FP32, PRECISION_TF32X3, PRECISIONS, Engine
 from ..model import Model, compile_frozen_graph
 from ..stream.share import MAX_DETECTIONS, Detection
 
@@ -51,12 +51,12 @@ def load_model_blob(model_path):
 
 
 def default_precision():
-    """`WATSOR_B200_PRECISION=fp32|tf32x3|bf16|fp16` (the reference's analogous switch is
+    """`WATSOR_B200_PRECISION=fp32|tf32x3|bf16|fp16` (or the diagnostic `tf32x1`; the reference's analogous switch is
     TRT_FLOAT_PRECISION, main_for_gpu.py:24).  Default: fp32-faithful tensor-core mode.  `16` selects bf16, as it
     always has; IEEE half is `fp16` (or `half`)."""
     v = os.environ.get('WATSOR_B200_PRECISION', 'tf32x3').lower()
-    return {'fp32': PRECISION_FP32, '32': PRECISION_FP32, 'bf16': PRECISION_BF16_TC, '16': PRECISION_BF16_TC,
-            'fp16': PRECISION_FP16_TC, 'half': PRECISION_FP16_TC, 'tf32x3': PRECISION_TF32X3}.get(v, PRECISION_TF32X3)
+    aliases = {'32': PRECISION_FP32, '16': PRECISION_BF16_TC, 'half': PRECISION_FP16_TC}
+    return {**PRECISIONS, **aliases}.get(v, PRECISION_TF32X3)
 
 
 class B200ObjectDetector(object):

@@ -13,9 +13,11 @@ from ._lib import ClassFilter, check
 from .windows import check_windows
 from .stream.share import MAX_DETECTIONS, Detection
 
-# 0: fp32 CUDA-core convs; 1: bf16 wgmma; 2: fp32 storage, dense convs as 3xTF32 wgmma (fp32-faithful);
-# 4: fp16 wgmma, activations saturated at +-65504 (include/watsor_b200.h, wb_create)
-PRECISION_FP32, PRECISION_BF16_TC, PRECISION_TF32X3, PRECISION_FP16_TC = 0, 1, 2, 4
+# wb_create's precision by name (include/watsor_b200.h): fp32 CUDA-core convs; bf16 wgmma; fp32 storage with the dense
+# convs as 3xTF32 wgmma (fp32-faithful); 1xTF32 wgmma (diagnostic); fp16 wgmma, activations saturated at +-65504
+PRECISIONS = {'fp32': 0, 'bf16': 1, 'tf32x3': 2, 'tf32x1': 3, 'fp16': 4}
+PRECISION_FP32, PRECISION_BF16_TC = PRECISIONS['fp32'], PRECISIONS['bf16']
+PRECISION_TF32X3, PRECISION_FP16_TC = PRECISIONS['tf32x3'], PRECISIONS['fp16']
 
 # frame layouts the hot path reads, by ffmpeg's -pix_fmt names -> wb_detect / wb_submit flag
 PIXEL_FORMATS = {'rgb24': 0, 'yuv420p': _lib.WB_F_YUV420P, 'nv12': _lib.WB_F_NV12}
