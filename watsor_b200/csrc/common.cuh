@@ -130,6 +130,16 @@ struct PerDeviceFlag {
   void set() { done[dev()] = true; }
 };
 
+// lets `kern` use up to `bytes` of dynamic shared memory on the current device; `done` remembers a success, so that
+// only the first launch on a device pays for the call and a failed call is made again by the next launch
+template <typename Kernel>
+cudaError_t max_dynamic_smem_once(Kernel kern, int bytes, PerDeviceFlag& done) {
+  if (done.get()) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) done.set();
+  return e;
+}
+
 struct LaunchCtx {
   cudaStream_t stream;
   int* launch_counter;  // host-side counter of kernel launches (bench: gpu_launches)

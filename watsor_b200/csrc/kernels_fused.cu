@@ -373,11 +373,7 @@ int fused_launch_dwpw(const LaunchCtx& lc, const TcWeights& tw, int pw_layer_ind
   const long tiles = (long)p.tiles_x * p.tiles_y * n;
   const dim3 grid((unsigned)std::min<long>(tiles, ctas));
   auto launch = [&](auto kern, PerDeviceFlag& done) {
-    if (!done.get()) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      if (e != cudaSuccess) return e;
-      done.set();
-    }
+    if (cudaError_t e = max_dynamic_smem_once(kern, 227 * 1024, done)) return e;
     kern<<<grid, F_THREADS, p.smem, lc.stream>>>(map_in, map_b, map_b_lo, g);
     return cudaGetLastError();
   };

@@ -26,12 +26,14 @@
 #include <vector>
 
 #include "../../include/watsor_b200.h"
+#include "host.cuh"
 #include "yuv420.cuh"
 
 namespace {
 
+// wb_fx_last_error's message, kept apart from wb_last_error's
 thread_local std::string g_fx_err;
-int fx_fail(const std::string& m) {
+int fail(const std::string& m) {
   g_fx_err = m;
   return 1;
 }
@@ -72,6 +74,13 @@ struct FxCamera {
   int32_t w, h;
   const uint8_t* alpha;      // [h][w] or nullptr
   const uint32_t* contours;  // [h][w] or nullptr
+};
+
+// a camera of wb_fx_set_camera: the view the kernels receive, and the rasters it points to
+struct FxCameraEntry {
+  FxCamera view{};
+  DevBuf<uint8_t> alpha;
+  DevBuf<uint32_t> contours;
 };
 
 struct FxFrameDesc {
@@ -415,70 +424,58 @@ __global__ void __launch_bounds__(256, 5)
 struct wb_fx {
   int device = 0;
   std::mutex mu;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  Stream stream;
+  Event ev0, ev1;
   FxFont font{};
-  int32_t* d_advance = nullptr;
-  uint8_t* d_lut = nullptr;
-  FxLabel* d_labels = nullptr;
+  DevBuf<int32_t> d_advance;
+  DevBuf<uint8_t> d_lut;
+  DevBuf<FxLabel> d_labels;
   int n_labels = 0;
-  uint8_t* d_digits = nullptr;
-  uint8_t* d_aw = nullptr;
-  std::map<int, FxCamera> cams;
-  std::vector<void*> cam_allocs;
+  DevBuf<uint8_t> d_digits;
+  DevBuf<uint8_t> d_aw;
+  std::map<int, FxCameraEntry> cams;
   // staging
   int cap_n = 0;
   size_t cap_bytes = 0;
-  uint8_t *d_in = nullptr, *d_out = nullptr;
-  wb_detection* d_rows = nullptr;
-  wb_detection* h_rows = nullptr;
-  FxFrameDesc* d_desc = nullptr;
-  FxFrameDesc* h_desc = nullptr;
-  FxFrame* d_prep = nullptr;
+  DevBuf<uint8_t> d_in, d_out;
+  DevBuf<wb_detection> d_rows;
+  PinnedBuf<wb_detection> h_rows;
+  DevBuf<FxFrameDesc> d_desc;
+  PinnedBuf<FxFrameDesc> h_desc;
+  DevBuf<FxFrame> d_prep;
 };
-
-#define FXCK(call)                                                                                       \
-  do {                                                                                                   \
-    cudaError_t e_ = (call);                                                                             \
-    if (e_ != cudaSuccess)                                                                               \
-      return fx_fail(std::string(#call) + ": " + cudaGetErrorString(e_) + " (" + __FILE__ + ":" +        \
-                     std::to_string(__LINE__) + ")");                                                    \
-  } while (0)
-#define FXREQ(cond, msg) \
-  do {                   \
-    if (!(cond)) return fx_fail(msg); \
-  } while (0)
 
 const char* wb_fx_last_error(void) { return g_fx_err.c_str(); }
 
 int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_label* labels, const uint8_t* digit_glyphs,
                  double alpha, wb_fx** out) {
-  FXREQ(font && labels && digit_glyphs && out, "NULL argument");
-  FXREQ(font->n_glyphs > 0 && font->n_glyphs <= 128 && font->rows > 0 && font->cols > 0 && font->cols <= 64,
-        "bad font geometry");
-  FXREQ(n_labels > 0 && n_labels <= 256, "n_labels must be in 1..256");
+  REQUIRE(font && labels && digit_glyphs && out, "NULL argument");
+  REQUIRE(font->n_glyphs > 0 && font->n_glyphs <= 128 && font->rows > 0 && font->cols > 0 && font->cols <= 64,
+          "bad font geometry");
+  REQUIRE(n_labels > 0 && n_labels <= 256, "n_labels must be in 1..256");
   for (int i = 0; i < n_labels; ++i) {
-    FXREQ(labels[i].n_prefix <= sizeof(labels[i].prefix), "label prefix too long");
-    for (int j = 0; j < labels[i].n_prefix; ++j) FXREQ(labels[i].prefix[j] < font->n_glyphs, "glyph index out of range");
+    REQUIRE(labels[i].n_prefix <= sizeof(labels[i].prefix), "label prefix too long");
+    for (int j = 0; j < labels[i].n_prefix; ++j) REQUIRE(labels[i].prefix[j] < font->n_glyphs, "glyph index out of range");
   }
-  for (int i = 0; i < 11; ++i) FXREQ(digit_glyphs[i] < font->n_glyphs, "digit glyph index out of range");
+  for (int i = 0; i < 11; ++i) REQUIRE(digit_glyphs[i] < font->n_glyphs, "digit glyph index out of range");
   int count = 0;
-  FXCK(cudaGetDeviceCount(&count));
-  FXREQ(device >= 0 && device < count, "no such CUDA device");
-  FXCK(cudaSetDevice(device));
+  CK(cudaGetDeviceCount(&count));
+  REQUIRE(device >= 0 && device < count, "no such CUDA device");
+  CK(cudaSetDevice(device));
   cudaDeviceProp prop;
-  FXCK(cudaGetDeviceProperties(&prop, device));
-  FXREQ(prop.major == 9 && prop.minor == 0, "libwatsor_b200 is built for sm_90a (H100) only");
-  std::unique_ptr<wb_fx> fx(new wb_fx());
+  CK(cudaGetDeviceProperties(&prop, device));
+  const std::string unsupported = unsupported_device(prop);
+  REQUIRE(unsupported.empty(), unsupported);
+  std::unique_ptr<wb_fx> fx(new wb_fx());  // every REQUIRE / CK early return below releases what it holds
   fx->device = device;
-  FXCK(cudaStreamCreateWithFlags(&fx->stream, cudaStreamNonBlocking));
-  FXCK(cudaEventCreate(&fx->ev0));
-  FXCK(cudaEventCreate(&fx->ev1));
+  CK(create(fx->stream));
+  CK(create(fx->ev0));
+  CK(create(fx->ev1));
   const size_t lut_bytes = (size_t)font->n_glyphs * 2 * (font->cols + 1) * font->rows * font->cols * 256;
-  FXCK(cudaMalloc(&fx->d_advance, sizeof(int32_t) * font->n_glyphs));
-  FXCK(cudaMalloc(&fx->d_lut, lut_bytes));
-  FXCK(cudaMemcpy(fx->d_advance, font->advance, sizeof(int32_t) * font->n_glyphs, cudaMemcpyHostToDevice));
-  FXCK(cudaMemcpy(fx->d_lut, font->lut, lut_bytes, cudaMemcpyHostToDevice));
+  CK(alloc(fx->d_advance, sizeof(int32_t) * font->n_glyphs));
+  CK(alloc(fx->d_lut, lut_bytes));
+  CK(cudaMemcpy(fx->d_advance, font->advance, sizeof(int32_t) * font->n_glyphs, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(fx->d_lut, font->lut, lut_bytes, cudaMemcpyHostToDevice));
   fx->font.n_glyphs = font->n_glyphs;
   fx->font.rows = font->rows;
   fx->font.cols = font->cols;
@@ -490,10 +487,10 @@ int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_l
   fx->font.lut = fx->d_lut;
   static_assert(sizeof(FxLabel) == sizeof(wb_fx_label), "label style layout");
   fx->n_labels = n_labels;
-  FXCK(cudaMalloc(&fx->d_labels, sizeof(FxLabel) * n_labels));
-  FXCK(cudaMemcpy(fx->d_labels, labels, sizeof(FxLabel) * n_labels, cudaMemcpyHostToDevice));
-  FXCK(cudaMalloc(&fx->d_digits, 16));
-  FXCK(cudaMemcpy(fx->d_digits, digit_glyphs, 11, cudaMemcpyHostToDevice));
+  CK(alloc(fx->d_labels, sizeof(FxLabel) * n_labels));
+  CK(cudaMemcpy(fx->d_labels, labels, sizeof(FxLabel) * n_labels, cudaMemcpyHostToDevice));
+  CK(alloc(fx->d_digits, 16));
+  CK(cudaMemcpy(fx->d_digits, digit_glyphs, 11, cudaMemcpyHostToDevice));
   // cv2.addWeighted(src1, alpha, src2, beta = 1 - alpha, 0) on 8-bit images:  saturate(rint(fmaf(a, alpha, b * beta)))
   // in float -- pinned against OpenCV on all 256 x 256 inputs (tests/test_effects_host.py)
   std::vector<uint8_t> aw((size_t)n_labels * 768);
@@ -505,97 +502,89 @@ int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_l
         const float r = nearbyintf(fmaf((float)a, fa, t));
         aw[(size_t)l * 768 + c * 256 + a] = (uint8_t)(r < 0.f ? 0.f : (r > 255.f ? 255.f : r));
       }
-  FXCK(cudaMalloc(&fx->d_aw, aw.size()));
-  FXCK(cudaMemcpy(fx->d_aw, aw.data(), aw.size(), cudaMemcpyHostToDevice));
+  CK(alloc(fx->d_aw, aw.size()));
+  CK(cudaMemcpy(fx->d_aw, aw.data(), aw.size(), cudaMemcpyHostToDevice));
   *out = fx.release();
   return 0;
 }
 
 int wb_fx_set_camera(wb_fx* fx, int cam_id, int width, int height, const uint8_t* alpha, const uint32_t* contour_bits) {
-  FXREQ(fx, "NULL fx");
-  FXREQ(width > 0 && height > 0, "bad frame size");
+  REQUIRE(fx, "NULL fx");
+  REQUIRE(width > 0 && height > 0, "bad frame size");
   std::lock_guard<std::mutex> lock(fx->mu);
-  FXCK(cudaSetDevice(fx->device));
-  FXCK(cudaStreamSynchronize(fx->stream));
-  FxCamera cam{width, height, nullptr, nullptr};
+  CK(cudaSetDevice(fx->device));
+  CK(cudaStreamSynchronize(fx->stream));
+  FxCameraEntry cam;
+  cam.view = FxCamera{width, height, nullptr, nullptr};
   const size_t px = (size_t)width * height;
   if (alpha) {
-    uint8_t* d = nullptr;
-    FXCK(cudaMalloc(&d, px));
-    FXCK(cudaMemcpy(d, alpha, px, cudaMemcpyHostToDevice));
-    fx->cam_allocs.push_back(d);
-    cam.alpha = d;
+    CK(alloc(cam.alpha, px));
+    CK(cudaMemcpy(cam.alpha, alpha, px, cudaMemcpyHostToDevice));
+    cam.view.alpha = cam.alpha;
   }
   if (contour_bits) {
-    uint32_t* d = nullptr;
-    FXCK(cudaMalloc(&d, px * 4));
-    FXCK(cudaMemcpy(d, contour_bits, px * 4, cudaMemcpyHostToDevice));
-    fx->cam_allocs.push_back(d);
-    cam.contours = d;
+    CK(alloc(cam.contours, px * 4));
+    CK(cudaMemcpy(cam.contours, contour_bits, px * 4, cudaMemcpyHostToDevice));
+    cam.view.contours = cam.contours;
   }
-  fx->cams[cam_id] = cam;
+  fx->cams[cam_id] = std::move(cam);  // an earlier configuration's rasters move to `cam`, which releases them
   return 0;
 }
 
 int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* const* images_out, const int32_t* cam_ids,
                  const wb_detection* const* rows, uint32_t flags, float* gpu_ms) {
-  FXREQ(fx, "NULL fx");
-  FXREQ(n > 0 && n <= 4096, "n out of range");
-  FXREQ(images_in && images_out && cam_ids && rows, "NULL argument");
+  REQUIRE(fx, "NULL fx");
+  REQUIRE(n > 0 && n <= 4096, "n out of range");
+  REQUIRE(images_in && images_out && cam_ids && rows, "NULL argument");
   std::lock_guard<std::mutex> lock(fx->mu);
-  FXCK(cudaSetDevice(fx->device));
+  CK(cudaSetDevice(fx->device));
   const bool on_device = (flags & WB_FX_ON_DEVICE) != 0;
-  FXREQ(!((flags & WB_FX_YUV420P) && (flags & WB_FX_NV12)), "WB_FX_YUV420P and WB_FX_NV12 are mutually exclusive");
-  const int fmt = (flags & WB_FX_YUV420P) ? WB_FMT_YUV420P : (flags & WB_FX_NV12) ? WB_FMT_NV12 : WB_FMT_RGB24;
+  const int fmt = pixel_format(flags & WB_FX_YUV420P, flags & WB_FX_NV12);
+  REQUIRE(fmt >= 0, "WB_FX_YUV420P and WB_FX_NV12 are mutually exclusive");
   size_t total = 0;
   int max_w = 0, max_h = 0;
   for (int i = 0; i < n; ++i) {
     auto it = fx->cams.find(cam_ids[i]);
-    FXREQ(it != fx->cams.end(), "cam_id " + std::to_string(cam_ids[i]) + " has not been configured with wb_fx_set_camera");
-    FXREQ(images_in[i] && images_out[i] && rows[i], "NULL frame / rows pointer");
+    REQUIRE(it != fx->cams.end(), "cam_id " + std::to_string(cam_ids[i]) + " has not been configured with wb_fx_set_camera");
+    REQUIRE(images_in[i] && images_out[i] && rows[i], "NULL frame / rows pointer");
+    const FxCamera& cam = it->second.view;
     if (fmt != WB_FMT_RGB24) {
-      FXREQ(it->second.w % 2 == 0 && it->second.h % 2 == 0,
-            "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(it->second.w) + "x" +
-                std::to_string(it->second.h) + ": 4:2:0 frames need an even width and height");
-      FXREQ(images_in[i] != images_out[i], "4:2:0 input cannot be rendered in place: images_out must be another buffer");
+      REQUIRE(cam.w % 2 == 0 && cam.h % 2 == 0,
+              "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(cam.w) + "x" + std::to_string(cam.h) +
+                  ": 4:2:0 frames need an even width and height");
+      REQUIRE(images_in[i] != images_out[i], "4:2:0 input cannot be rendered in place: images_out must be another buffer");
     }
     // labels are placed inside the frame only if it is high enough for one above/below/inside a box (draw.py:68-73);
     // lower frames would need OpenCV's re-capping of strokes cut by the bottom border, which the tables do not hold
     const int min_h = 2 * (fx->font.text_height + 2 * fx->font.margin + fx->font.baseline) + 1;
-    FXREQ(!(flags & WB_FX_DRAW) || it->second.h >= min_h,
-          "the draw effect needs frames of at least " + std::to_string(min_h) + " rows");
-    total += ((size_t)it->second.w * it->second.h * 3 + 255) / 256 * 256;
-    max_w = std::max(max_w, it->second.w);
-    max_h = std::max(max_h, it->second.h);
+    REQUIRE(!(flags & WB_FX_DRAW) || cam.h >= min_h,
+            "the draw effect needs frames of at least " + std::to_string(min_h) + " rows");
+    total += ((size_t)cam.w * cam.h * 3 + 255) / 256 * 256;
+    max_w = std::max(max_w, cam.w);
+    max_h = std::max(max_h, cam.h);
   }
+  // staging that is too small is replaced once the stream is done with it; after a failed allocation the capacity is 0
   if (n > fx->cap_n) {
-    FXCK(cudaStreamSynchronize(fx->stream));
-    cudaFree(fx->d_rows);
-    cudaFree(fx->d_desc);
-    cudaFree(fx->d_prep);
-    cudaFreeHost(fx->h_rows);
-    cudaFreeHost(fx->h_desc);
+    CK(cudaStreamSynchronize(fx->stream));
     fx->cap_n = 0;
-    FXCK(cudaMalloc(&fx->d_rows, sizeof(wb_detection) * WB_MAX_DETECTIONS * n));
-    FXCK(cudaMalloc(&fx->d_desc, sizeof(FxFrameDesc) * n));
-    FXCK(cudaMalloc(&fx->d_prep, sizeof(FxFrame) * n));
-    FXCK(cudaMallocHost(&fx->h_rows, sizeof(wb_detection) * WB_MAX_DETECTIONS * n));
-    FXCK(cudaMallocHost(&fx->h_desc, sizeof(FxFrameDesc) * n));
+    CK(alloc(fx->d_rows, sizeof(wb_detection) * WB_MAX_DETECTIONS * n));
+    CK(alloc(fx->d_desc, sizeof(FxFrameDesc) * n));
+    CK(alloc(fx->d_prep, sizeof(FxFrame) * n));
+    CK(alloc(fx->h_rows, sizeof(wb_detection) * WB_MAX_DETECTIONS * n));
+    CK(alloc(fx->h_desc, sizeof(FxFrameDesc) * n));
     fx->cap_n = n;
   }
   if (!on_device && total > fx->cap_bytes) {
-    FXCK(cudaStreamSynchronize(fx->stream));
-    cudaFree(fx->d_in);
-    cudaFree(fx->d_out);
+    CK(cudaStreamSynchronize(fx->stream));
     fx->cap_bytes = 0;
-    FXCK(cudaMalloc(&fx->d_in, total));
-    FXCK(cudaMalloc(&fx->d_out, total));
+    CK(alloc(fx->d_in, total));
+    CK(alloc(fx->d_out, total));
     fx->cap_bytes = total;
   }
   cudaStream_t st = fx->stream;
   size_t off = 0;
   for (int i = 0; i < n; ++i) {
-    const FxCamera& cam = fx->cams[cam_ids[i]];
+    const FxCamera& cam = fx->cams[cam_ids[i]].view;
     const size_t bytes = (size_t)cam.w * cam.h * 3;  // staging slot: the RGB24 output, at least the input
     memcpy(fx->h_rows + (size_t)i * WB_MAX_DETECTIONS, rows[i], sizeof(wb_detection) * WB_MAX_DETECTIONS);
     FxFrameDesc d;
@@ -605,56 +594,40 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
       d.in = images_in[i];
       d.out = images_out[i];
     } else {
-      FXCK(cudaMemcpyAsync(fx->d_in + off, images_in[i], frame_bytes(fmt, cam.w, cam.h), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(fx->d_in + off, images_in[i], frame_bytes(fmt, cam.w, cam.h), cudaMemcpyHostToDevice, st));
       d.in = fx->d_in + off;
       d.out = fx->d_out + off;
     }
     fx->h_desc[i] = d;
     off += (bytes + 255) / 256 * 256;
   }
-  FXCK(cudaMemcpyAsync(fx->d_rows, fx->h_rows, sizeof(wb_detection) * WB_MAX_DETECTIONS * n, cudaMemcpyHostToDevice, st));
-  FXCK(cudaMemcpyAsync(fx->d_desc, fx->h_desc, sizeof(FxFrameDesc) * n, cudaMemcpyHostToDevice, st));
-  FXCK(cudaEventRecord(fx->ev0, st));
+  CK(cudaMemcpyAsync(fx->d_rows, fx->h_rows, sizeof(wb_detection) * WB_MAX_DETECTIONS * n, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(fx->d_desc, fx->h_desc, sizeof(FxFrameDesc) * n, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(fx->ev0, st));
   if (flags & WB_FX_DRAW)
     k_fx_prepare<<<n, 128, 0, st>>>(fx->d_rows, fx->d_desc, fx->font, fx->d_labels, fx->n_labels, fx->d_digits, fx->d_prep);
   dim3 grid((max_w + FX_TW - 1) / FX_TW, (max_h + FX_TH - 1) / FX_TH, n);
   k_fx_render<<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
-  FXCK(cudaGetLastError());
-  FXCK(cudaEventRecord(fx->ev1, st));
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(fx->ev1, st));
   if (!on_device) {
     off = 0;
     for (int i = 0; i < n; ++i) {
-      const FxCamera& cam = fx->cams[cam_ids[i]];
+      const FxCamera& cam = fx->cams[cam_ids[i]].view;
       const size_t bytes = (size_t)cam.w * cam.h * 3;
-      FXCK(cudaMemcpyAsync(images_out[i], fx->d_out + off, bytes, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(images_out[i], fx->d_out + off, bytes, cudaMemcpyDeviceToHost, st));
       off += (bytes + 255) / 256 * 256;
     }
   }
-  FXCK(cudaStreamSynchronize(st));
-  if (gpu_ms) FXCK(cudaEventElapsedTime(gpu_ms, fx->ev0, fx->ev1));
+  CK(cudaStreamSynchronize(st));
+  if (gpu_ms) CK(cudaEventElapsedTime(gpu_ms, fx->ev0, fx->ev1));
   return 0;
 }
 
 int wb_fx_destroy(wb_fx* fx) {
   if (!fx) return 0;
   cudaSetDevice(fx->device);
-  if (fx->stream) cudaStreamSynchronize(fx->stream);
-  for (void* p : fx->cam_allocs) cudaFree(p);
-  cudaFree(fx->d_advance);
-  cudaFree(fx->d_lut);
-  cudaFree(fx->d_labels);
-  cudaFree(fx->d_digits);
-  cudaFree(fx->d_aw);
-  cudaFree(fx->d_in);
-  cudaFree(fx->d_out);
-  cudaFree(fx->d_rows);
-  cudaFree(fx->d_desc);
-  cudaFree(fx->d_prep);
-  cudaFreeHost(fx->h_rows);
-  cudaFreeHost(fx->h_desc);
-  if (fx->ev0) cudaEventDestroy(fx->ev0);
-  if (fx->ev1) cudaEventDestroy(fx->ev1);
-  if (fx->stream) cudaStreamDestroy(fx->stream);
-  delete fx;
+  cudaStreamSynchronize(fx->stream);
+  delete fx;  // releases the owned buffers, rasters, stream and events
   return 0;
 }

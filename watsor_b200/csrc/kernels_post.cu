@@ -551,12 +551,9 @@ void launch_post(const LaunchCtx& lc, int n, const PostParams& pp, const float* 
   cudaMemsetAsync(kept_hist, 0, sizeof(int) * (size_t)n * KEPT_BINS, lc.stream);
   int sort_cap = 32;
   while (sort_cap < N) sort_cap <<= 1;
-  static PerDeviceFlag attr_done;
-  if (!attr_done.get()) {
-    cudaFuncSetAttribute(k_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(k_merge_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);
-    attr_done.set();
-  }
+  static PerDeviceFlag nms_attr, merge_attr;
+  max_dynamic_smem_once(k_nms, 200 * 1024, nms_attr);
+  max_dynamic_smem_once(k_merge_filter, 160 * 1024, merge_attr);
   // the chunk buffer (every key may land in one chunk) and the scores: 23.5 KB for 1917 anchors
   const size_t nms_smem = sizeof(unsigned long long) * sort_cap + sizeof(unsigned) * (size_t)N;
   k_nms<<<dim3(C, n), 256, nms_smem, lc.stream>>>(pp, enc, logits, anchors, sort_cap, sel_count, sel_key, sel_box,

@@ -357,10 +357,7 @@ void launch_stem(const LaunchCtx& lc, const FrameDesc* frames, const float* pre,
   const size_t smem = ((((size_t)tile_h * tile_w * 3 + 3) & ~(size_t)3) +
                        (((size_t)L.kh * L.kw * 3 * L.n_pad + 3) & ~(size_t)3)) * sizeof(float);
   static PerDeviceFlag attr_done;
-  if (!attr_done.get()) {
-    cudaFuncSetAttribute(k_stem<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr_done.set();
-  }
+  max_dynamic_smem_once(k_stem<T>, 200 * 1024, attr_done);
   k_stem<T><<<grid, ST_TY * ST_TX, smem, lc.stream>>>(frames, pre, L, in_h, in_w, mul, sub, w, scale, offset, out);
   ++*lc.launch_counter;
 }

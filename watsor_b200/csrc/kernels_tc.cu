@@ -409,7 +409,7 @@ bool tc_layer_supported(const wb_layer& L, int mode, bool conv) {
 int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb_tensor_entry>& tensors,
                        const float* host_data, int mode, bool conv, TcWeights* out, std::string* err) {
   out->mode = mode;
-  out->layers.assign(layers.size(), TcLayerWeights{});
+  out->layers = std::vector<TcLayerWeights>(layers.size());
   for (size_t li = 0; li < layers.size(); ++li) {
     const wb_layer& L = layers[li];
     if (!tc_layer_supported(L, mode, conv)) continue;
@@ -453,32 +453,25 @@ int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb
           }
         }
       }
-    if (cudaMalloc(&w.w, bytes) != cudaSuccess || cudaMemcpy(w.w, hi.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
-      *err = "cudaMalloc/cudaMemcpy of tensor-core weights failed";
-      return 1;
-    }
-    if (!make_map(reinterpret_cast<CUtensorMap*>(w.tmap_b), w.w, mode, NP, K, w.block_n, err)) return 1;
-    if (mode == TC_TF32X3) {
-      if (cudaMalloc(&w.w_lo, bytes) != cudaSuccess ||
-          cudaMemcpy(w.w_lo, lo.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
-        *err = "cudaMalloc/cudaMemcpy of tensor-core weights failed";
-        return 1;
+    // copies `host` to `dev`, and encodes the tensor map of the copy into `tmap`
+    auto upload = [&](DevBuf<void>& dev, const std::vector<uint8_t>& host, unsigned char* tmap) {
+      cudaError_t e = alloc(dev, bytes);
+      if (e == cudaSuccess) e = cudaMemcpy(dev, host.data(), bytes, cudaMemcpyHostToDevice);
+      if (e != cudaSuccess) {
+        *err = std::string("cudaMalloc/cudaMemcpy of tensor-core weights failed: ") + cudaGetErrorString(e);
+        return false;
       }
-      if (!make_map(reinterpret_cast<CUtensorMap*>(w.tmap_b_lo), w.w_lo, mode, NP, K, w.block_n, err)) return 1;
+      return make_map(reinterpret_cast<CUtensorMap*>(tmap), dev, mode, NP, K, w.block_n, err);
+    };
+    if (!upload(w.w, hi, w.tmap_b)) return 1;
+    if (mode == TC_TF32X3) {
+      if (!upload(w.w_lo, lo, w.tmap_b_lo)) return 1;
     } else {
       memcpy(w.tmap_b_lo, w.tmap_b, sizeof(w.tmap_b));
     }
     w.ready = true;
   }
   return 0;
-}
-
-void tc_free_weights(TcWeights* w) {
-  for (auto& l : w->layers) {
-    if (l.w) cudaFree(l.w);
-    if (l.w_lo) cudaFree(l.w_lo);
-  }
-  w->layers.clear();
 }
 
 int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, int n, const wb_layer& L, const void* in,
@@ -567,11 +560,7 @@ int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, in
   memcpy(&map_b_lo, w.tmap_b_lo, sizeof(map_b_lo));
   // split-K launches: the `splits` CTAs of a tile are one thread-block cluster (1, 1, splits)
   auto launch = [&](auto kern, PerDeviceFlag& attr_done) {
-    if (!attr_done.get()) {
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-      if (e != cudaSuccess) return e;
-      attr_done.set();
-    }
+    if (cudaError_t e = max_dynamic_smem_once(kern, 227 * 1024, attr_done)) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = dim3(GEMM_THREADS);

@@ -4,14 +4,15 @@
 #include <vector>
 
 #include "common.cuh"
+#include "host.cuh"
 
 enum TcMode { TC_BF16 = 0, TC_TF32X1 = 1, TC_TF32X3 = 2, TC_FP16 = 3 };
 // bytes per operand element: 2 in the 16-bit modes, 4 (fp32 read as TF32) otherwise
 inline int tc_elem_bytes(int mode) { return mode == TC_BF16 || mode == TC_FP16 ? 2 : 4; }
 
 struct TcLayerWeights {
-  void* w = nullptr;     // [n_pad][K] K-major (bf16, fp16, or fp32 "hi" part), device
-  void* w_lo = nullptr;  // fp32 "lo" part (TF32X3)
+  DevBuf<void> w;     // [n_pad][K] K-major (bf16, fp16, or fp32 "hi" part)
+  DevBuf<void> w_lo;  // fp32 "lo" part (TF32X3)
   int n_pad = 0, k = 0, block_n = 0;
   bool ready = false;
   alignas(64) unsigned char tmap_b[128];     // CUtensorMap of w
@@ -27,7 +28,6 @@ struct TcWeights {
 bool tc_layer_supported(const wb_layer& L, int mode, bool conv);
 int tc_prepare_weights(const std::vector<wb_layer>& layers, const std::vector<wb_tensor_entry>& tensors,
                        const float* host_data, int mode, bool conv, TcWeights* out, std::string* err);
-void tc_free_weights(TcWeights* w);
 // `split_k`: latency-bound shapes may split K over a thread-block cluster
 int tc_launch_gemm(const LaunchCtx& lc, const TcWeights& tw, int layer_index, int n, const wb_layer& L, const void* in,
                    const float* scale, const float* offset, void* out, float* enc, float* logits, int num_anchors,

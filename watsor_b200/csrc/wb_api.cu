@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "host.cuh"
 #include "kernels_tc.cuh"
 
 #define WB_MAX_CAMERAS 256
@@ -23,50 +24,6 @@ static int fail(const std::string& msg) {
   g_err = msg;
   return 1;
 }
-#define CK(call)                                                                              \
-  do {                                                                                        \
-    cudaError_t e_ = (call);                                                                  \
-    if (e_ != cudaSuccess)                                                                    \
-      return fail(std::string(#call) + ": " + cudaGetErrorString(e_) + " (" + __FILE__ + ":" + \
-                  std::to_string(__LINE__) + ")");                                            \
-  } while (0)
-#define REQUIRE(cond, msg) \
-  do {                     \
-    if (!(cond)) return fail(msg); \
-  } while (0)
-
-// An owned CUDA handle (a device or pinned allocation, a stream, an event or a graph exec), released with the Slot,
-// wb_ctx or scope that holds it, so that neither wb_destroy nor an early error return has to list it.  It converts to
-// the raw handle.
-template <typename H, auto Release>
-struct Owned {
-  H h = nullptr;
-  Owned() = default;
-  Owned(const Owned&) = delete;
-  Owned& operator=(const Owned&) = delete;
-  ~Owned() { reset(); }
-  operator H() const { return h; }
-  cudaError_t reset() {
-    const cudaError_t e = h ? Release(h) : cudaSuccess;
-    h = nullptr;
-    return e;
-  }
-};
-template <typename T>
-using DevBuf = Owned<T*, cudaFree>;
-template <typename T>
-using PinnedBuf = Owned<T*, cudaFreeHost>;
-using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
-using Event = Owned<cudaEvent_t, cudaEventDestroy>;
-
-// (re-)allocate `bytes` of device or pinned memory; the previous allocation is released first
-template <typename T, auto Release>
-static cudaError_t alloc(Owned<T*, Release>& b, size_t bytes) {
-  if (cudaError_t e = b.reset()) return e;
-  return Release == cudaFreeHost ? cudaMallocHost(&b.h, bytes) : cudaMalloc(&b.h, bytes);
-}
-static cudaError_t create(Stream& s) { return cudaStreamCreateWithFlags(&s.h, cudaStreamNonBlocking); }
-static cudaError_t create(Event& e) { return cudaEventCreate(&e.h); }
 
 // The precision modes, indexed by wb_create's `precision` (include/watsor_b200.h).  Every precision-dependent choice of
 // the executor reads the mode's row: the activation storage type and the tensor-core GEMMs' operand mode.
@@ -115,7 +72,7 @@ struct Slot {
   bool busy = false;
   int launches = 0;
   // CUDA graph of the kernel sequence, keyed by (model images, flags, frames, windowed)
-  Owned<cudaGraphExec_t, cudaGraphExecDestroy> graph_exec;
+  GraphExec graph_exec;
   int graph_n = -1;
   int graph_frames = -1;
   bool graph_windowed = false;
@@ -141,7 +98,9 @@ struct wb_ctx {
   std::vector<wb_layer> layers;
   std::vector<wb_tensor_entry> tensors;
   DevBuf<float> d_weights;
-  TcWeights tc;  // the GEMM weights in the tensor cores' operand format (modes with a tc_mode)
+  // the GEMM weights in the tensor cores' operand format (modes with a tc_mode).  Declared before `slots`, so the slots'
+  // graph execs, whose kernels read these weights, are released first.
+  TcWeights tc;
   PostParams pp;
   DevBuf<CameraCfg> d_cams;
   std::vector<CameraCfg> h_cams;
@@ -250,9 +209,8 @@ int wb_create(int device, const void* model_blob, size_t blob_bytes, int max_bat
   c->sw.tc_conv = getenv("WB_NO_TC_CONV") == nullptr;
   c->sw.split_k = getenv("WB_NO_SPLITK") == nullptr;
   CK(cudaGetDeviceProperties(&c->prop, device));
-  REQUIRE(c->prop.major == 9 && c->prop.minor == 0, std::string("libwatsor_b200 is built for sm_90a only; device is ") +
-                                   c->prop.name + " (sm_" + std::to_string(c->prop.major) +
-                                   std::to_string(c->prop.minor) + ")");
+  const std::string unsupported = unsupported_device(c->prop);
+  REQUIRE(unsupported.empty(), unsupported);
   memcpy(&c->hdr, model_blob, sizeof(wb_model_header));
   REQUIRE(memcmp(c->hdr.magic, WB_MODEL_MAGIC, 8) == 0, "bad model blob magic");
   const uint8_t* p = static_cast<const uint8_t*>(model_blob) + sizeof(wb_model_header);
@@ -336,9 +294,7 @@ int wb_destroy(wb_ctx* c) {
   cudaDeviceSynchronize();
   wb_comm_destroy(c);
   for (void* r : c->registered) cudaHostUnregister(r);
-  for (auto& s : c->slots) s.graph_exec.reset();
-  tc_free_weights(&c->tc);
-  delete c;  // releases the owned buffers, streams and events
+  delete c;  // releases the owned buffers, streams, events and graph execs
   return 0;
 }
 
@@ -673,13 +629,6 @@ static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t 
   return 0;
 }
 
-// pixel format of a batch from its WB_F_* flags
-static int frame_format(uint32_t flags, int* fmt) {
-  REQUIRE(!((flags & WB_F_YUV420P) && (flags & WB_F_NV12)), "WB_F_YUV420P and WB_F_NV12 are mutually exclusive");
-  *fmt = (flags & WB_F_YUV420P) ? WB_FMT_YUV420P : (flags & WB_F_NV12) ? WB_FMT_NV12 : WB_FMT_RGB24;
-  return 0;
-}
-
 // Copies n host frames of bytes[i] each to s.d_frames, 256-byte aligned, and points dev[i] at frame i's copy.  A buffer
 // that is too small is replaced, once the stream is done with it, by one with 25 % headroom.
 static int upload_frames(Slot& s, cudaStream_t st, int n, const uint8_t* const* frames, const size_t* bytes,
@@ -811,8 +760,8 @@ int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const in
   REQUIRE(!s.busy, "slot is busy: collect it first");
   CK(cudaSetDevice(c->device));
   cudaStream_t st = c->stream_of(slot);
-  int fmt = WB_FMT_RGB24;
-  if (int rc = frame_format(flags, &fmt)) return rc;
+  const int fmt = pixel_format(flags & WB_F_YUV420P, flags & WB_F_NV12);
+  REQUIRE(fmt >= 0, "WB_F_YUV420P and WB_F_NV12 are mutually exclusive");
   CK(cudaEventRecord(s.ev0, st));
   int n_images = n;
   if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &n_images))
@@ -987,8 +936,8 @@ int wb_backbone_frames(wb_ctx* c, int n, const uint8_t* const* frames, const int
   if (h.rc) return h.rc;
   Slot& s = h.s;
   cudaStream_t st = h.st;
-  int fmt = WB_FMT_RGB24;
-  if (int rc = frame_format(flags, &fmt)) return rc;
+  const int fmt = pixel_format(flags & WB_F_YUV420P, flags & WB_F_NV12);
+  REQUIRE(fmt >= 0, "WB_F_YUV420P and WB_F_NV12 are mutually exclusive");
   int ni = n;
   if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &ni)) return rc;
   if (stop_layer >= 0) {
