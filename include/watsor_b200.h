@@ -213,6 +213,8 @@ typedef struct wb_fx_label {      /* drawing attributes of one label index (conf
 #define WB_FX_ON_DEVICE 8u /* images_in / images_out are device pointers */
 #define WB_FX_YUV420P 16u  /* images_in are yuv420p [h*3/2][w] (layouts as for wb_detect); images_out stay RGB24 */
 #define WB_FX_NV12 32u     /* images_in are NV12 [h*3/2][w]; not with WB_FX_YUV420P */
+#define WB_FX_OUT_YUV420P 64u /* images_out are yuv420p [h*3/2][w], for an encoder that takes 4:2:0 */
+#define WB_FX_OUT_NV12 128u   /* images_out are NV12 [h*3/2][w]; not with WB_FX_OUT_YUV420P */
 /* labels[0] is also the style of unknown label indices (coco.py:124-131); digit_glyphs = glyph indices of '0'..'9','%';
  * alpha = opacity of the label box (coco.py:119) */
 int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_label* labels,
@@ -222,8 +224,11 @@ int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_l
 int wb_fx_set_camera(wb_fx* fx, int cam_id, int width, int height, const uint8_t* alpha, const uint32_t* contour_bits);
 /* rows[i]: the 100 Detection rows of frame i (host memory: header.detections).  images: RGB24, host pointers unless
  * WB_FX_ON_DEVICE.  With WB_FX_YUV420P / WB_FX_NV12 images_in are 4:2:0 (even width and height), converted as
- * cv2.cvtColor does, and images_out[i] must not be images_in[i]; without effect flags the call is then a pure
- * converter.  gpu_ms: kernels only. */
+ * cv2.cvtColor does.  With WB_FX_OUT_YUV420P / WB_FX_OUT_NV12 images_out are 4:2:0 (even width and height), the
+ * rendered RGB24 frame converted as cv2.cvtColor(COLOR_RGB2YUV_I420) does (U and V of a 2x2 block from its top-left
+ * pixel; NV12 = the same bytes with U and V interleaved); host output then moves w*h*3/2 bytes per frame.  Any input
+ * format goes with any output format and every effect flag.  With either side 4:2:0, images_out[i] must not be
+ * images_in[i].  Without effect flags the call is a pure format converter.  gpu_ms: kernels only. */
 int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* const* images_out, const int32_t* cam_ids,
                  const wb_detection* const* rows, uint32_t flags, float* gpu_ms);
 int wb_fx_destroy(wb_fx* fx);

@@ -85,9 +85,10 @@ struct FxCameraEntry {
 
 struct FxFrameDesc {
   const uint8_t* in;  // frame_bytes(fmt, w, h) bytes
-  uint8_t* out;       // RGB24
+  uint8_t* out;       // frame_bytes(out_fmt, w, h) bytes
   FxCamera cam;
-  int32_t fmt;        // WB_FMT_* (yuv420.cuh)
+  int32_t fmt;        // WB_FMT_* (yuv420.cuh) of `in`
+  int32_t out_fmt;    // WB_FMT_* of `out`
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -208,6 +209,9 @@ __global__ void __launch_bounds__(128)
 constexpr int FX_TW = 128, FX_TH = 8;
 
 // (forcing 32 registers for 8 blocks per SM instead of 5 spills and measured 8 % slower)
+// YUV_OUT: the frames' out_fmt is yuv420p or NV12.  The RGB24 pass has an instantiation of its own because the 4:2:0
+// store, as a run-time branch, made it 0.8 % slower.
+template <bool YUV_OUT>
 __global__ void __launch_bounds__(256, 5)
     k_fx_render(const FxFrameDesc* __restrict__ frames, const FxFrame* __restrict__ prep, FxFont font,
                 const FxLabel* __restrict__ labels, const uint8_t* __restrict__ aw_lut, uint32_t flags) {
@@ -229,10 +233,13 @@ __global__ void __launch_bounds__(256, 5)
   const size_t px0 = row + (live ? xb : 0);
   const bool yuv = fd.fmt != WB_FMT_RGB24;
   const uint8_t* src = fd.in + px0 * (yuv ? 1 : 3);  // RGB24 pixels, or the luma of a 4:2:0 frame
-  uint8_t* dst = fd.out + px0 * 3;
+  const bool rgb_out = !YUV_OUT;
+  uint8_t* dst = fd.out + px0 * (rgb_out ? 3 : 1);  // RGB24 pixels, or the luma of a 4:2:0 frame
   const bool blend = (flags & WB_FX_BLEND) && fd.cam.alpha != nullptr;
   const bool outline = (flags & WB_FX_CONTOURS) && fd.cam.contours != nullptr;
-  const bool vec = npx == 4 && (((yuv ? 0 : reinterpret_cast<uintptr_t>(src)) | reinterpret_cast<uintptr_t>(dst)) & 3) == 0;
+  // RGB24 loads and stores are whole words when every 4-pixel group of the thread's input and output is aligned
+  const bool vec = npx == 4 && (((yuv ? 0 : reinterpret_cast<uintptr_t>(src)) |
+                                 (rgb_out ? reinterpret_cast<uintptr_t>(dst) : 0)) & 3) == 0;
   // ---- loads first
   uint32_t ws[3] = {0u, 0u, 0u};  // RGB24: the 12 bytes; 4:2:0: 4 Y bytes, then U and V of the 2 chroma samples
   uint8_t v[4][3];
@@ -400,7 +407,43 @@ __global__ void __launch_bounds__(256, 5)
         v[p][2] = 0;
       }
   }
-  if (vec) {
+  if (!rgb_out) {
+    // 4:2:0 as cv2.cvtColor(COLOR_RGB2YUV_I420) computes it: Y of every pixel; U and V of a 2x2 block from its top-left
+    // pixel, which is pixel 0 or 2 of a thread on an even row, so each thread writes only what it holds
+    uint32_t y4 = 0u, us[2], vs[2];
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      uint32_t Y, U, V;
+      rgb_to_yuv(v[p][0], v[p][1], v[p][2], Y, U, V);
+      y4 |= Y << (8 * p);
+      if ((p & 1) == 0) {
+        us[p >> 1] = U;
+        vs[p >> 1] = V;
+      }
+    }
+    if (npx == 4 && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
+      *reinterpret_cast<uint32_t*>(dst) = y4;
+    } else {
+#pragma unroll
+      for (int p = 0; p < 4; ++p)
+        if (p < npx) dst[p] = (uint8_t)(y4 >> (8 * p));
+    }
+    if ((y & 1) == 0) {
+      const ChromaLayout cl = chroma_layout(fd.out_fmt, W, H);
+      uint8_t* c = chroma_ptr(fd.out + (size_t)W * H, cl, xb, y);
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        if (2 * q >= npx) continue;  // npx == 2: one chroma sample
+        uint8_t* cq = c + q * cl.step;
+        if (fd.out_fmt == WB_FMT_NV12 && (reinterpret_cast<uintptr_t>(cq) & 1) == 0) {
+          *reinterpret_cast<uint16_t*>(cq) = (uint16_t)(us[q] | (vs[q] << 8));
+        } else {
+          cq[0] = (uint8_t)us[q];
+          cq[cl.v_off] = (uint8_t)vs[q];
+        }
+      }
+    }
+  } else if (vec) {
     uint32_t wo[3] = {0u, 0u, 0u};
 #pragma unroll
     for (int i = 0; i < 12; ++i) wo[i >> 2] |= (uint32_t)v[i / 3][i % 3] << (8 * (i & 3));
@@ -541,6 +584,8 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   const bool on_device = (flags & WB_FX_ON_DEVICE) != 0;
   const int fmt = pixel_format(flags & WB_FX_YUV420P, flags & WB_FX_NV12);
   REQUIRE(fmt >= 0, "WB_FX_YUV420P and WB_FX_NV12 are mutually exclusive");
+  const int out_fmt = pixel_format(flags & WB_FX_OUT_YUV420P, flags & WB_FX_OUT_NV12);
+  REQUIRE(out_fmt >= 0, "WB_FX_OUT_YUV420P and WB_FX_OUT_NV12 are mutually exclusive");
   size_t total = 0;
   int max_w = 0, max_h = 0;
   for (int i = 0; i < n; ++i) {
@@ -548,11 +593,14 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
     REQUIRE(it != fx->cams.end(), "cam_id " + std::to_string(cam_ids[i]) + " has not been configured with wb_fx_set_camera");
     REQUIRE(images_in[i] && images_out[i] && rows[i], "NULL frame / rows pointer");
     const FxCamera& cam = it->second.view;
-    if (fmt != WB_FMT_RGB24) {
+    if (fmt != WB_FMT_RGB24 || out_fmt != WB_FMT_RGB24) {
       REQUIRE(cam.w % 2 == 0 && cam.h % 2 == 0,
               "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(cam.w) + "x" + std::to_string(cam.h) +
                   ": 4:2:0 frames need an even width and height");
-      REQUIRE(images_in[i] != images_out[i], "4:2:0 input cannot be rendered in place: images_out must be another buffer");
+      // in place, the stores of some threads would overwrite bytes that others still read
+      REQUIRE(images_in[i] != images_out[i], std::string(fmt != WB_FMT_RGB24 ? "4:2:0 input" : "4:2:0 output") +
+                                                 " cannot be rendered in place: images_out must be another buffer (cam_id " +
+                                                 std::to_string(cam_ids[i]) + ")");
     }
     // labels are placed inside the frame only if it is high enough for one above/below/inside a box (draw.py:68-73);
     // lower frames would need OpenCV's re-capping of strokes cut by the bottom border, which the tables do not hold
@@ -590,6 +638,7 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
     FxFrameDesc d;
     d.cam = cam;
     d.fmt = fmt;
+    d.out_fmt = out_fmt;
     if (on_device) {
       d.in = images_in[i];
       d.out = images_out[i];
@@ -607,16 +656,18 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   if (flags & WB_FX_DRAW)
     k_fx_prepare<<<n, 128, 0, st>>>(fx->d_rows, fx->d_desc, fx->font, fx->d_labels, fx->n_labels, fx->d_digits, fx->d_prep);
   dim3 grid((max_w + FX_TW - 1) / FX_TW, (max_h + FX_TH - 1) / FX_TH, n);
-  k_fx_render<<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
+  if (out_fmt == WB_FMT_RGB24)
+    k_fx_render<false><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
+  else
+    k_fx_render<true><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
   CK(cudaGetLastError());
   CK(cudaEventRecord(fx->ev1, st));
   if (!on_device) {
     off = 0;
     for (int i = 0; i < n; ++i) {
       const FxCamera& cam = fx->cams[cam_ids[i]].view;
-      const size_t bytes = (size_t)cam.w * cam.h * 3;
-      CK(cudaMemcpyAsync(images_out[i], fx->d_out + off, bytes, cudaMemcpyDeviceToHost, st));
-      off += (bytes + 255) / 256 * 256;
+      CK(cudaMemcpyAsync(images_out[i], fx->d_out + off, frame_bytes(out_fmt, cam.w, cam.h), cudaMemcpyDeviceToHost, st));
+      off += ((size_t)cam.w * cam.h * 3 + 255) / 256 * 256;
     }
   }
   CK(cudaStreamSynchronize(st));

@@ -1,4 +1,5 @@
-// yuv420.cuh -- 4:2:0 frames (what video decoders emit) converted to the RGB24 bytes the kernels read.
+// yuv420.cuh -- 4:2:0 frames (what video decoders emit) converted to the RGB24 bytes the kernels read, and RGB24
+// pixels converted to the 4:2:0 frames the effects pass can write for an encoder.
 //
 // A 4:2:0 frame of w x h pixels (w, h even) is packed in w*h*3/2 bytes: the full-resolution luma plane, then the
 // chroma at half resolution in both directions.  The two layouts differ only in where the chroma lives, which
@@ -33,8 +34,9 @@ __host__ __device__ __forceinline__ size_t frame_bytes(int fmt, int w, int h) {
 }
 
 // address of the U sample of pixel (x, y) given that of pixel (0, 0); the V sample is at + v_off.  A window of a frame
-// (x0, y0 even) has its own origin `chroma` and keeps the parent frame's layout.
-__device__ __forceinline__ const uint8_t* chroma_ptr(const uint8_t* chroma, const ChromaLayout& cl, int x, int y) {
+// (x0, y0 even) has its own origin `chroma` and keeps the parent frame's layout.  T: uint8_t or const uint8_t.
+template <typename T>
+__device__ __forceinline__ T* chroma_ptr(T* chroma, const ChromaLayout& cl, int x, int y) {
   return chroma + (size_t)(y >> 1) * cl.row + (size_t)(x >> 1) * cl.step;
 }
 
@@ -57,4 +59,16 @@ __device__ __forceinline__ void yuv_to_rgb(uint32_t Y, uint32_t U, uint32_t V, u
   r = yuv_sat(y + 1673527 * v);
   g = yuv_sat(y - 852492 * v - 409993 * u);
   b = yuv_sat(y + 2116026 * u);
+}
+
+// The other direction, for the frames the effects pass writes: Y, U, V of one RGB pixel, BT.601 limited range in 20-bit
+// fixed point, which equals cv2.cvtColor(COLOR_RGB2YUV_I420) on every (R, G, B) triple (tests/test_yuv_out_host.py,
+// tests/test_gpu_yuv_out.py).  OpenCV takes a 2x2 block's U and V from its top-left pixel alone, without averaging,
+// so a caller converts every pixel for Y and only the top-left ones for U and V.  The results lie in 16..240 and every
+// intermediate fits in int32; integer only, so the result does not depend on the file's -fmad setting.
+__device__ __forceinline__ void rgb_to_yuv(uint32_t r, uint32_t g, uint32_t b, uint32_t& Y, uint32_t& U, uint32_t& V) {
+  const int R = (int)r, G = (int)g, B = (int)b;
+  Y = yuv_sat(269484 * R + 528482 * G + 102760 * B + (1 << 19) + (16 << 20));
+  U = yuv_sat(-155188 * R - 305135 * G + 460324 * B + (1 << 19) + (128 << 20));
+  V = yuv_sat(460324 * R - 385875 * G - 74448 * B + (1 << 19) + (128 << 20));
 }

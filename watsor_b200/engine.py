@@ -30,7 +30,8 @@ def _check_format(pixel_format):
 
 def frame_shape(pixel_format, width, height):
     """numpy shape of one packed uint8 frame of a `width` x `height` camera: (H, W, 3) for rgb24, (H*3//2, W) for the
-    4:2:0 formats (luma plane, then the chroma; include/watsor_b200.h), which need an even width and height."""
+    4:2:0 formats (luma plane, then the chroma; include/watsor_b200.h), which need an even width and height.  The same
+    shapes hold for the frames the effects pass reads and writes (output.effects, `output_format`)."""
     _check_format(pixel_format)
     if pixel_format == 'rgb24':
         return (height, width, 3)

@@ -4,7 +4,9 @@ Same class names, constructors and `apply(image_in, image_out, shape, header_in,
 reference, so `Watsor._create_effects` (watsor/main.py:302-312) can return them unchanged; every class is one call
 into `wb_fx_render` (include/watsor_b200.h).  `FusedEffects` does what the whole chain of main.py does for a camera
 -- copy or blend, then draw, then the zone outlines -- in ONE pass over the frame; `EffectsEngine.render` is the batched
-form for several cameras.  There is no CPU fallback: without the library and an H100 the constructors raise.
+form for several cameras.  Both can write the output as yuv420p or NV12 for an encoder, converted on the GPU as
+cv2.cvtColor(COLOR_RGB2YUV_I420) would convert the RGB24 result; the single chained effects stay RGB24, since DrawEffect
+draws onto image_out in place.  There is no CPU fallback: without the library and an H100 the constructors raise.
 
 The output bytes are the reference's: BlendEffect's float32 arithmetic is restated (blend.py:15-32), cv2.rectangle at
 thickness 1 is the box outline, cv2.addWeighted is one float fused multiply-add rounded half to even, the label text
@@ -17,13 +19,15 @@ import numpy as np
 
 from .. import _lib
 from ..config.coco import COCO_CLASSES, get_coco_class
-from ..engine import check_frames
+from ..engine import check_frames, frame_shape
 from ..stream.share import MAX_DETECTIONS, Detection
 from .font import FontAtlas
 
 WB_FX_BLEND, WB_FX_DRAW, WB_FX_CONTOURS, WB_FX_ON_DEVICE = 1, 2, 4, 8
 WB_FX_YUV420P, WB_FX_NV12 = 16, 32
+WB_FX_OUT_YUV420P, WB_FX_OUT_NV12 = 64, 128
 _FX_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_YUV420P, 'nv12': WB_FX_NV12}
+_FX_OUT_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_OUT_YUV420P, 'nv12': WB_FX_OUT_NV12}
 
 
 class _Font(Structure):
@@ -122,13 +126,18 @@ class EffectsEngine:
         self._sizes[cam] = (width, height)
         return cam
 
-    def render(self, images_in, images_out, cam_ids, rows, flags, pixel_format='rgb24'):
+    def render(self, images_in, images_out, cam_ids, rows, flags, pixel_format='rgb24', output_format='rgb24'):
         """images: uint8 arrays (or device pointers with WB_FX_ON_DEVICE); rows: per frame the `Detection * 100`
         array of a frame header (or its address).  pixel_format: layout of images_in, 'rgb24' or a 4:2:0 layout
-        'yuv420p' / 'nv12' (converted as cv2.cvtColor does; see engine.frame_shape).  images_out are RGB24, and with
-        4:2:0 input they must be other buffers than images_in."""
-        check_frames(images_in, [self._sizes.get(c) for c in cam_ids], pixel_format)
-        flags |= _FX_FORMATS[pixel_format]
+        'yuv420p' / 'nv12' (converted as cv2.cvtColor does; see engine.frame_shape).  output_format: layout of
+        images_out, 'rgb24' or 'yuv420p' / 'nv12' for an encoder that takes 4:2:0 (the rendered frame converted as
+        cv2.cvtColor(COLOR_RGB2YUV_I420) does).  With either side 4:2:0, images_out must be other buffers than
+        images_in."""
+        sizes = [self._sizes.get(c) for c in cam_ids]
+        check_frames(images_in, sizes, pixel_format)
+        if output_format != 'rgb24':
+            check_frames(images_out, sizes, output_format)
+        flags |= _FX_FORMATS[pixel_format] | _FX_OUT_FORMATS[output_format]
         n = len(images_in)
 
         def addr(x):
@@ -248,10 +257,14 @@ class DrawEffectWithContours(DrawEffect):
 
 class FusedEffects(_Effect):
     """The image part of the effect chain main.py:302-312 builds for a camera, as one pass:
-    with a mask   BlendEffect + DrawEffectWithContours;   without   CopyImageEffect + DrawEffect."""
+    with a mask   BlendEffect + DrawEffectWithContours;   without   CopyImageEffect + DrawEffect.
+    output_format 'yuv420p' / 'nv12' writes image_out as the 4:2:0 frame an encoder takes (engine.frame_shape), so the
+    output FrameBuffer holds w*h*3//2 bytes and no RGB -> 4:2:0 conversion is left to the encoder."""
 
-    def __init__(self, camera_config, engine=None):
+    def __init__(self, camera_config, engine=None, output_format='rgb24'):
         super().__init__(engine)
+        frame_shape(output_format, camera_config['width'], camera_config['height'])   # a known format, even sizes
+        self.output_format = output_format
         if 'mask' in camera_config:
             alpha, cont = _camera_tables(camera_config, True, True)
             self.flags = WB_FX_BLEND | WB_FX_DRAW | WB_FX_CONTOURS
@@ -261,7 +274,8 @@ class FusedEffects(_Effect):
         self._cam = self._engine_or_default().add_camera(camera_config['width'], camera_config['height'], alpha, cont)
 
     def apply(self, image_in, image_out, shape, header_in, header_out):
-        self._engine.render([image_in], [image_out], [self._cam], [self._rows(header_out)], self.flags)
+        self._engine.render([image_in], [image_out], [self._cam], [self._rows(header_out)], self.flags,
+                            output_format=self.output_format)
 
 
 def new_rows():
@@ -271,4 +285,4 @@ def new_rows():
 
 __all__ = ['EffectsEngine', 'CopyHeaderEffect', 'CopyImageEffect', 'BlendEffect', 'DrawEffect',
            'DrawEffectWithContours', 'FusedEffects', 'contour_bits', 'new_rows', 'WB_FX_BLEND', 'WB_FX_DRAW',
-           'WB_FX_CONTOURS', 'WB_FX_ON_DEVICE', 'WB_FX_YUV420P', 'WB_FX_NV12']
+           'WB_FX_CONTOURS', 'WB_FX_ON_DEVICE', 'WB_FX_YUV420P', 'WB_FX_NV12', 'WB_FX_OUT_YUV420P', 'WB_FX_OUT_NV12']
