@@ -115,7 +115,8 @@ int wb_set_camera(wb_ctx* ctx, int cam_id, int width, int height, int n_zones,
  * (confidence descending, window, row); a row is dropped when an already kept row of the same label from another
  * window covers more than merge_threshold (in [0, 1]) of the smaller of the two inclusive pixel boxes; the first 100
  * kept rows are filtered as the camera's rows always are.  In a batch with windows, a camera without any is one
- * full-frame window.  4:2:0 batches need even window origins and sizes.  n_windows = 0 removes the windows;
+ * full-frame window.  4:2:0 batches need even window origins and sizes, 4:2:2 batches an even x and width.
+ * n_windows = 0 removes the windows;
  * wb_set_camera clears them. */
 #define WB_MAX_WINDOWS 16
 int wb_set_camera_windows(wb_ctx* ctx, int cam_id, int n_windows, const int32_t* xywh, double merge_threshold);
@@ -132,7 +133,11 @@ int wb_unregister_host(wb_ctx* ctx, void* ptr);
  *               for yuv420p; [h/2][w/2] interleaved (U, V) pairs for NV12).  4:2:0 needs an even w and h; the
  *               conversion to RGB (BT.601 limited range) is fused into the resize and equals cv2.cvtColor's
  *               COLOR_YUV2RGB_I420 / COLOR_YUV2RGB_NV12 byte for byte, so the rows equal those of the RGB frame
- *               cvtColor makes.  The format is one per batch.
+ *               cvtColor makes.  With WB_F_YUYV422 or WB_F_UYVY422 a
+ *               packed 4:2:2 frame [h][w][2]: each pixel pair (2k, 2k+1) of a row shares one macropixel, Y0 U Y1 V
+ *               (YUYV) or U Y0 V Y1 (UYVY), and every row has its own chroma.  4:2:2 needs an even w (any h); its
+ *               conversion equals COLOR_YUV2RGB_YUYV / COLOR_YUV2RGB_UYVY the same way.  The format is one per
+ *               batch: at most one of the four format flags.
  *   out[i]      Detection[100] block of that frame's header (share.py:27-32); all 100 rows written
  *   verdicts[i] optional uint32[100] filter verdicts (NULL to skip)
  *   flags       WB_F_* below
@@ -145,7 +150,9 @@ int wb_unregister_host(wb_ctx* ctx, void* ptr);
 /* n counts frames; a batch whose cameras have detection windows (wb_set_camera_windows) runs one model image per
  * window and needs n_images <= max_batch */
 #define WB_F_YUV420P 8u          /* frames[] are yuv420p (ffmpeg -pix_fmt yuv420p)                */
-#define WB_F_NV12 16u            /* frames[] are NV12 (NVDEC's output, packed); not with YUV420P   */
+#define WB_F_NV12 16u            /* frames[] are NV12 (NVDEC's output, packed)                    */
+#define WB_F_YUYV422 32u         /* frames[] are YUYV 4:2:2 (ffmpeg yuyv422: UVC webcams)         */
+#define WB_F_UYVY422 64u         /* frames[] are UYVY 4:2:2 (ffmpeg uyvy422: HDMI / SDI capture)  */
 int wb_detect(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_t* cam_ids,
               uint32_t flags, wb_detection* const* out, uint32_t* const* verdicts, float* gpu_ms);
 
@@ -212,9 +219,11 @@ typedef struct wb_fx_label {      /* drawing attributes of one label index (conf
 #define WB_FX_CONTOURS 4u  /* ... WithContours */
 #define WB_FX_ON_DEVICE 8u /* images_in / images_out are device pointers */
 #define WB_FX_YUV420P 16u  /* images_in are yuv420p [h*3/2][w] (layouts as for wb_detect); images_out stay RGB24 */
-#define WB_FX_NV12 32u     /* images_in are NV12 [h*3/2][w]; not with WB_FX_YUV420P */
+#define WB_FX_NV12 32u     /* images_in are NV12 [h*3/2][w] */
 #define WB_FX_OUT_YUV420P 64u /* images_out are yuv420p [h*3/2][w], for an encoder that takes 4:2:0 */
 #define WB_FX_OUT_NV12 128u   /* images_out are NV12 [h*3/2][w]; not with WB_FX_OUT_YUV420P */
+#define WB_FX_YUYV422 256u    /* images_in are YUYV 4:2:2 [h][w][2] (layouts as for wb_detect) */
+#define WB_FX_UYVY422 512u    /* images_in are UYVY 4:2:2 [h][w][2]; at most one input format flag is set */
 /* labels[0] is also the style of unknown label indices (coco.py:124-131); digit_glyphs = glyph indices of '0'..'9','%';
  * alpha = opacity of the label box (coco.py:119) */
 int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_label* labels,
@@ -224,11 +233,12 @@ int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_l
 int wb_fx_set_camera(wb_fx* fx, int cam_id, int width, int height, const uint8_t* alpha, const uint32_t* contour_bits);
 /* rows[i]: the 100 Detection rows of frame i (host memory: header.detections).  images: RGB24, host pointers unless
  * WB_FX_ON_DEVICE.  With WB_FX_YUV420P / WB_FX_NV12 images_in are 4:2:0 (even width and height), converted as
- * cv2.cvtColor does.  With WB_FX_OUT_YUV420P / WB_FX_OUT_NV12 images_out are 4:2:0 (even width and height), the
+ * cv2.cvtColor does; with WB_FX_YUYV422 / WB_FX_UYVY422 they are packed 4:2:2 (even width, any height),
+ * converted the same way.  With WB_FX_OUT_YUV420P / WB_FX_OUT_NV12 images_out are 4:2:0 (even width and height), the
  * rendered RGB24 frame converted as cv2.cvtColor(COLOR_RGB2YUV_I420) does (U and V of a 2x2 block from its top-left
  * pixel; NV12 = the same bytes with U and V interleaved); host output then moves w*h*3/2 bytes per frame.  Any input
- * format goes with any output format and every effect flag.  With either side 4:2:0, images_out[i] must not be
- * images_in[i].  Without effect flags the call is a pure format converter.  gpu_ms: kernels only. */
+ * format goes with any output format and every effect flag.  With either side in a YUV format, images_out[i] must
+ * not be images_in[i].  Without effect flags the call is a pure format converter.  gpu_ms: kernels only. */
 int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* const* images_out, const int32_t* cam_ids,
                  const wb_detection* const* rows, uint32_t flags, float* gpu_ms);
 int wb_fx_destroy(wb_fx* fx);
@@ -243,9 +253,11 @@ int wb_preprocess(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_
  * copies that layer's activation (float32 NHWC) to layer_out. */
 int wb_backbone(wb_ctx* ctx, int n, const float* pre, float* enc, float* logits, int stop_layer,
                 float* layer_out, size_t layer_out_floats);
-/* the product path's own input handling (frames as wb_submit takes them: host or device, rgb24 / yuv420p / nv12,
+/* the product path's own input handling (frames as wb_submit takes them: host or device, rgb24 / yuv420p / nv12 /
+ * yuyv422 / uyvy422,
  * a camera's detection windows expanded into model images), run to stop_layer; n_images = model images of the batch.
- * flags: WB_F_YUV420P, WB_F_NV12, WB_F_FRAMES_ON_DEVICE, WB_F_FUSE_FILTERS.  Runs on slot 0.
+ * flags: one format flag (WB_F_YUV420P, WB_F_NV12, WB_F_YUYV422, WB_F_UYVY422), WB_F_FRAMES_ON_DEVICE,
+ * WB_F_FUSE_FILTERS.  Runs on slot 0.
  *   stop_layer >= 0: the layers up to stop_layer, eagerly; layer_out as for wb_backbone, for n_images images.
  *   stop_layer == -1: the kernels of wb_submit (CUDA graph, post stage, window merge).
  * enc / logits (optional): [n_images][anchors][4] / [n_images][anchors][classes+1] as the run left them -- unlike

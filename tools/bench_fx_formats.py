@@ -4,9 +4,9 @@
     python tools/bench_fx_formats.py --steps 200 --warmup 20 --rounds 5
 
 Workload: bench.py's effects record -- 8 masked cameras of 640x480 (tests/workload.py), 8 labelled detections per
-frame, BlendEffect + DrawEffectWithContours as one wb_fx_render per tick -- with the input in rgb24 or NV12 and the
-output in rgb24, yuv420p or NV12.  The RGB input frames are cv2.cvtColor of the NV12 ones, so every combination
-renders the same pixels.  Per combination and round:
+frame, BlendEffect + DrawEffectWithContours as one wb_fx_render per tick -- with the input in rgb24, NV12, YUYV or UYVY
+and the output in rgb24, yuv420p or NV12.  The RGB input frames are cv2.cvtColor of the NV12 ones and the 4:2:2 ones
+repeat each 4:2:0 chroma row for its two luma rows, so every combination renders the same pixels.  Per combination and round:
   device_fps  frames / s from the library's device time (CUDA events, kernels only) with device pointers
   e2e_fps     frames / s of synchronous wb_fx_render calls from pinned host frames to pinned host frames
               (H2D + kernels + D2H), wall clock
@@ -28,13 +28,14 @@ sys.path.insert(0, ROOT)
 from tests import workload  # noqa: E402
 from tests.artist import artist_frame  # noqa: E402
 from tests.fx_cases import random_rows  # noqa: E402
+from tests.yuv422_emulation import from_i420  # noqa: E402
 from tests.yuv_emulation import cv2_rgb, from_rgb  # noqa: E402
 from watsor_b200.engine import frame_shape  # noqa: E402
 from watsor_b200.filter.mask import get_alpha_channel  # noqa: E402
 from watsor_b200.output.effects import (WB_FX_BLEND, WB_FX_CONTOURS, WB_FX_DRAW, WB_FX_ON_DEVICE,  # noqa: E402
                                         EffectsEngine, contour_bits)
 
-IN_FORMATS = ('rgb24', 'nv12')
+IN_FORMATS = ('rgb24', 'nv12', 'yuyv422', 'uyvy422')
 OUT_FORMATS = ('rgb24', 'yuv420p', 'nv12')
 CAMS, W, H = 8, 640, 480
 
@@ -56,13 +57,16 @@ def main():
     info = card()
     rng = np.random.default_rng(3)
     eng = EffectsEngine(0)
-    cams, rows, frames = [], [], {'rgb24': [], 'nv12': []}
+    cams, rows, frames = [], [], {f: [] for f in IN_FORMATS}
     for c in range(CAMS):
         alpha, _ = get_alpha_channel(workload.camera_config(c)['mask'], W, H)
         cams.append(eng.add_camera(W, H, alpha, contour_bits(alpha)))
         rows.append(random_rows(rng, W, H, 8, n_zones=1))
+        i420 = from_rgb(artist_frame(W, H, c, 0), 'yuv420p')
         nv12 = from_rgb(artist_frame(W, H, c, 0), 'nv12')
         frames['nv12'].append(nv12)
+        for f in ('yuyv422', 'uyvy422'):
+            frames[f].append(from_i420(i420, f))
         frames['rgb24'].append(np.ascontiguousarray(cv2_rgb(nv12, 'nv12')))
     flags = WB_FX_BLEND | WB_FX_DRAW | WB_FX_CONTOURS
     combos = [(i, o) for i in IN_FORMATS for o in OUT_FORMATS]

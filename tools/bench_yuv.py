@@ -1,12 +1,14 @@
 #!/usr/bin/env python
-"""Detection throughput by input pixel format: rgb24 against the 4:2:0 layouts decoders emit (yuv420p, NV12).
+"""Detection throughput by input pixel format: rgb24 against the 4:2:0 layouts decoders emit (yuv420p, NV12) and the
+packed 4:2:2 layouts of webcams and capture cards (yuyv422, uyvy422).
 
     python tools/bench_yuv.py --steps 200 --warmup 20 --rounds 5
 
 Workloads (tests/workload.py): BASELINE configs[2] (8 cameras of 640x480, SSD-MobileNet-v2 with 90 classes at score
 threshold 1e-8, a mask per camera, fused filters) and 2 cameras of 1920x1080 with the same model.  The RGB frames are
-cv2.cvtColor of the 4:2:0 ones, so every format computes the same rows, and the script checks that the last step's
-rows and verdicts are identical across the three formats.  Per format and round:
+cv2.cvtColor of the 4:2:0 ones and the 4:2:2 frames repeat each 4:2:0 chroma row for its two luma rows, so every format
+computes the same rows, and the script checks that the last step's rows and verdicts are identical across the
+formats.  Per format and round:
   device_fps  frames / s from the library's device time (CUDA events) with the frames resident on the GPU
   e2e_fps     frames / s of synchronous detect_batch calls from pinned host frames (H2D + kernels + D2H), wall clock
 The formats run alternately within each round; the figures are the medians over rounds.  One JSON line per
@@ -26,10 +28,11 @@ sys.path.insert(0, ROOT)
 from tests import workload  # noqa: E402
 from tests.artist import artist_frame  # noqa: E402
 from tests.gpu_util import new_rows, rows_bytes  # noqa: E402
+from tests.yuv422_emulation import from_i420  # noqa: E402
 from tests.yuv_emulation import cv2_rgb, from_rgb  # noqa: E402
 from watsor_b200.detection.b200 import B200ObjectDetector  # noqa: E402
 
-FORMATS = ('rgb24', 'yuv420p', 'nv12')
+FORMATS = ('rgb24', 'yuv420p', 'nv12', 'yuyv422', 'uyvy422')
 
 
 def card():
@@ -40,7 +43,8 @@ def card():
 
 
 def frames_for(w, h, cams, ring):
-    """ring x cams frames per format: 4:2:0 made from Artist frames, RGB = cvtColor of the yuv420p ones"""
+    """ring x cams frames per format: 4:2:0 made from Artist frames, RGB = cvtColor of the yuv420p ones, 4:2:2 with
+    the yuv420p ones' pixels"""
     out = {f: [] for f in FORMATS}
     for r in range(ring):
         for c in range(cams):
@@ -49,6 +53,8 @@ def frames_for(w, h, cams, ring):
             out['yuv420p'].append(i420)
             out['nv12'].append(from_rgb(rgb, 'nv12'))
             out['rgb24'].append(np.ascontiguousarray(cv2_rgb(i420, 'yuv420p')))
+            for f in ('yuyv422', 'uyvy422'):
+                out[f].append(from_i420(i420, f))
     return out
 
 

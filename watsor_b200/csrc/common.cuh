@@ -13,13 +13,14 @@
 // detection window of one (wb_set_camera_windows); either way its rows start at `ptr`, `pitch` bytes apart.
 // Replaces the (image_shape, image_np) pair of ObjectDetector.detect (tensorflow_cpu.py:74).
 struct FrameDesc {
-  const uint8_t* ptr;     // device pointer to pixel (0, 0): RGB24 HWC (share.py:68-73), or the luma of a 4:2:0 frame
-  const uint8_t* chroma;  // 4:2:0: the U sample of pixel (0, 0) (packed frame: ptr + w*h)
+  const uint8_t* ptr;     // device pointer to pixel (0, 0): RGB24 HWC (share.py:68-73), or its Y sample in a YUV frame
+  const uint8_t* chroma;  // YUV: the U sample of pixel (0, 0) (packed frame: ptr + w*h for 4:2:0; the U byte of the
+                          // pixel's macropixel for 4:2:2)
   int32_t w, h;
-  int32_t pitch;          // bytes between rows of the RGB24 / luma plane (packed frame: 3w / w)
+  int32_t pitch;          // bytes between rows of the RGB24 / luma plane / macropixels (packed frame: 3w / w / 2w)
   int32_t cam;            // -1: no camera (a window's rows are filtered after the merge, k_window_merge)
   int32_t fmt;            // WB_FMT_* (yuv420.cuh)
-  int32_t v_off;          // 4:2:0: bytes from a U sample to its V sample (ChromaLayout::v_off of the parent frame)
+  int32_t v_off;          // YUV: bytes from a U sample to its V sample (ChromaLayout::v_off of the parent frame; 2 for 4:2:2)
 };
 
 // The model images of one frame of a windowed batch, for k_window_merge: images [first, first + count) are its

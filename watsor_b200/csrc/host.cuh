@@ -5,6 +5,7 @@
 
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "yuv420.cuh"
 
@@ -67,8 +68,27 @@ inline std::string unsupported_device(const cudaDeviceProp& prop) {
          std::to_string(prop.major) + std::to_string(prop.minor) + ")";
 }
 
-// the pixel format (WB_FMT_*) that a call's two 4:2:0 flag bits select, or -1 when both are set
-inline int pixel_format(bool yuv420p, bool nv12) {
-  if (yuv420p && nv12) return -1;
-  return yuv420p ? WB_FMT_YUV420P : nv12 ? WB_FMT_NV12 : WB_FMT_RGB24;
+// one pixel-format flag bit of a C-ABI call: the format (WB_FMT_*) it selects and its name for error messages
+struct FormatFlag {
+  uint32_t bit;
+  int fmt;
+  const char* name;
+};
+
+// the pixel format that the format bits of `flags` select (WB_FMT_RGB24 when none is set); -1 when more than one is
+// set, with `err` naming them ("WB_F_YUV420P and WB_F_NV12 are mutually exclusive")
+template <size_t N>
+inline int pixel_format(uint32_t flags, const FormatFlag (&table)[N], std::string& err) {
+  int fmt = WB_FMT_RGB24;
+  std::vector<const char*> set;
+  for (const FormatFlag& f : table)
+    if (flags & f.bit) {
+      fmt = f.fmt;
+      set.push_back(f.name);
+    }
+  if (set.size() <= 1) return fmt;
+  err.clear();
+  for (size_t i = 0; i < set.size(); ++i) err += std::string(i == 0 ? "" : i + 1 == set.size() ? " and " : ", ") + set[i];
+  err += " are mutually exclusive";
+  return -1;
 }

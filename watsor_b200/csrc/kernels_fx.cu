@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(256, 5)
   const int npx = live ? min(4, W - xb) : 0;
   const size_t px0 = row + (live ? xb : 0);
   const bool yuv = fd.fmt != WB_FMT_RGB24;
-  const uint8_t* src = fd.in + px0 * (yuv ? 1 : 3);  // RGB24 pixels, or the luma of a 4:2:0 frame
+  const uint8_t* src = fd.in + px0 * 3;  // RGB24 pixels (a YUV frame's samples are addressed below)
   const bool rgb_out = !YUV_OUT;
   uint8_t* dst = fd.out + px0 * (rgb_out ? 3 : 1);  // RGB24 pixels, or the luma of a 4:2:0 frame
   const bool blend = (flags & WB_FX_BLEND) && fd.cam.alpha != nullptr;
@@ -241,23 +241,30 @@ __global__ void __launch_bounds__(256, 5)
   const bool vec = npx == 4 && (((yuv ? 0 : reinterpret_cast<uintptr_t>(src)) |
                                  (rgb_out ? reinterpret_cast<uintptr_t>(dst) : 0)) & 3) == 0;
   // ---- loads first
-  uint32_t ws[3] = {0u, 0u, 0u};  // RGB24: the 12 bytes; 4:2:0: 4 Y bytes, then U and V of the 2 chroma samples
+  uint32_t ws[3] = {0u, 0u, 0u};  // RGB24: the 12 bytes; YUV: 4 Y bytes, then U and V of the 2 chroma samples
   uint8_t v[4][3];
   uint8_t al[4] = {255, 255, 255, 255};
   uint32_t cb[4] = {0u, 0u, 0u, 0u};
   if (yuv) {
-    // 4 pixels starting at a multiple of 4 in an even-width frame: exactly 2 chroma samples
-    const ChromaLayout cl = chroma_layout(fd.fmt, W, H);
-    const uint8_t* c = chroma_ptr(fd.in + (size_t)W * H, cl, live ? xb : 0, live ? y : 0);
+    // 4 pixels starting at a multiple of 4 in an even-width frame: exactly 2 chroma samples (4:2:2: two macropixels,
+    // or one when the width is 2 mod 4).  4:2:2 and 4:2:0 branch apart so that each sees its layout as constants.
+    auto load = [&](const ChromaLayout& cl, const uint8_t* luma, const uint8_t* chroma) {
+      const uint8_t* c = chroma_ptr(chroma, cl, live ? xb : 0, live ? y : 0);
 #pragma unroll
-    for (int p = 0; p < 4; ++p)
-      if (p < npx) ws[0] |= (uint32_t)__ldg(src + p) << (8 * p);
+      for (int p = 0; p < 4; ++p)
+        if (p < npx) ws[0] |= (uint32_t)__ldg(luma + (px0 + p) * cl.luma_step) << (8 * p);
 #pragma unroll
-    for (int q = 0; q < 2; ++q)
-      if (2 * q < npx) {
-        ws[1] |= (uint32_t)__ldg(c + q * cl.step) << (8 * q);
-        ws[2] |= (uint32_t)__ldg(c + q * cl.step + cl.v_off) << (8 * q);
-      }
+      for (int q = 0; q < 2; ++q)
+        if (2 * q < npx) {
+          ws[1] |= (uint32_t)__ldg(c + q * cl.step) << (8 * q);
+          ws[2] |= (uint32_t)__ldg(c + q * cl.step + cl.v_off) << (8 * q);
+        }
+    };
+    if (fmt_422(fd.fmt)) {
+      load(chroma_layout(WB_FMT_YUYV422, W, H), fd.in + luma_origin(fd.fmt), fd.in + chroma_origin(fd.fmt, W, H));
+    } else {
+      load(chroma_layout(fd.fmt == WB_FMT_NV12 ? WB_FMT_NV12 : WB_FMT_YUV420P, W, H), fd.in, fd.in + (size_t)W * H);
+    }
   } else if (vec) {
     const uint32_t* s32 = reinterpret_cast<const uint32_t*>(src);
     ws[0] = __ldg(s32);
@@ -429,17 +436,18 @@ __global__ void __launch_bounds__(256, 5)
         if (p < npx) dst[p] = (uint8_t)(y4 >> (8 * p));
     }
     if ((y & 1) == 0) {
-      const ChromaLayout cl = chroma_layout(fd.out_fmt, W, H);
-      uint8_t* c = chroma_ptr(fd.out + (size_t)W * H, cl, xb, y);
+      // out_fmt is yuv420p or NV12: spelt out, so that the layout's 4:2:0 steps and shifts are constants here
+      const ChromaLayout co = chroma_layout(fd.out_fmt == WB_FMT_NV12 ? WB_FMT_NV12 : WB_FMT_YUV420P, W, H);
+      uint8_t* c = chroma_ptr(fd.out + (size_t)W * H, co, xb, y);
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         if (2 * q >= npx) continue;  // npx == 2: one chroma sample
-        uint8_t* cq = c + q * cl.step;
+        uint8_t* cq = c + q * co.step;
         if (fd.out_fmt == WB_FMT_NV12 && (reinterpret_cast<uintptr_t>(cq) & 1) == 0) {
           *reinterpret_cast<uint16_t*>(cq) = (uint16_t)(us[q] | (vs[q] << 8));
         } else {
           cq[0] = (uint8_t)us[q];
-          cq[cl.v_off] = (uint8_t)vs[q];
+          cq[co.v_off] = (uint8_t)vs[q];
         }
       }
     }
@@ -582,10 +590,18 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   std::lock_guard<std::mutex> lock(fx->mu);
   CK(cudaSetDevice(fx->device));
   const bool on_device = (flags & WB_FX_ON_DEVICE) != 0;
-  const int fmt = pixel_format(flags & WB_FX_YUV420P, flags & WB_FX_NV12);
-  REQUIRE(fmt >= 0, "WB_FX_YUV420P and WB_FX_NV12 are mutually exclusive");
-  const int out_fmt = pixel_format(flags & WB_FX_OUT_YUV420P, flags & WB_FX_OUT_NV12);
-  REQUIRE(out_fmt >= 0, "WB_FX_OUT_YUV420P and WB_FX_OUT_NV12 are mutually exclusive");
+  static const FormatFlag in_formats[] = {{WB_FX_YUV420P, WB_FMT_YUV420P, "WB_FX_YUV420P"},
+                                          {WB_FX_NV12, WB_FMT_NV12, "WB_FX_NV12"},
+                                          {WB_FX_YUYV422, WB_FMT_YUYV422, "WB_FX_YUYV422"},
+                                          {WB_FX_UYVY422, WB_FMT_UYVY422, "WB_FX_UYVY422"}};
+  static const FormatFlag out_formats[] = {{WB_FX_OUT_YUV420P, WB_FMT_YUV420P, "WB_FX_OUT_YUV420P"},
+                                           {WB_FX_OUT_NV12, WB_FMT_NV12, "WB_FX_OUT_NV12"}};
+  std::string err;
+  const int fmt = pixel_format(flags, in_formats, err);
+  REQUIRE(fmt >= 0, err);
+  const int out_fmt = pixel_format(flags, out_formats, err);
+  REQUIRE(out_fmt >= 0, err);
+  const bool yuv420 = fmt == WB_FMT_YUV420P || fmt == WB_FMT_NV12 || out_fmt != WB_FMT_RGB24;
   size_t total = 0;
   int max_w = 0, max_h = 0;
   for (int i = 0; i < n; ++i) {
@@ -594,13 +610,15 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
     REQUIRE(images_in[i] && images_out[i] && rows[i], "NULL frame / rows pointer");
     const FxCamera& cam = it->second.view;
     if (fmt != WB_FMT_RGB24 || out_fmt != WB_FMT_RGB24) {
-      REQUIRE(cam.w % 2 == 0 && cam.h % 2 == 0,
-              "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(cam.w) + "x" + std::to_string(cam.h) +
-                  ": 4:2:0 frames need an even width and height");
+      const std::string size = "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(cam.w) + "x" +
+                               std::to_string(cam.h);
+      REQUIRE(!yuv420 || (cam.w % 2 == 0 && cam.h % 2 == 0), size + ": 4:2:0 frames need an even width and height");
+      REQUIRE(cam.w % 2 == 0, size + ": 4:2:2 frames need an even width");
       // in place, the stores of some threads would overwrite bytes that others still read
-      REQUIRE(images_in[i] != images_out[i], std::string(fmt != WB_FMT_RGB24 ? "4:2:0 input" : "4:2:0 output") +
-                                                 " cannot be rendered in place: images_out must be another buffer (cam_id " +
-                                                 std::to_string(cam_ids[i]) + ")");
+      REQUIRE(images_in[i] != images_out[i],
+              std::string(fmt_422(fmt) ? "4:2:2 input" : fmt != WB_FMT_RGB24 ? "4:2:0 input" : "4:2:0 output") +
+                  " cannot be rendered in place: images_out must be another buffer (cam_id " +
+                  std::to_string(cam_ids[i]) + ")");
     }
     // labels are placed inside the frame only if it is high enough for one above/below/inside a box (draw.py:68-73);
     // lower frames would need OpenCV's re-capping of strokes cut by the bottom border, which the tables do not hold

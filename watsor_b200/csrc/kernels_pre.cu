@@ -36,8 +36,8 @@ __device__ __forceinline__ float lerp_px(float tl, float tr, float bl, float br,
 }
 
 // The 12 source bytes one resized pixel interpolates: channel c of tap k (tl, tr, bl, br) goes to raw[c * 4 + k].
-// For a 4:2:0 frame the slots hold Y, U, V of each tap, and resized_pixel_lerp converts them to the RGB24 bytes of
-// cv2.cvtColor first, so the interpolation sees the same bytes as for the converted RGB frame.
+// For a YUV frame (4:2:0 or 4:2:2) the slots hold Y, U, V of each tap, and resized_pixel_lerp converts them to the
+// RGB24 bytes of cv2.cvtColor first, so the interpolation sees the same bytes as for the converted RGB frame.
 __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const AxisTap& ty, const AxisTap& tx,
                                                    uint32_t (&raw)[12]) {
   if (fd.fmt == WB_FMT_RGB24) {
@@ -51,13 +51,18 @@ __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const Ax
       raw[c * 4 + 3] = __ldg(r1 + tx.hi * 3 + c);
     }
   } else {
-    // the chroma rows are half as many bytes apart as the luma rows (yuv420p) or as many (NV12's U, V pairs)
-    const bool nv12 = fd.fmt == WB_FMT_NV12;
-    const ChromaLayout cl{nv12 ? 2 : 1, nv12 ? fd.pitch : fd.pitch / 2, (size_t)fd.v_off};
-    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.lo, ty.lo, raw[0], raw[4], raw[8]);
-    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.hi, ty.lo, raw[1], raw[5], raw[9]);
-    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.lo, ty.hi, raw[2], raw[6], raw[10]);
-    yuv420_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.hi, ty.hi, raw[3], raw[7], raw[11]);
+    // 4:2:2 and 4:2:0 branch apart so that each sees its layout's steps and shifts as constants (a layout chosen at
+    // run time kept them in registers, and the generic stem spilled)
+    auto taps = [&](const ChromaLayout& cl) {
+      yuv_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.lo, ty.lo, raw[0], raw[4], raw[8]);
+      yuv_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.hi, ty.lo, raw[1], raw[5], raw[9]);
+      yuv_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.lo, ty.hi, raw[2], raw[6], raw[10]);
+      yuv_load(fd.ptr, fd.pitch, fd.chroma, cl, tx.hi, ty.hi, raw[3], raw[7], raw[11]);
+    };
+    if (fmt_422(fd.fmt))
+      taps(chroma_layout_of(WB_FMT_YUYV422, fd.pitch, 2));
+    else
+      taps(chroma_layout_of(fd.fmt == WB_FMT_NV12 ? WB_FMT_NV12 : WB_FMT_YUV420P, fd.pitch, (size_t)fd.v_off));
   }
 }
 __device__ __forceinline__ void resized_pixel_lerp(uint32_t (&raw)[12], bool yuv, float lx, float ly, float mul,

@@ -649,6 +649,12 @@ static int upload_frames(Slot& s, cudaStream_t st, int n, const uint8_t* const* 
   return 0;
 }
 
+// the frame formats of wb_detect / wb_submit / wb_backbone_frames
+static const FormatFlag kFrameFormats[] = {{WB_F_YUV420P, WB_FMT_YUV420P, "WB_F_YUV420P"},
+                                           {WB_F_NV12, WB_FMT_NV12, "WB_F_NV12"},
+                                           {WB_F_YUYV422, WB_FMT_YUYV422, "WB_F_YUYV422"},
+                                           {WB_F_UYVY422, WB_FMT_UYVY422, "WB_F_UYVY422"}};
+
 // One descriptor per model image.  With use_windows and at least one camera of the batch having detection windows, the
 // batch is windowed: every window of a frame is one image (a camera without windows: one full-frame window, camera
 // -1), and s.h_win / s.d_win describe the frames for k_window_merge.  Otherwise an image is a frame, as always.  A host
@@ -665,19 +671,24 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
             "cam_id " + std::to_string(cam) + " has not been configured with wb_set_camera");
     REQUIRE(frames == nullptr || frames[i] != nullptr, "NULL frame pointer");
     const CameraCfg& cc = c->h_cams[cam];
-    REQUIRE(fmt == WB_FMT_RGB24 || (cc.width % 2 == 0 && cc.height % 2 == 0),
-            "cam_id " + std::to_string(cam) + " is " + std::to_string(cc.width) + "x" + std::to_string(cc.height) +
-                ": 4:2:0 frames need an even width and height");
+    // 4:2:0 chroma covers 2x2 pixels, 4:2:2 chroma a pixel pair of one row
+    const bool yuv420 = fmt == WB_FMT_YUV420P || fmt == WB_FMT_NV12;
+    const std::string size = "cam_id " + std::to_string(cam) + " is " + std::to_string(cc.width) + "x" +
+                             std::to_string(cc.height);
+    REQUIRE(!yuv420 || (cc.width % 2 == 0 && cc.height % 2 == 0), size + ": 4:2:0 frames need an even width and height");
+    REQUIRE(!fmt_422(fmt) || cc.width % 2 == 0, size + ": 4:2:2 frames need an even width");
     bytes[i] = frame_bytes(fmt, cc.width, cc.height);
     const int nw = use_windows ? (int)c->cam_windows[cam].size() : 0;
     windowed |= nw > 0;
     n_images += std::max(nw, 1);
     for (int k = 0; k < nw; ++k) {
       const int4 wd = c->cam_windows[cam][k];
-      REQUIRE(fmt == WB_FMT_RGB24 || (wd.x % 2 == 0 && wd.y % 2 == 0 && wd.z % 2 == 0 && wd.w % 2 == 0),
-              "cam_id " + std::to_string(cam) + " window " + std::to_string(k) + " (" + std::to_string(wd.x) + ", " +
-                  std::to_string(wd.y) + ", " + std::to_string(wd.z) + ", " + std::to_string(wd.w) +
-                  "): 4:2:0 frames need an even window origin, width and height");
+      const std::string win = "cam_id " + std::to_string(cam) + " window " + std::to_string(k) + " (" +
+                              std::to_string(wd.x) + ", " + std::to_string(wd.y) + ", " + std::to_string(wd.z) + ", " +
+                              std::to_string(wd.w) + ")";
+      REQUIRE(!yuv420 || (wd.x % 2 == 0 && wd.y % 2 == 0 && wd.z % 2 == 0 && wd.w % 2 == 0),
+              win + ": 4:2:0 frames need an even window origin, width and height");
+      REQUIRE(!fmt_422(fmt) || (wd.x % 2 == 0 && wd.z % 2 == 0), win + ": 4:2:2 frames need an even window x and width");
     }
   }
   REQUIRE(n_images <= c->max_batch, "the batch's detection windows add up to " + std::to_string(n_images) +
@@ -695,7 +706,8 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
     const CameraCfg& cc = c->h_cams[cam];
     const uint8_t* base = dev[i];
     const ChromaLayout cl = chroma_layout(fmt, cc.width, cc.height);
-    const int bpp = fmt == WB_FMT_RGB24 ? 3 : 1;  // bytes per pixel of the RGB24 / luma plane
+    const int bpp = fmt == WB_FMT_RGB24 ? 3 : cl.luma_step;  // bytes per pixel of the RGB24 / luma plane / macropixels
+    const size_t luma0 = fmt == WB_FMT_RGB24 ? 0 : luma_origin(fmt);
     const std::vector<int4>& wins = c->cam_windows[cam];
     const int nw = windowed ? std::max((int)wins.size(), 1) : 1;
     if (windowed) {
@@ -709,8 +721,9 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
     for (int k = 0; k < nw; ++k) {
       const int4 wd = (windowed && !wins.empty()) ? wins[k] : make_int4(0, 0, cc.width, cc.height);
       FrameDesc d;
-      d.ptr = base ? base + ((size_t)wd.y * cc.width + wd.x) * bpp : nullptr;
-      d.chroma = base ? base + (size_t)cc.width * cc.height + (size_t)(wd.y >> 1) * cl.row + (size_t)(wd.x >> 1) * cl.step
+      d.ptr = base ? base + luma0 + ((size_t)wd.y * cc.width + wd.x) * bpp : nullptr;
+      d.chroma = base ? base + chroma_origin(fmt, cc.width, cc.height) + (size_t)(wd.y >> cl.row_shift) * cl.row +
+                            (size_t)(wd.x >> 1) * cl.step
                       : nullptr;
       d.w = wd.z;
       d.h = wd.w;
@@ -760,8 +773,9 @@ int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const in
   REQUIRE(!s.busy, "slot is busy: collect it first");
   CK(cudaSetDevice(c->device));
   cudaStream_t st = c->stream_of(slot);
-  const int fmt = pixel_format(flags & WB_F_YUV420P, flags & WB_F_NV12);
-  REQUIRE(fmt >= 0, "WB_F_YUV420P and WB_F_NV12 are mutually exclusive");
+  std::string err;
+  const int fmt = pixel_format(flags, kFrameFormats, err);
+  REQUIRE(fmt >= 0, err);
   CK(cudaEventRecord(s.ev0, st));
   int n_images = n;
   if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &n_images))
@@ -930,14 +944,17 @@ int wb_backbone_frames(wb_ctx* c, int n, const uint8_t* const* frames, const int
                        int32_t* n_images) {
   REQUIRE(c && frames && cam_ids, "NULL argument");
   REQUIRE(stop_layer >= -1 && stop_layer < (int)c->layers.size(), "stop_layer out of range");
-  REQUIRE((flags & ~(WB_F_YUV420P | WB_F_NV12 | WB_F_FRAMES_ON_DEVICE | WB_F_FUSE_FILTERS)) == 0,
-          "flags may only hold WB_F_YUV420P, WB_F_NV12, WB_F_FRAMES_ON_DEVICE and WB_F_FUSE_FILTERS");
+  REQUIRE((flags & ~(WB_F_YUV420P | WB_F_NV12 | WB_F_YUYV422 | WB_F_UYVY422 | WB_F_FRAMES_ON_DEVICE |
+                     WB_F_FUSE_FILTERS)) == 0,
+          "flags may only hold WB_F_YUV420P, WB_F_NV12, WB_F_YUYV422, WB_F_UYVY422, WB_F_FRAMES_ON_DEVICE and "
+          "WB_F_FUSE_FILTERS");
   StageHook h(c, n);
   if (h.rc) return h.rc;
   Slot& s = h.s;
   cudaStream_t st = h.st;
-  const int fmt = pixel_format(flags & WB_F_YUV420P, flags & WB_F_NV12);
-  REQUIRE(fmt >= 0, "WB_F_YUV420P and WB_F_NV12 are mutually exclusive");
+  std::string err;
+  const int fmt = pixel_format(flags, kFrameFormats, err);
+  REQUIRE(fmt >= 0, err);
   int ni = n;
   if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &ni)) return rc;
   if (stop_layer >= 0) {

@@ -1,14 +1,18 @@
-// yuv420.cuh -- 4:2:0 frames (what video decoders emit) converted to the RGB24 bytes the kernels read, and RGB24
-// pixels converted to the 4:2:0 frames the effects pass can write for an encoder.
+// yuv420.cuh -- YUV frames (what video decoders and capture devices emit) converted to the RGB24 bytes the kernels
+// read, and RGB24 pixels converted to the 4:2:0 frames the effects pass can write for an encoder.
 //
 // A 4:2:0 frame of w x h pixels (w, h even) is packed in w*h*3/2 bytes: the full-resolution luma plane, then the
-// chroma at half resolution in both directions.  The two layouts differ only in where the chroma lives, which
-// ChromaLayout holds as data:
+// chroma at half resolution in both directions.  A packed 4:2:2 frame (w even, any h) is [h][w][2] bytes: each pair of
+// pixels (2k, 2k+1) of a row shares one 4-byte macropixel, and every row has its own chroma.  The layouts differ only
+// in where the samples live, which ChromaLayout holds as data:
 //   yuv420p (ffmpeg's software decoders): U plane [h/2][w/2], then V plane [h/2][w/2]
 //   NV12 (NVDEC): one plane [h/2][w/2] of interleaved (U, V) pairs
+//   YUYV (ffmpeg yuyv422, UVC webcams): macropixel Y0 U Y1 V
+//   UYVY (ffmpeg uyvy422, HDMI / SDI capture cards): macropixel U Y0 V Y1
 // The arithmetic is BT.601 limited range in 20-bit fixed point, which equals cv2.cvtColor(COLOR_YUV2RGB_I420 /
-// COLOR_YUV2RGB_NV12) on every (Y, U, V) triple (tests/test_yuv_host.py, tests/test_gpu_yuv.py).  Integer only, so
-// the result does not depend on the file's -fmad setting.
+// COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_YUYV / COLOR_YUV2RGB_UYVY) on every (Y, U, V) triple (tests/test_yuv_host.py,
+// tests/test_yuv422_host.py and their GPU counterparts).  Integer only, so the result does not depend on the file's
+// -fmad setting.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -16,36 +20,57 @@
 #define WB_FMT_RGB24 0
 #define WB_FMT_YUV420P 1
 #define WB_FMT_NV12 2
+#define WB_FMT_YUYV422 3
+#define WB_FMT_UYVY422 4
+
+__host__ __device__ __forceinline__ bool fmt_422(int fmt) { return fmt == WB_FMT_YUYV422 || fmt == WB_FMT_UYVY422; }
 
 struct ChromaLayout {
-  int step;      // bytes between horizontally adjacent U samples
-  int row;       // bytes between chroma rows
-  size_t v_off;  // V sample = U sample + v_off
+  int luma_step;  // bytes between horizontally adjacent Y samples: 1 (4:2:0 luma plane), 2 (4:2:2 macropixels)
+  int step;       // bytes between horizontally adjacent U samples
+  int row;        // bytes between chroma rows
+  int row_shift;  // luma row y has chroma row y >> row_shift: 1 (4:2:0, one per two luma rows), 0 (4:2:2, one per row)
+  size_t v_off;   // V sample = U sample + v_off
 };
 
+// the layout of a YUV frame, or of a window of one, whose luma rows are `pitch` bytes apart; v_off is only read for
+// yuv420p, where it is the parent frame's (w/2) * (h/2)
+__host__ __device__ __forceinline__ ChromaLayout chroma_layout_of(int fmt, int pitch, size_t v_off) {
+  if (fmt_422(fmt)) return ChromaLayout{2, 4, pitch, 0, 2};
+  if (fmt == WB_FMT_NV12) return ChromaLayout{1, 2, pitch, 1, 1};
+  return ChromaLayout{1, 1, pitch / 2, 1, v_off};
+}
+
+// the layout of a packed w x h frame
 __host__ __device__ __forceinline__ ChromaLayout chroma_layout(int fmt, int w, int h) {
-  if (fmt == WB_FMT_NV12) return ChromaLayout{2, w, 1};
-  return ChromaLayout{1, w / 2, (size_t)(w / 2) * (h / 2)};
+  return chroma_layout_of(fmt, fmt_422(fmt) ? 2 * w : w, (size_t)(w / 2) * (h / 2));
+}
+
+// byte offsets, from the first byte of a packed w x h frame, of the Y and the U sample of pixel (0, 0)
+__host__ __device__ __forceinline__ size_t luma_origin(int fmt) { return fmt == WB_FMT_UYVY422 ? 1 : 0; }
+__host__ __device__ __forceinline__ size_t chroma_origin(int fmt, int w, int h) {
+  return fmt == WB_FMT_YUYV422 ? 1 : fmt == WB_FMT_UYVY422 ? 0 : (size_t)w * h;
 }
 
 // bytes of one packed frame
 __host__ __device__ __forceinline__ size_t frame_bytes(int fmt, int w, int h) {
-  return fmt == WB_FMT_RGB24 ? (size_t)w * h * 3 : (size_t)w * h * 3 / 2;
+  return fmt == WB_FMT_RGB24 ? (size_t)w * h * 3 : fmt_422(fmt) ? (size_t)w * h * 2 : (size_t)w * h * 3 / 2;
 }
 
 // address of the U sample of pixel (x, y) given that of pixel (0, 0); the V sample is at + v_off.  A window of a frame
-// (x0, y0 even) has its own origin `chroma` and keeps the parent frame's layout.  T: uint8_t or const uint8_t.
+// (x0 even, and y0 even for 4:2:0) has its own origin `chroma` and keeps the parent frame's layout.  T: uint8_t or
+// const uint8_t.
 template <typename T>
 __device__ __forceinline__ T* chroma_ptr(T* chroma, const ChromaLayout& cl, int x, int y) {
-  return chroma + (size_t)(y >> 1) * cl.row + (size_t)(x >> 1) * cl.step;
+  return chroma + (size_t)(y >> cl.row_shift) * cl.row + (size_t)(x >> 1) * cl.step;
 }
 
 // Y, U, V bytes of pixel (x, y) of the frame whose luma rows start at `luma`, `pitch` bytes apart; yuv_to_rgb below
 // converts them (two halves, so that a caller can have the loads of several pixels in flight before it converts any)
-__device__ __forceinline__ void yuv420_load(const uint8_t* __restrict__ luma, int pitch, const uint8_t* __restrict__ chroma,
-                                            const ChromaLayout& cl, int x, int y, uint32_t& Y, uint32_t& U, uint32_t& V) {
+__device__ __forceinline__ void yuv_load(const uint8_t* __restrict__ luma, int pitch, const uint8_t* __restrict__ chroma,
+                                         const ChromaLayout& cl, int x, int y, uint32_t& Y, uint32_t& U, uint32_t& V) {
   const uint8_t* c = chroma_ptr(chroma, cl, x, y);
-  Y = __ldg(luma + (size_t)y * pitch + x);
+  Y = __ldg(luma + (size_t)y * pitch + (size_t)x * cl.luma_step);
   U = __ldg(c);
   V = __ldg(c + cl.v_off);
 }

@@ -20,7 +20,8 @@ PRECISION_FP32, PRECISION_BF16_TC = PRECISIONS['fp32'], PRECISIONS['bf16']
 PRECISION_TF32X3, PRECISION_FP16_TC = PRECISIONS['tf32x3'], PRECISIONS['fp16']
 
 # frame layouts the hot path reads, by ffmpeg's -pix_fmt names -> wb_detect / wb_submit flag
-PIXEL_FORMATS = {'rgb24': 0, 'yuv420p': _lib.WB_F_YUV420P, 'nv12': _lib.WB_F_NV12}
+PIXEL_FORMATS = {'rgb24': 0, 'yuv420p': _lib.WB_F_YUV420P, 'nv12': _lib.WB_F_NV12,
+                 'yuyv422': _lib.WB_F_YUYV422, 'uyvy422': _lib.WB_F_UYVY422}
 
 
 def _check_format(pixel_format):
@@ -30,11 +31,16 @@ def _check_format(pixel_format):
 
 def frame_shape(pixel_format, width, height):
     """numpy shape of one packed uint8 frame of a `width` x `height` camera: (H, W, 3) for rgb24, (H*3//2, W) for the
-    4:2:0 formats (luma plane, then the chroma; include/watsor_b200.h), which need an even width and height.  The same
-    shapes hold for the frames the effects pass reads and writes (output.effects, `output_format`)."""
+    4:2:0 formats (luma plane, then the chroma; include/watsor_b200.h), which need an even width and height, and
+    (H, W, 2) for the packed 4:2:2 formats (the shape cv2.cvtColor takes), which need an even width.  The same shapes
+    hold for the frames the effects pass reads and writes (output.effects, `output_format`)."""
     _check_format(pixel_format)
     if pixel_format == 'rgb24':
         return (height, width, 3)
+    if pixel_format in ('yuyv422', 'uyvy422'):
+        if width % 2:
+            raise ValueError('%s frames need an even width; the camera is %dx%d' % (pixel_format, width, height))
+        return (height, width, 2)
     if width % 2 or height % 2:
         raise ValueError('%s frames need an even width and height; the camera is %dx%d' % (pixel_format, width, height))
     return (height * 3 // 2, width)
@@ -186,7 +192,7 @@ class Engine:
 
     def detect(self, frames, cam_ids, out, verdicts=None, flags=0, pixel_format='rgb24'):
         """frames: host uint8 arrays (or device pointers with WB_F_FRAMES_ON_DEVICE) in `pixel_format`
-        ('rgb24', 'yuv420p' or 'nv12', see frame_shape); out: per frame a `Detection*100` ctypes array / address.
+        ('rgb24', 'yuv420p', 'nv12', 'yuyv422' or 'uyvy422', see frame_shape); out: per frame a `Detection*100` ctypes array / address.
         Returns device ms."""
         flags |= self._format_flags(frames, cam_ids, pixel_format)
         n, fp, cams, op, vp = self._io(frames, cam_ids, out, verdicts)

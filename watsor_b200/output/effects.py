@@ -26,7 +26,9 @@ from .font import FontAtlas
 WB_FX_BLEND, WB_FX_DRAW, WB_FX_CONTOURS, WB_FX_ON_DEVICE = 1, 2, 4, 8
 WB_FX_YUV420P, WB_FX_NV12 = 16, 32
 WB_FX_OUT_YUV420P, WB_FX_OUT_NV12 = 64, 128
-_FX_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_YUV420P, 'nv12': WB_FX_NV12}
+WB_FX_YUYV422, WB_FX_UYVY422 = 256, 512
+_FX_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_YUV420P, 'nv12': WB_FX_NV12, 'yuyv422': WB_FX_YUYV422,
+               'uyvy422': WB_FX_UYVY422}
 _FX_OUT_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_OUT_YUV420P, 'nv12': WB_FX_OUT_NV12}
 
 
@@ -38,6 +40,12 @@ class _Font(Structure):
 
 class _Label(Structure):
     _fields_ = [('box_color', c_uint8 * 3), ('n_prefix', c_uint8), ('prefix', c_uint8 * 60)]
+
+
+def _check_output_format(output_format):
+    # 4:2:2 is an input format only: OpenCV's RGB -> 4:2:2 arithmetic is not the I420 one the kernel restates
+    if output_format not in _FX_OUT_FORMATS:
+        raise ValueError('output_format must be one of %s, not %r' % (', '.join(_FX_OUT_FORMATS), output_format))
 
 
 def _check(rc):
@@ -128,11 +136,12 @@ class EffectsEngine:
 
     def render(self, images_in, images_out, cam_ids, rows, flags, pixel_format='rgb24', output_format='rgb24'):
         """images: uint8 arrays (or device pointers with WB_FX_ON_DEVICE); rows: per frame the `Detection * 100`
-        array of a frame header (or its address).  pixel_format: layout of images_in, 'rgb24' or a 4:2:0 layout
-        'yuv420p' / 'nv12' (converted as cv2.cvtColor does; see engine.frame_shape).  output_format: layout of
-        images_out, 'rgb24' or 'yuv420p' / 'nv12' for an encoder that takes 4:2:0 (the rendered frame converted as
-        cv2.cvtColor(COLOR_RGB2YUV_I420) does).  With either side 4:2:0, images_out must be other buffers than
-        images_in."""
+        array of a frame header (or its address).  pixel_format: layout of images_in, 'rgb24', a 4:2:0 layout
+        'yuv420p' / 'nv12' or a packed 4:2:2 layout 'yuyv422' / 'uyvy422' (converted as cv2.cvtColor does; see
+        engine.frame_shape).  output_format: layout of images_out, 'rgb24' or 'yuv420p' / 'nv12' for an encoder that
+        takes 4:2:0 (the rendered frame converted as cv2.cvtColor(COLOR_RGB2YUV_I420) does).  With either side in a YUV
+        format, images_out must be other buffers than images_in."""
+        _check_output_format(output_format)
         sizes = [self._sizes.get(c) for c in cam_ids]
         check_frames(images_in, sizes, pixel_format)
         if output_format != 'rgb24':
@@ -263,7 +272,8 @@ class FusedEffects(_Effect):
 
     def __init__(self, camera_config, engine=None, output_format='rgb24'):
         super().__init__(engine)
-        frame_shape(output_format, camera_config['width'], camera_config['height'])   # a known format, even sizes
+        _check_output_format(output_format)
+        frame_shape(output_format, camera_config['width'], camera_config['height'])   # even sizes
         self.output_format = output_format
         if 'mask' in camera_config:
             alpha, cont = _camera_tables(camera_config, True, True)
@@ -285,4 +295,5 @@ def new_rows():
 
 __all__ = ['EffectsEngine', 'CopyHeaderEffect', 'CopyImageEffect', 'BlendEffect', 'DrawEffect',
            'DrawEffectWithContours', 'FusedEffects', 'contour_bits', 'new_rows', 'WB_FX_BLEND', 'WB_FX_DRAW',
-           'WB_FX_CONTOURS', 'WB_FX_ON_DEVICE', 'WB_FX_YUV420P', 'WB_FX_NV12', 'WB_FX_OUT_YUV420P', 'WB_FX_OUT_NV12']
+           'WB_FX_CONTOURS', 'WB_FX_ON_DEVICE', 'WB_FX_YUV420P', 'WB_FX_NV12', 'WB_FX_OUT_YUV420P', 'WB_FX_OUT_NV12',
+           'WB_FX_YUYV422', 'WB_FX_UYVY422']

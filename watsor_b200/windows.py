@@ -9,13 +9,14 @@ import math
 from ._lib import WB_MAX_WINDOWS
 
 FOUR_TWO_ZERO = ('yuv420p', 'nv12')
+FOUR_TWO_TWO = ('yuyv422', 'uyvy422')
 
 
 def grid_windows(width, height, cols, rows, overlap=0.25, full_frame=True, align=2):
     """[(x, y, w, h), ...]: the whole frame first (unless `full_frame` is False), then a `cols` x `rows` grid of windows
     that cover the frame, neighbours overlapping by at least `overlap` of a window's size (less at most `align` px).
     Origins and sizes are multiples of `align` wherever the frame's size allows (an odd frame size leaves the last
-    window of a row or column odd), so align=2 suits the 4:2:0 formats."""
+    window of a row or column odd), so align=2 suits the 4:2:0 and 4:2:2 formats."""
     if cols < 1 or rows < 1 or not 0 <= overlap < 1 or align < 1:
         raise ValueError('need cols, rows >= 1, 0 <= overlap < 1 and align >= 1')
 
@@ -37,7 +38,8 @@ def grid_windows(width, height, cols, rows, overlap=0.25, full_frame=True, align
 
 def check_windows(windows, width, height, pixel_format='rgb24'):
     """Raises ValueError unless `windows` is a list of at most WB_MAX_WINDOWS (x, y, w, h) integer rectangles with
-    w, h >= 1 inside a `width` x `height` frame, with even origins and sizes for the 4:2:0 formats."""
+    w, h >= 1 inside a `width` x `height` frame, with even origins and sizes for the 4:2:0 formats and an even x and w
+    for the 4:2:2 formats (their chroma is shared by pixel pairs of a row only)."""
     windows = list(windows)
     if len(windows) > WB_MAX_WINDOWS:
         raise ValueError('a camera may have at most %d detection windows, not %d' % (WB_MAX_WINDOWS, len(windows)))
@@ -52,4 +54,6 @@ def check_windows(windows, width, height, pixel_format='rgb24'):
         if pixel_format in FOUR_TWO_ZERO and (x % 2 or y % 2 or w % 2 or h % 2):
             raise ValueError('window %d %r: %s frames need an even window origin, width and height'
                              % (i, tuple(win), pixel_format))
+        if pixel_format in FOUR_TWO_TWO and (x % 2 or w % 2):
+            raise ValueError('window %d %r: %s frames need an even window x and width' % (i, tuple(win), pixel_format))
     return [tuple(int(v) for v in win) for win in windows]
