@@ -139,9 +139,15 @@ def _point_in_polygon(x, y, P, Q):
 def rect_intersects_polygon(x0, y0, x1, y1, poly):
     """closed rect (corners as given in mask.py:45-48) vs closed polygon region."""
     P = np.asarray(poly, dtype=np.int64).reshape(-1, 2)
+    if max(abs(int(v)) for v in (x0, y0, x1, y1)) >= 2 ** 30:
+        # int32 corners: the orientation products of a rectangle edge reach 2^64, so compute in Python integers
+        P = P.astype(object)
+        x0, y0, x1, y1 = (int(v) for v in (x0, y0, x1, y1))
     Q = np.roll(P, -1, axis=0)
     xa, xb = min(x0, x1), max(x0, x1)
     ya, yb = min(y0, y1), max(y0, y1)
+    if xb < P[:, 0].min() or xa > P[:, 0].max() or yb < P[:, 1].min() or ya > P[:, 1].max():
+        return False                          # disjoint from the polygon's bounding box
     inside = (P[:, 0] >= xa) & (P[:, 0] <= xb) & (P[:, 1] >= ya) & (P[:, 1] <= yb)
     if inside.any():
         return True

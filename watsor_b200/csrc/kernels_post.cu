@@ -342,6 +342,19 @@ __device__ __forceinline__ int sat_count(const int32_t* s, int W1, int x0, int y
          s[(size_t)y0 * W1 + x0];
 }
 
+// abs((x1 - x0 + 1) * (y1 - y0 + 1)) >= thr for any int32 corners, compared as Python compares an int with a float:
+// exactly.  Each span is taken in 64 bits and is at most 2^32, so the area is at most 2^64: it overflows 64 bits only
+// when both spans are 2^32, and then 2^64 >= thr is decided on its own.
+__device__ __forceinline__ bool area_at_least(int x0, int y0, int x1, int y1, double thr) {
+  const long long sx = (long long)x1 - x0 + 1, sy = (long long)y1 - y0 + 1;
+  const unsigned long long ax = (unsigned long long)(sx < 0 ? -sx : sx), ay = (unsigned long long)(sy < 0 ? -sy : sy);
+  if (thr <= 0.0) return true;
+  if (!(thr <= 18446744073709551616.0)) return false;  // above 2^64, or NaN
+  const double c = ceil(thr);                          // an integer area is >= thr iff it is >= ceil(thr)
+  if (c == 18446744073709551616.0) return ax == (1ull << 32) && ay == (1ull << 32);
+  return __umul64hi(ax, ay) != 0ull || ax * ay >= (unsigned long long)c;
+}
+
 // The lazily evaluated predicate chain of watsor/filter/track.py:26.
 __device__ uint32_t apply_filters(const CameraCfg* __restrict__ cam, wb_detection* d, bool write_zones) {
   uint32_t v = 0;
@@ -366,14 +379,13 @@ __device__ uint32_t apply_filters(const CameraCfg* __restrict__ cam, wb_detectio
   } else {
     return v;  // confidence.py:18 / area.py:21: `... is not None and ...`
   }
-  // confidence.py:17-19
-  if (!(d->confidence >= conf_thr)) return v;
+  // confidence.py:17-19.  A -inf threshold is no confidence predicate: the stand-alone AreaFilter / MaskFilter tables
+  // (area.py and mask.py never read the confidence, so a NaN confidence passes them)
+  if (conf_thr != -INFINITY && !(d->confidence >= conf_thr)) return v;
   v |= WB_V_CONFIDENCE;
   // area.py:20-26  abs((x_max - x_min + 1) * (y_max - y_min + 1)) >= pct/100 * W*H
   const wb_bounding_box bb = d->bounding_box;
-  long long a = (long long)(bb.x_max - bb.x_min + 1) * (long long)(bb.y_max - bb.y_min + 1);
-  if (a < 0) a = -a;
-  if (!((double)a >= area_thr)) return v;
+  if (!area_at_least(bb.x_min, bb.y_min, bb.x_max, bb.y_max, area_thr)) return v;
   v |= WB_V_AREA;
   if (cam->has_mask) {
     // mask.py:44-59: closed bbox rectangle intersects zone polygon  <=>  it covers >= 1 pixel of the
@@ -632,7 +644,7 @@ __global__ void __launch_bounds__(WM_THREADS)
         lab = d.label;
         b = make_int4(d.bounding_box.x_min + wf.x[w], d.bounding_box.y_min + wf.y[w], d.bounding_box.x_max + wf.x[w],
                       d.bounding_box.y_max + wf.y[w]);
-        area = (long long)(b.z - b.x + 1) * (long long)(b.w - b.y + 1);
+        area = ((long long)b.z - b.x + 1) * ((long long)b.w - b.y + 1);
       }
       for (int t = 0; t < cnt && nk < max_out; ++t) {
         const int tid = __shfl_sync(0xffffffffu, id, t), tlab = __shfl_sync(0xffffffffu, lab, t);

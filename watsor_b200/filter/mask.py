@@ -9,8 +9,14 @@ summed-area tables in HBM, and "bounding box intersects zone polygon" (mask.py:5
 same predicate because contour vertices are pixel centres joined by 8-connected unit steps
 (DESIGN.md section 5; tests/test_oracle_filters.py::test_raster_sat_equals_exact_polygon_intersection checks the raster /
 summed-area form against exact integer geometry on porch.png and random masks with holes and islands, including
-zero-width / zero-height boxes).  Not covered: GEOS' treatment of invalid self-touching rings from 1-pixel-wide zones
-(shapely is not installable here).  One visible difference from the reference: the fused detector path
+zero-width / zero-height boxes; tests/test_zone_masks_host.py checks it on 32-zone grids of rectangles, ellipses and
+45-degree diamonds at 640x480, 1920x1080 and 3840x2160, zones on every frame edge and corner, single-pixel-wide L shapes
+and bars, staircases, 2-pixel 45-degree bands, two blocks joined only through a diagonal pixel (findContours makes them
+one zone whose ring touches itself) and zones with equal centroid keys, each with edge boxes on every corner and
+outside the frame).  The claim held on every family, so no kind of zone is refused beyond what the reference refuses.
+Not covered: GEOS' own treatment of invalid self-touching rings (1-pixel-wide parts, diagonal joins), which the exact
+integer geometry of oracle/filters.py stands in for.  Zones of fewer than 3 contour points have zero area and fail,
+as in the reference, in the centroid key (ZeroDivisionError) before the 3-point assertion is reached.  One visible difference from the reference: the fused detector path
 (`WB_F_FUSE_FILTERS`) clears `zones[]` of every row before judging it, whereas `TensorFlowObjectDetector.detect`
 never touches zones (ref:tensorflow_cpu.py:79-90; the reference's sieve works on a zeroed clone, sieve.py:24-27, so
 the published rows agree).
