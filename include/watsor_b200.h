@@ -136,8 +136,12 @@ int wb_unregister_host(wb_ctx* ctx, void* ptr);
  *               cvtColor makes.  With WB_F_YUYV422 or WB_F_UYVY422 a
  *               packed 4:2:2 frame [h][w][2]: each pixel pair (2k, 2k+1) of a row shares one macropixel, Y0 U Y1 V
  *               (YUYV) or U Y0 V Y1 (UYVY), and every row has its own chroma.  4:2:2 needs an even w (any h); its
- *               conversion equals COLOR_YUV2RGB_YUYV / COLOR_YUV2RGB_UYVY the same way.  The format is one per
- *               batch: at most one of the four format flags.
+ *               conversion equals COLOR_YUV2RGB_YUYV / COLOR_YUV2RGB_UYVY the same way.  With WB_F_BGR24 a
+ *               BGR24 frame [h][w][3] (OpenCV's order: cv2.VideoCapture, cv2.imread); with WB_F_RGBA / WB_F_BGRA a
+ *               4-byte frame [h][w][4], R G B A / B G R A (also rgb0 / bgr0: the fourth byte is not read).  These
+ *               are read as the RGB24 frame cv2.cvtColor(COLOR_BGR2RGB / COLOR_RGBA2RGB / COLOR_BGRA2RGB) makes,
+ *               so the rows equal that frame's; any size, any window.  The format is one per batch: at most one of
+ *               the seven format flags.
  *   out[i]      Detection[100] block of that frame's header (share.py:27-32); all 100 rows written
  *   verdicts[i] optional uint32[100] filter verdicts (NULL to skip)
  *   flags       WB_F_* below
@@ -153,6 +157,9 @@ int wb_unregister_host(wb_ctx* ctx, void* ptr);
 #define WB_F_NV12 16u            /* frames[] are NV12 (NVDEC's output, packed)                    */
 #define WB_F_YUYV422 32u         /* frames[] are YUYV 4:2:2 (ffmpeg yuyv422: UVC webcams)         */
 #define WB_F_UYVY422 64u         /* frames[] are UYVY 4:2:2 (ffmpeg uyvy422: HDMI / SDI capture)  */
+#define WB_F_BGR24 128u          /* frames[] are BGR24 [h][w][3] (OpenCV, ffmpeg bgr24)           */
+#define WB_F_RGBA 256u           /* frames[] are RGBA [h][w][4] (also rgb0; the A byte is ignored) */
+#define WB_F_BGRA 512u           /* frames[] are BGRA [h][w][4] (also bgr0; the A byte is ignored) */
 int wb_detect(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_t* cam_ids,
               uint32_t flags, wb_detection* const* out, uint32_t* const* verdicts, float* gpu_ms);
 
@@ -223,7 +230,11 @@ typedef struct wb_fx_label {      /* drawing attributes of one label index (conf
 #define WB_FX_OUT_YUV420P 64u /* images_out are yuv420p [h*3/2][w], for an encoder that takes 4:2:0 */
 #define WB_FX_OUT_NV12 128u   /* images_out are NV12 [h*3/2][w]; not with WB_FX_OUT_YUV420P */
 #define WB_FX_YUYV422 256u    /* images_in are YUYV 4:2:2 [h][w][2] (layouts as for wb_detect) */
-#define WB_FX_UYVY422 512u    /* images_in are UYVY 4:2:2 [h][w][2]; at most one input format flag is set */
+#define WB_FX_UYVY422 512u    /* images_in are UYVY 4:2:2 [h][w][2] */
+#define WB_FX_BGR24 1024u     /* images_in are BGR24 [h][w][3] */
+#define WB_FX_RGBA 2048u      /* images_in are RGBA [h][w][4] (also rgb0) */
+#define WB_FX_BGRA 4096u      /* images_in are BGRA [h][w][4] (also bgr0); at most one input format flag is set */
+#define WB_FX_OUT_BGR24 8192u /* images_out are BGR24 [h][w][3], for cv2.imencode; at most one output format flag */
 /* labels[0] is also the style of unknown label indices (coco.py:124-131); digit_glyphs = glyph indices of '0'..'9','%';
  * alpha = opacity of the label box (coco.py:119) */
 int wb_fx_create(int device, const wb_fx_font* font, int n_labels, const wb_fx_label* labels,
@@ -234,11 +245,15 @@ int wb_fx_set_camera(wb_fx* fx, int cam_id, int width, int height, const uint8_t
 /* rows[i]: the 100 Detection rows of frame i (host memory: header.detections).  images: RGB24, host pointers unless
  * WB_FX_ON_DEVICE.  With WB_FX_YUV420P / WB_FX_NV12 images_in are 4:2:0 (even width and height), converted as
  * cv2.cvtColor does; with WB_FX_YUYV422 / WB_FX_UYVY422 they are packed 4:2:2 (even width, any height),
- * converted the same way.  With WB_FX_OUT_YUV420P / WB_FX_OUT_NV12 images_out are 4:2:0 (even width and height), the
+ * converted the same way; with WB_FX_BGR24 / WB_FX_RGBA / WB_FX_BGRA they are BGR24 [h][w][3] or RGBA / BGRA
+ * [h][w][4] (alpha ignored: the blend alpha is the camera's), read as cv2.cvtColor's RGB24 of them.  With
+ * WB_FX_OUT_BGR24 images_out are BGR24, the rendered RGB24 frame with R and B swapped (cv2.cvtColor(COLOR_RGB2BGR)),
+ * which cv2.imencode takes as it is.  With WB_FX_OUT_YUV420P / WB_FX_OUT_NV12 images_out are 4:2:0 (even width and height), the
  * rendered RGB24 frame converted as cv2.cvtColor(COLOR_RGB2YUV_I420) does (U and V of a 2x2 block from its top-left
  * pixel; NV12 = the same bytes with U and V interleaved); host output then moves w*h*3/2 bytes per frame.  Any input
- * format goes with any output format and every effect flag.  With either side in a YUV format, images_out[i] must
- * not be images_in[i].  Without effect flags the call is a pure format converter.  gpu_ms: kernels only. */
+ * format goes with any output format and every effect flag.  images_out[i] may be images_in[i] only when both are
+ * RGB24 or BGR24 (the same pixel size, no YUV); otherwise it must be another buffer.  Without effect flags the call
+ * is a pure format converter.  gpu_ms: kernels only. */
 int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* const* images_out, const int32_t* cam_ids,
                  const wb_detection* const* rows, uint32_t flags, float* gpu_ms);
 int wb_fx_destroy(wb_fx* fx);
@@ -254,9 +269,10 @@ int wb_preprocess(wb_ctx* ctx, int n, const uint8_t* const* frames, const int32_
 int wb_backbone(wb_ctx* ctx, int n, const float* pre, float* enc, float* logits, int stop_layer,
                 float* layer_out, size_t layer_out_floats);
 /* the product path's own input handling (frames as wb_submit takes them: host or device, rgb24 / yuv420p / nv12 /
- * yuyv422 / uyvy422,
+ * yuyv422 / uyvy422 / bgr24 / rgba / bgra,
  * a camera's detection windows expanded into model images), run to stop_layer; n_images = model images of the batch.
- * flags: one format flag (WB_F_YUV420P, WB_F_NV12, WB_F_YUYV422, WB_F_UYVY422), WB_F_FRAMES_ON_DEVICE,
+ * flags: one format flag (WB_F_YUV420P, WB_F_NV12, WB_F_YUYV422, WB_F_UYVY422, WB_F_BGR24, WB_F_RGBA, WB_F_BGRA),
+ * WB_F_FRAMES_ON_DEVICE,
  * WB_F_FUSE_FILTERS.  Runs on slot 0.
  *   stop_layer >= 0: the layers up to stop_layer, eagerly; layer_out as for wb_backbone, for n_images images.
  *   stop_layer == -1: the kernels of wb_submit (CUDA graph, post stage, window merge).

@@ -11,6 +11,7 @@ LIB_PATH = os.path.join(_HERE, 'csrc', 'libwatsor_b200.so')
 WB_F_FRAMES_ON_DEVICE, WB_F_FUSE_FILTERS, WB_F_OUT_ON_DEVICE = 1, 2, 4
 WB_F_YUV420P, WB_F_NV12 = 8, 16
 WB_F_YUYV422, WB_F_UYVY422 = 32, 64
+WB_F_BGR24, WB_F_RGBA, WB_F_BGRA = 128, 256, 512
 WB_V_LABEL, WB_V_CONFIDENCE, WB_V_AREA, WB_V_MASK, WB_V_PASS = 1, 2, 4, 8, 16
 WB_CAM_NO_LABEL_CHECK = 1
 WB_MAX_WINDOWS = 16

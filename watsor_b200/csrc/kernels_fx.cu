@@ -211,7 +211,9 @@ constexpr int FX_TW = 128, FX_TH = 8;
 // (forcing 32 registers for 8 blocks per SM instead of 5 spills and measured 8 % slower)
 // YUV_OUT: the frames' out_fmt is yuv420p or NV12.  The RGB24 pass has an instantiation of its own because the 4:2:0
 // store, as a run-time branch, made it 0.8 % slower.
-template <bool YUV_OUT>
+// RGB_ORDERS: the input is BGR24, RGBA or BGRA, or the output is BGR24 (fx_rgb_orders).  Those byte orders have
+// instantiations of their own for the same reason, so the <false, false> pass compiles to what it was without them.
+template <bool YUV_OUT, bool RGB_ORDERS>
 __global__ void __launch_bounds__(256, 5)
     k_fx_render(const FxFrameDesc* __restrict__ frames, const FxFrame* __restrict__ prep, FxFont font,
                 const FxLabel* __restrict__ labels, const uint8_t* __restrict__ aw_lut, uint32_t flags) {
@@ -231,17 +233,23 @@ __global__ void __launch_bounds__(256, 5)
   const size_t row = (size_t)(live ? y : 0) * W;
   const int npx = live ? min(4, W - xb) : 0;
   const size_t px0 = row + (live ? xb : 0);
-  const bool yuv = fd.fmt != WB_FMT_RGB24;
-  const uint8_t* src = fd.in + px0 * 3;  // RGB24 pixels (a YUV frame's samples are addressed below)
+  const bool yuv = RGB_ORDERS ? !fmt_rgb(fd.fmt) : fd.fmt != WB_FMT_RGB24;
+  // the packed RGB input's byte order (rgb_layout: G is byte 1 of every order, R and B bytes 0 and 2)
+  const RgbLayout il = rgb_layout(RGB_ORDERS ? fd.fmt : WB_FMT_RGB24);
+  const bool quad = RGB_ORDERS && !yuv && il.bpp == 4;  // RGBA / BGRA input
+  const uint8_t* src = fd.in + px0 * (quad ? 4 : 3);  // RGB pixels (a YUV frame's samples are addressed below)
   const bool rgb_out = !YUV_OUT;
-  uint8_t* dst = fd.out + px0 * (rgb_out ? 3 : 1);  // RGB24 pixels, or the luma of a 4:2:0 frame
+  uint8_t* dst = fd.out + px0 * (rgb_out ? 3 : 1);  // RGB24 / BGR24 pixels, or the luma of a 4:2:0 frame
   const bool blend = (flags & WB_FX_BLEND) && fd.cam.alpha != nullptr;
   const bool outline = (flags & WB_FX_CONTOURS) && fd.cam.contours != nullptr;
-  // RGB24 loads and stores are whole words when every 4-pixel group of the thread's input and output is aligned
-  const bool vec = npx == 4 && (((yuv ? 0 : reinterpret_cast<uintptr_t>(src)) |
+  // 3-byte loads and stores are whole words when every 4-pixel group of the thread's input and output is aligned
+  const bool vec = npx == 4 && (((yuv || quad ? 0 : reinterpret_cast<uintptr_t>(src)) |
                                  (rgb_out ? reinterpret_cast<uintptr_t>(dst) : 0)) & 3) == 0;
+  // 4-byte input: the 16 bytes of the thread's pixels are one uint4 when they are 16-byte aligned
+  const bool vec4 = quad && npx == 4 && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
   // ---- loads first
-  uint32_t ws[3] = {0u, 0u, 0u};  // RGB24: the 12 bytes; YUV: 4 Y bytes, then U and V of the 2 chroma samples
+  // RGB24 / BGR24: the 12 bytes; RGBA / BGRA: the 16 bytes; YUV: 4 Y bytes, then U and V of the 2 chroma samples
+  uint32_t ws[RGB_ORDERS ? 4 : 3] = {0u, 0u, 0u};
   uint8_t v[4][3];
   uint8_t al[4] = {255, 255, 255, 255};
   uint32_t cb[4] = {0u, 0u, 0u, 0u};
@@ -264,6 +272,21 @@ __global__ void __launch_bounds__(256, 5)
       load(chroma_layout(WB_FMT_YUYV422, W, H), fd.in + luma_origin(fd.fmt), fd.in + chroma_origin(fd.fmt, W, H));
     } else {
       load(chroma_layout(fd.fmt == WB_FMT_NV12 ? WB_FMT_NV12 : WB_FMT_YUV420P, W, H), fd.in, fd.in + (size_t)W * H);
+    }
+  } else if (quad) {
+    if (vec4) {
+      const uint4 q = __ldg(reinterpret_cast<const uint4*>(src));
+      ws[0] = q.x;
+      ws[1] = q.y;
+      ws[2] = q.z;
+      ws[RGB_ORDERS ? 3 : 0] = q.w;
+    } else {
+#pragma unroll
+      for (int p = 0; p < 4; ++p)
+        if (p < npx) {
+#pragma unroll
+          for (int c = 0; c < 3; ++c) v[p][c] = __ldg(src + p * 4 + c);
+        }
     }
   } else if (vec) {
     const uint32_t* s32 = reinterpret_cast<const uint32_t*>(src);
@@ -345,9 +368,23 @@ __global__ void __launch_bounds__(256, 5)
       v[p][1] = (uint8_t)g;
       v[p][2] = (uint8_t)b;
     }
-  } else if (vec) {
+  } else if (vec4) {
+#pragma unroll
+    for (int p = 0; p < 4; ++p)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[p][c] = (uint8_t)(ws[RGB_ORDERS ? p : 0] >> (8 * c));
+  } else if (vec && !quad) {
 #pragma unroll
     for (int i = 0; i < 12; ++i) v[i / 3][i % 3] = (uint8_t)(ws[i >> 2] >> (8 * (i & 3)));
+  }
+  // BGR24 / BGRA input: v holds bytes 0, 1, 2 of each pixel; R is byte 2
+  if (RGB_ORDERS && !yuv && il.r == 2) {
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      const uint8_t t = v[p][0];
+      v[p][0] = v[p][2];
+      v[p][2] = t;
+    }
   }
   // CopyImageEffect / BlendEffect
   if (blend) {
@@ -413,6 +450,15 @@ __global__ void __launch_bounds__(256, 5)
         v[p][1] = 255;
         v[p][2] = 0;
       }
+  }
+  // BGR24 output: the RGB24 result with R and B swapped, stored as RGB24 is
+  if (RGB_ORDERS && rgb_out && rgb_layout(fd.out_fmt).r == 2) {
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      const uint8_t t = v[p][0];
+      v[p][0] = v[p][2];
+      v[p][2] = t;
+    }
   }
   if (!rgb_out) {
     // 4:2:0 as cv2.cvtColor(COLOR_RGB2YUV_I420) computes it: Y of every pixel; U and V of a 2x2 block from its top-left
@@ -593,15 +639,27 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   static const FormatFlag in_formats[] = {{WB_FX_YUV420P, WB_FMT_YUV420P, "WB_FX_YUV420P"},
                                           {WB_FX_NV12, WB_FMT_NV12, "WB_FX_NV12"},
                                           {WB_FX_YUYV422, WB_FMT_YUYV422, "WB_FX_YUYV422"},
-                                          {WB_FX_UYVY422, WB_FMT_UYVY422, "WB_FX_UYVY422"}};
+                                          {WB_FX_UYVY422, WB_FMT_UYVY422, "WB_FX_UYVY422"},
+                                          {WB_FX_BGR24, WB_FMT_BGR24, "WB_FX_BGR24"},
+                                          {WB_FX_RGBA, WB_FMT_RGBA, "WB_FX_RGBA"},
+                                          {WB_FX_BGRA, WB_FMT_BGRA, "WB_FX_BGRA"}};
   static const FormatFlag out_formats[] = {{WB_FX_OUT_YUV420P, WB_FMT_YUV420P, "WB_FX_OUT_YUV420P"},
-                                           {WB_FX_OUT_NV12, WB_FMT_NV12, "WB_FX_OUT_NV12"}};
+                                           {WB_FX_OUT_NV12, WB_FMT_NV12, "WB_FX_OUT_NV12"},
+                                           {WB_FX_OUT_BGR24, WB_FMT_BGR24, "WB_FX_OUT_BGR24"}};
   std::string err;
   const int fmt = pixel_format(flags, in_formats, err);
   REQUIRE(fmt >= 0, err);
   const int out_fmt = pixel_format(flags, out_formats, err);
   REQUIRE(out_fmt >= 0, err);
-  const bool yuv420 = fmt == WB_FMT_YUV420P || fmt == WB_FMT_NV12 || out_fmt != WB_FMT_RGB24;
+  const bool yuv420 = fmt == WB_FMT_YUV420P || fmt == WB_FMT_NV12 || !fmt_rgb(out_fmt);
+  // in place only between packed RGB layouts of one pixel size: a thread then writes exactly the bytes it read
+  const bool in_place_ok = fmt_rgb(fmt) && fmt_rgb(out_fmt) && rgb_layout(fmt).bpp == rgb_layout(out_fmt).bpp;
+  // the BGR24 / RGBA / BGRA passes are instantiations of their own (k_fx_render)
+  const bool rgb_orders = (fmt_rgb(fmt) && fmt != WB_FMT_RGB24) || out_fmt == WB_FMT_BGR24;
+  // host staging: one slot per frame, 256-byte aligned, of the RGB24 output's size or the input's if that is larger
+  auto slot_bytes = [&](const FxCamera& cam) {
+    return (std::max((size_t)cam.w * cam.h * 3, frame_bytes(fmt, cam.w, cam.h)) + 255) / 256 * 256;
+  };
   size_t total = 0;
   int max_w = 0, max_h = 0;
   for (int i = 0; i < n; ++i) {
@@ -609,23 +667,24 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
     REQUIRE(it != fx->cams.end(), "cam_id " + std::to_string(cam_ids[i]) + " has not been configured with wb_fx_set_camera");
     REQUIRE(images_in[i] && images_out[i] && rows[i], "NULL frame / rows pointer");
     const FxCamera& cam = it->second.view;
-    if (fmt != WB_FMT_RGB24 || out_fmt != WB_FMT_RGB24) {
-      const std::string size = "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(cam.w) + "x" +
-                               std::to_string(cam.h);
-      REQUIRE(!yuv420 || (cam.w % 2 == 0 && cam.h % 2 == 0), size + ": 4:2:0 frames need an even width and height");
-      REQUIRE(cam.w % 2 == 0, size + ": 4:2:2 frames need an even width");
-      // in place, the stores of some threads would overwrite bytes that others still read
-      REQUIRE(images_in[i] != images_out[i],
-              std::string(fmt_422(fmt) ? "4:2:2 input" : fmt != WB_FMT_RGB24 ? "4:2:0 input" : "4:2:0 output") +
-                  " cannot be rendered in place: images_out must be another buffer (cam_id " +
-                  std::to_string(cam_ids[i]) + ")");
-    }
+    const std::string size = "cam_id " + std::to_string(cam_ids[i]) + " is " + std::to_string(cam.w) + "x" +
+                             std::to_string(cam.h);
+    REQUIRE(!yuv420 || (cam.w % 2 == 0 && cam.h % 2 == 0), size + ": 4:2:0 frames need an even width and height");
+    REQUIRE(!fmt_422(fmt) || cam.w % 2 == 0, size + ": 4:2:2 frames need an even width");
+    // in place, the stores of some threads would overwrite bytes that others still read
+    REQUIRE(in_place_ok || images_in[i] != images_out[i],
+            std::string(fmt_422(fmt)             ? "4:2:2 input"
+                        : !fmt_rgb(fmt)          ? "4:2:0 input"
+                        : !fmt_rgb(out_fmt)      ? "4:2:0 output"
+                                                 : "input and output of different pixel sizes") +
+                " cannot be rendered in place: images_out must be another buffer (cam_id " +
+                std::to_string(cam_ids[i]) + ", " + fmt_name(fmt) + " input, " + fmt_name(out_fmt) + " output)");
     // labels are placed inside the frame only if it is high enough for one above/below/inside a box (draw.py:68-73);
     // lower frames would need OpenCV's re-capping of strokes cut by the bottom border, which the tables do not hold
     const int min_h = 2 * (fx->font.text_height + 2 * fx->font.margin + fx->font.baseline) + 1;
     REQUIRE(!(flags & WB_FX_DRAW) || cam.h >= min_h,
             "the draw effect needs frames of at least " + std::to_string(min_h) + " rows");
-    total += ((size_t)cam.w * cam.h * 3 + 255) / 256 * 256;
+    total += slot_bytes(cam);
     max_w = std::max(max_w, cam.w);
     max_h = std::max(max_h, cam.h);
   }
@@ -651,7 +710,6 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   size_t off = 0;
   for (int i = 0; i < n; ++i) {
     const FxCamera& cam = fx->cams[cam_ids[i]].view;
-    const size_t bytes = (size_t)cam.w * cam.h * 3;  // staging slot: the RGB24 output, at least the input
     memcpy(fx->h_rows + (size_t)i * WB_MAX_DETECTIONS, rows[i], sizeof(wb_detection) * WB_MAX_DETECTIONS);
     FxFrameDesc d;
     d.cam = cam;
@@ -666,7 +724,7 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
       d.out = fx->d_out + off;
     }
     fx->h_desc[i] = d;
-    off += (bytes + 255) / 256 * 256;
+    off += slot_bytes(cam);
   }
   CK(cudaMemcpyAsync(fx->d_rows, fx->h_rows, sizeof(wb_detection) * WB_MAX_DETECTIONS * n, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(fx->d_desc, fx->h_desc, sizeof(FxFrameDesc) * n, cudaMemcpyHostToDevice, st));
@@ -674,10 +732,15 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
   if (flags & WB_FX_DRAW)
     k_fx_prepare<<<n, 128, 0, st>>>(fx->d_rows, fx->d_desc, fx->font, fx->d_labels, fx->n_labels, fx->d_digits, fx->d_prep);
   dim3 grid((max_w + FX_TW - 1) / FX_TW, (max_h + FX_TH - 1) / FX_TH, n);
-  if (out_fmt == WB_FMT_RGB24)
-    k_fx_render<false><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
+  const bool yuv_out = !fmt_rgb(out_fmt);
+  if (!rgb_orders && !yuv_out)
+    k_fx_render<false, false><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
+  else if (!rgb_orders)
+    k_fx_render<true, false><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
+  else if (!yuv_out)
+    k_fx_render<false, true><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
   else
-    k_fx_render<true><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
+    k_fx_render<true, true><<<grid, 256, 0, st>>>(fx->d_desc, fx->d_prep, fx->font, fx->d_labels, fx->d_aw, flags);
   CK(cudaGetLastError());
   CK(cudaEventRecord(fx->ev1, st));
   if (!on_device) {
@@ -685,7 +748,7 @@ int wb_fx_render(wb_fx* fx, int n, const uint8_t* const* images_in, uint8_t* con
     for (int i = 0; i < n; ++i) {
       const FxCamera& cam = fx->cams[cam_ids[i]].view;
       CK(cudaMemcpyAsync(images_out[i], fx->d_out + off, frame_bytes(out_fmt, cam.w, cam.h), cudaMemcpyDeviceToHost, st));
-      off += ((size_t)cam.w * cam.h * 3 + 255) / 256 * 256;
+      off += slot_bytes(cam);
     }
   }
   CK(cudaStreamSynchronize(st));

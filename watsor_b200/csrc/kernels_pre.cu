@@ -37,7 +37,8 @@ __device__ __forceinline__ float lerp_px(float tl, float tr, float bl, float br,
 
 // The 12 source bytes one resized pixel interpolates: channel c of tap k (tl, tr, bl, br) goes to raw[c * 4 + k].
 // For a YUV frame (4:2:0 or 4:2:2) the slots hold Y, U, V of each tap, and resized_pixel_lerp converts them to the
-// RGB24 bytes of cv2.cvtColor first, so the interpolation sees the same bytes as for the converted RGB frame.
+// RGB24 bytes of cv2.cvtColor first, so the interpolation sees the same bytes as for the converted RGB frame.  The
+// other RGB byte orders put each tap's R, G and B in the same slots as RGB24 does, so their lerp is RGB24's.
 __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const AxisTap& ty, const AxisTap& tx,
                                                    uint32_t (&raw)[12]) {
   if (fd.fmt == WB_FMT_RGB24) {
@@ -50,6 +51,38 @@ __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const Ax
       raw[c * 4 + 2] = __ldg(r1 + tx.lo * 3 + c);
       raw[c * 4 + 3] = __ldg(r1 + tx.hi * 3 + c);
     }
+  } else if (fmt_rgb(fd.fmt)) {
+    // BGR24, RGBA, BGRA: each call below sees its layout as constants
+    const uint8_t* r0 = fd.ptr + (size_t)ty.lo * fd.pitch;
+    const uint8_t* r1 = fd.ptr + (size_t)ty.hi * fd.pitch;
+    auto bytes = [&](const RgbLayout& L) {
+      const uint8_t* const p[4] = {r0 + tx.lo * L.bpp, r0 + tx.hi * L.bpp, r1 + tx.lo * L.bpp, r1 + tx.hi * L.bpp};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        raw[0 + k] = __ldg(p[k] + L.r);
+        raw[4 + k] = __ldg(p[k] + L.g);
+        raw[8 + k] = __ldg(p[k] + L.b);
+      }
+    };
+    // 4-byte pixels of a word-aligned frame (its pitch, 4w, always is): one 32-bit load per tap
+    auto words = [&](const RgbLayout& L) {
+      const uint32_t* q0 = reinterpret_cast<const uint32_t*>(r0);
+      const uint32_t* q1 = reinterpret_cast<const uint32_t*>(r1);
+      const uint32_t px[4] = {__ldg(q0 + tx.lo), __ldg(q0 + tx.hi), __ldg(q1 + tx.lo), __ldg(q1 + tx.hi)};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        raw[0 + k] = (px[k] >> (8 * L.r)) & 255u;
+        raw[4 + k] = (px[k] >> (8 * L.g)) & 255u;
+        raw[8 + k] = (px[k] >> (8 * L.b)) & 255u;
+      }
+    };
+    const bool aligned = (reinterpret_cast<uintptr_t>(fd.ptr) & 3) == 0;
+    if (fd.fmt == WB_FMT_BGR24)
+      bytes(rgb_layout(WB_FMT_BGR24));
+    else if (fd.fmt == WB_FMT_RGBA)
+      aligned ? words(rgb_layout(WB_FMT_RGBA)) : bytes(rgb_layout(WB_FMT_RGBA));
+    else
+      aligned ? words(rgb_layout(WB_FMT_BGRA)) : bytes(rgb_layout(WB_FMT_BGRA));
   } else {
     // 4:2:2 and 4:2:0 branch apart so that each sees its layout's steps and shifts as constants (a layout chosen at
     // run time kept them in registers, and the generic stem spilled)
@@ -84,7 +117,7 @@ __device__ __forceinline__ void resized_pixel(const FrameDesc& fd, const AxisTap
                                               float sub, float* out3) {
   uint32_t raw[12];
   resized_pixel_load(fd, ty, tx, raw);
-  resized_pixel_lerp(raw, fd.fmt != WB_FMT_RGB24, tx.lerp, ty.lerp, mul, sub, out3);
+  resized_pixel_lerp(raw, !fmt_rgb(fd.fmt), tx.lerp, ty.lerp, mul, sub, out3);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -266,7 +299,7 @@ __global__ void __launch_bounds__(256)
         const int i = i0 + u * 256;
         if (i < tile_h * tile_w) {
           float v[3] = {0.f, 0.f, 0.f};
-          if (inside[u]) resized_pixel_lerp(raw[u], fd.fmt != WB_FMT_RGB24, txs[u].lerp, tys[u].lerp, mul, sub, v);
+          if (inside[u]) resized_pixel_lerp(raw[u], !fmt_rgb(fd.fmt), txs[u].lerp, tys[u].lerp, mul, sub, v);
           s_in[i * 3 + 0] = v[0];
           s_in[i * 3 + 1] = v[1];
           s_in[i * 3 + 2] = v[2];

@@ -597,7 +597,7 @@ static int run_all(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, i
 
 // kernels of one batch, through a CUDA graph when possible (launch-bound at small batch).  The pixel format is not part
 // of the graph's key: the kernels read it from the frame descriptors, which fill_desc copies to the device before every
-// launch, so one graph serves RGB24 and 4:2:0 batches alike.
+// launch, so one graph serves batches of every pixel format alike.
 static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t flags, int n_frames, bool windowed) {
   const uint32_t gflags = flags & WB_F_FUSE_FILTERS;
   if (!c->sw.graph) {
@@ -653,7 +653,10 @@ static int upload_frames(Slot& s, cudaStream_t st, int n, const uint8_t* const* 
 static const FormatFlag kFrameFormats[] = {{WB_F_YUV420P, WB_FMT_YUV420P, "WB_F_YUV420P"},
                                            {WB_F_NV12, WB_FMT_NV12, "WB_F_NV12"},
                                            {WB_F_YUYV422, WB_FMT_YUYV422, "WB_F_YUYV422"},
-                                           {WB_F_UYVY422, WB_FMT_UYVY422, "WB_F_UYVY422"}};
+                                           {WB_F_UYVY422, WB_FMT_UYVY422, "WB_F_UYVY422"},
+                                           {WB_F_BGR24, WB_FMT_BGR24, "WB_F_BGR24"},
+                                           {WB_F_RGBA, WB_FMT_RGBA, "WB_F_RGBA"},
+                                           {WB_F_BGRA, WB_FMT_BGRA, "WB_F_BGRA"}};
 
 // One descriptor per model image.  With use_windows and at least one camera of the batch having detection windows, the
 // batch is windowed: every window of a frame is one image (a camera without windows: one full-frame window, camera
@@ -706,8 +709,9 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
     const CameraCfg& cc = c->h_cams[cam];
     const uint8_t* base = dev[i];
     const ChromaLayout cl = chroma_layout(fmt, cc.width, cc.height);
-    const int bpp = fmt == WB_FMT_RGB24 ? 3 : cl.luma_step;  // bytes per pixel of the RGB24 / luma plane / macropixels
-    const size_t luma0 = fmt == WB_FMT_RGB24 ? 0 : luma_origin(fmt);
+    // bytes per pixel of the packed RGB frame / luma plane / macropixels
+    const int bpp = fmt_rgb(fmt) ? rgb_layout(fmt).bpp : cl.luma_step;
+    const size_t luma0 = fmt_rgb(fmt) ? 0 : luma_origin(fmt);
     const std::vector<int4>& wins = c->cam_windows[cam];
     const int nw = windowed ? std::max((int)wins.size(), 1) : 1;
     if (windowed) {
@@ -944,10 +948,13 @@ int wb_backbone_frames(wb_ctx* c, int n, const uint8_t* const* frames, const int
                        int32_t* n_images) {
   REQUIRE(c && frames && cam_ids, "NULL argument");
   REQUIRE(stop_layer >= -1 && stop_layer < (int)c->layers.size(), "stop_layer out of range");
-  REQUIRE((flags & ~(WB_F_YUV420P | WB_F_NV12 | WB_F_YUYV422 | WB_F_UYVY422 | WB_F_FRAMES_ON_DEVICE |
-                     WB_F_FUSE_FILTERS)) == 0,
-          "flags may only hold WB_F_YUV420P, WB_F_NV12, WB_F_YUYV422, WB_F_UYVY422, WB_F_FRAMES_ON_DEVICE and "
-          "WB_F_FUSE_FILTERS");
+  uint32_t allowed = WB_F_FRAMES_ON_DEVICE | WB_F_FUSE_FILTERS;
+  std::string names;
+  for (const FormatFlag& f : kFrameFormats) {
+    allowed |= f.bit;
+    names += std::string(f.name) + ", ";
+  }
+  REQUIRE((flags & ~allowed) == 0, "flags may only hold " + names + "WB_F_FRAMES_ON_DEVICE and WB_F_FUSE_FILTERS");
   StageHook h(c, n);
   if (h.rc) return h.rc;
   Slot& s = h.s;

@@ -1,5 +1,6 @@
-// yuv420.cuh -- YUV frames (what video decoders and capture devices emit) converted to the RGB24 bytes the kernels
-// read, and RGB24 pixels converted to the 4:2:0 frames the effects pass can write for an encoder.
+// yuv420.cuh -- the frame layouts the kernels read: YUV frames (what video decoders and capture devices emit) converted
+// to the RGB24 bytes the kernels work on, RGB24 pixels converted to the 4:2:0 frames the effects pass can write for an
+// encoder, and the packed RGB byte orders (RGB24, BGR24, RGBA, BGRA) described by one table, rgb_layout below.
 //
 // A 4:2:0 frame of w x h pixels (w, h even) is packed in w*h*3/2 bytes: the full-resolution luma plane, then the
 // chroma at half resolution in both directions.  A packed 4:2:2 frame (w even, any h) is [h][w][2] bytes: each pair of
@@ -22,8 +23,36 @@
 #define WB_FMT_NV12 2
 #define WB_FMT_YUYV422 3
 #define WB_FMT_UYVY422 4
+#define WB_FMT_BGR24 5
+#define WB_FMT_RGBA 6  // also rgb0: the fourth byte is not read
+#define WB_FMT_BGRA 7  // also bgr0
 
 __host__ __device__ __forceinline__ bool fmt_422(int fmt) { return fmt == WB_FMT_YUYV422 || fmt == WB_FMT_UYVY422; }
+
+// Packed RGB frames [h][w][bpp], one byte per channel, in any of four byte orders.  These facts are all that the
+// detection path (resized_pixel_load) and the effects pass (k_fx_render) know about the orders; converting one to
+// RGB24 is a byte permutation, so the kernels' results equal cv2.cvtColor(COLOR_BGR2RGB / RGBA2RGB / BGRA2RGB) of the
+// frame exactly.
+struct RgbLayout {
+  int bpp;      // bytes per pixel
+  int r, g, b;  // byte offsets of R, G and B within a pixel
+};
+__host__ __device__ __forceinline__ bool fmt_rgb(int fmt) {
+  return fmt == WB_FMT_RGB24 || fmt == WB_FMT_BGR24 || fmt == WB_FMT_RGBA || fmt == WB_FMT_BGRA;
+}
+// the layout of a packed RGB format (fmt_rgb(fmt)); a constant where fmt is one
+__host__ __device__ __forceinline__ constexpr RgbLayout rgb_layout(int fmt) {
+  return fmt == WB_FMT_BGR24  ? RgbLayout{3, 2, 1, 0}
+         : fmt == WB_FMT_RGBA ? RgbLayout{4, 0, 1, 2}
+         : fmt == WB_FMT_BGRA ? RgbLayout{4, 2, 1, 0}
+                              : RgbLayout{3, 0, 1, 2};
+}
+
+// the format's name, as ffmpeg's -pix_fmt and the Python layer spell it (for error messages)
+inline const char* fmt_name(int fmt) {
+  static const char* const names[] = {"rgb24", "yuv420p", "nv12", "yuyv422", "uyvy422", "bgr24", "rgba", "bgra"};
+  return fmt >= 0 && fmt < 8 ? names[fmt] : "unknown";
+}
 
 struct ChromaLayout {
   int luma_step;  // bytes between horizontally adjacent Y samples: 1 (4:2:0 luma plane), 2 (4:2:2 macropixels)
@@ -54,7 +83,7 @@ __host__ __device__ __forceinline__ size_t chroma_origin(int fmt, int w, int h) 
 
 // bytes of one packed frame
 __host__ __device__ __forceinline__ size_t frame_bytes(int fmt, int w, int h) {
-  return fmt == WB_FMT_RGB24 ? (size_t)w * h * 3 : fmt_422(fmt) ? (size_t)w * h * 2 : (size_t)w * h * 3 / 2;
+  return fmt_rgb(fmt) ? (size_t)w * h * rgb_layout(fmt).bpp : fmt_422(fmt) ? (size_t)w * h * 2 : (size_t)w * h * 3 / 2;
 }
 
 // address of the U sample of pixel (x, y) given that of pixel (0, 0); the V sample is at + v_off.  A window of a frame

@@ -109,9 +109,11 @@ class B200ObjectDetector(object):
 
     def detect_batch(self, frames, cam_ids, detections, verdicts=None, fuse_filters=True,
                      frames_on_device=False, pixel_format='rgb24'):
-        """pixel_format: 'rgb24' (H, W, 3), the 4:2:0 layouts decoders emit, 'yuv420p' / 'nv12' (H*3//2, W), or the
-        packed 4:2:2 layouts of webcams and capture cards, 'yuyv422' / 'uyvy422' (H, W, 2): those are converted on the
-        GPU exactly as cv2.cvtColor converts them.  One format per batch."""
+        """pixel_format: 'rgb24' (H, W, 3); OpenCV's 'bgr24' (H, W, 3) as cv2.VideoCapture and cv2.imread return it;
+        the 4-byte 'rgba' / 'bgra' (H, W, 4) of GPU pipelines (alpha ignored); the 4:2:0 layouts decoders emit,
+        'yuv420p' / 'nv12' (H*3//2, W); or the packed 4:2:2 layouts of webcams and capture cards, 'yuyv422' /
+        'uyvy422' (H, W, 2).  All are converted on the GPU exactly as cv2.cvtColor converts them to RGB24.  One format
+        per batch."""
         flags = (_lib.WB_F_FUSE_FILTERS if fuse_filters else 0) | \
                 (_lib.WB_F_FRAMES_ON_DEVICE if frames_on_device else 0)
         return self.engine.detect(frames, cam_ids, detections, verdicts, flags, pixel_format)

@@ -19,24 +19,35 @@ PRECISIONS = {'fp32': 0, 'bf16': 1, 'tf32x3': 2, 'tf32x1': 3, 'fp16': 4}
 PRECISION_FP32, PRECISION_BF16_TC = PRECISIONS['fp32'], PRECISIONS['bf16']
 PRECISION_TF32X3, PRECISION_FP16_TC = PRECISIONS['tf32x3'], PRECISIONS['fp16']
 
-# frame layouts the hot path reads, by ffmpeg's -pix_fmt names -> wb_detect / wb_submit flag
+# frame layouts the hot path reads, by ffmpeg's -pix_fmt names -> wb_detect / wb_submit flag: RGB24 and YUV ...
 PIXEL_FORMATS = {'rgb24': 0, 'yuv420p': _lib.WB_F_YUV420P, 'nv12': _lib.WB_F_NV12,
                  'yuyv422': _lib.WB_F_YUYV422, 'uyvy422': _lib.WB_F_UYVY422}
+# ... and the other packed RGB byte orders: BGR24 (OpenCV's frames) and the 4-byte RGBA / BGRA (also rgb0 / bgr0, the
+# fourth byte is not read), read as the RGB24 frame cv2.cvtColor makes of them.  Every function here that takes a
+# pixel_format accepts these as well, except frame_shape, which keeps its contract (layout_shape covers every layout);
+# PIXEL_FORMATS keeps listing the layouts it always listed.
+RGB_ORDERS = {'bgr24': _lib.WB_F_BGR24, 'rgba': _lib.WB_F_RGBA, 'bgra': _lib.WB_F_BGRA}
+# every layout, by name -> flag
+FRAME_FORMATS = dict(PIXEL_FORMATS, **RGB_ORDERS)
+_BYTES_PER_PIXEL = {'rgb24': 3, 'bgr24': 3, 'rgba': 4, 'bgra': 4}
 
 
-def _check_format(pixel_format):
-    if pixel_format not in PIXEL_FORMATS:
-        raise ValueError('pixel_format must be one of %s, not %r' % (', '.join(PIXEL_FORMATS), pixel_format))
+def _check_format(pixel_format, formats=FRAME_FORMATS):
+    if pixel_format not in formats:
+        raise ValueError('pixel_format must be one of %s, not %r%s' % (
+            ', '.join(formats), pixel_format,
+            ' (engine.layout_shape gives the shape of a %s frame)' % pixel_format if pixel_format in FRAME_FORMATS else ''))
 
 
-def frame_shape(pixel_format, width, height):
-    """numpy shape of one packed uint8 frame of a `width` x `height` camera: (H, W, 3) for rgb24, (H*3//2, W) for the
-    4:2:0 formats (luma plane, then the chroma; include/watsor_b200.h), which need an even width and height, and
-    (H, W, 2) for the packed 4:2:2 formats (the shape cv2.cvtColor takes), which need an even width.  The same shapes
-    hold for the frames the effects pass reads and writes (output.effects, `output_format`)."""
+def layout_shape(pixel_format, width, height):
+    """numpy shape of one packed uint8 frame of a `width` x `height` camera in any layout of FRAME_FORMATS: (H, W, 3)
+    for rgb24 and bgr24, (H, W, 4) for rgba and bgra, (H*3//2, W) for the 4:2:0 formats (luma plane, then the chroma;
+    include/watsor_b200.h), which need an even width and height, and (H, W, 2) for the packed 4:2:2 formats (the shape
+    cv2.cvtColor takes), which need an even width.  The same shapes hold for the frames the effects pass reads and
+    writes (output.effects, `output_format`)."""
     _check_format(pixel_format)
-    if pixel_format == 'rgb24':
-        return (height, width, 3)
+    if pixel_format in _BYTES_PER_PIXEL:
+        return (height, width, _BYTES_PER_PIXEL[pixel_format])
     if pixel_format in ('yuyv422', 'uyvy422'):
         if width % 2:
             raise ValueError('%s frames need an even width; the camera is %dx%d' % (pixel_format, width, height))
@@ -46,15 +57,22 @@ def frame_shape(pixel_format, width, height):
     return (height * 3 // 2, width)
 
 
+def frame_shape(pixel_format, width, height):
+    """layout_shape for the RGB24 and YUV layouts of PIXEL_FORMATS, the names this function has always taken; it
+    refuses the other RGB byte orders (bgr24, rgba, bgra) as it always has, and layout_shape gives their shapes."""
+    _check_format(pixel_format, PIXEL_FORMATS)
+    return layout_shape(pixel_format, width, height)
+
+
 def check_frames(frames, sizes, pixel_format):
-    """Raises ValueError unless every numpy frame is a C-contiguous uint8 array of `frame_shape` for its camera's
+    """Raises ValueError unless every numpy frame is a C-contiguous uint8 array of `layout_shape` for its camera's
     (width, height) in `sizes`.  A size of None (a camera unknown here, which the library reports) and raw addresses
     are passed through unchecked."""
     _check_format(pixel_format)
     for i, (frame, size) in enumerate(zip(frames, sizes)):
         if size is None:
             continue
-        shape = frame_shape(pixel_format, *size)
+        shape = layout_shape(pixel_format, *size)
         if isinstance(frame, np.ndarray) and (frame.dtype != np.uint8 or frame.shape != shape or
                                               not frame.flags['C_CONTIGUOUS']):
             raise ValueError('frame %d: a %s frame of a %dx%d camera is a C-contiguous uint8 array of shape %s, not %s %s%s'
@@ -188,11 +206,12 @@ class Engine:
         for c in set(cam_ids):
             if c in self.windows:
                 check_windows(self.windows[c], *self.cameras[c], pixel_format)
-        return PIXEL_FORMATS[pixel_format]
+        return FRAME_FORMATS[pixel_format]
 
     def detect(self, frames, cam_ids, out, verdicts=None, flags=0, pixel_format='rgb24'):
         """frames: host uint8 arrays (or device pointers with WB_F_FRAMES_ON_DEVICE) in `pixel_format`
-        ('rgb24', 'yuv420p', 'nv12', 'yuyv422' or 'uyvy422', see frame_shape); out: per frame a `Detection*100` ctypes array / address.
+        (a name of FRAME_FORMATS: 'rgb24', 'bgr24', 'rgba', 'bgra', 'yuv420p', 'nv12', 'yuyv422' or 'uyvy422', see
+        layout_shape); out: per frame a `Detection*100` ctypes array / address.
         Returns device ms."""
         flags |= self._format_flags(frames, cam_ids, pixel_format)
         n, fp, cams, op, vp = self._io(frames, cam_ids, out, verdicts)

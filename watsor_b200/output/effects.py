@@ -19,7 +19,7 @@ import numpy as np
 
 from .. import _lib
 from ..config.coco import COCO_CLASSES, get_coco_class
-from ..engine import check_frames, frame_shape
+from ..engine import check_frames, layout_shape
 from ..stream.share import MAX_DETECTIONS, Detection
 from .font import FontAtlas
 
@@ -27,9 +27,11 @@ WB_FX_BLEND, WB_FX_DRAW, WB_FX_CONTOURS, WB_FX_ON_DEVICE = 1, 2, 4, 8
 WB_FX_YUV420P, WB_FX_NV12 = 16, 32
 WB_FX_OUT_YUV420P, WB_FX_OUT_NV12 = 64, 128
 WB_FX_YUYV422, WB_FX_UYVY422 = 256, 512
+WB_FX_BGR24, WB_FX_RGBA, WB_FX_BGRA = 1024, 2048, 4096
+WB_FX_OUT_BGR24 = 8192
 _FX_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_YUV420P, 'nv12': WB_FX_NV12, 'yuyv422': WB_FX_YUYV422,
-               'uyvy422': WB_FX_UYVY422}
-_FX_OUT_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_OUT_YUV420P, 'nv12': WB_FX_OUT_NV12}
+               'uyvy422': WB_FX_UYVY422, 'bgr24': WB_FX_BGR24, 'rgba': WB_FX_RGBA, 'bgra': WB_FX_BGRA}
+_FX_OUT_FORMATS = {'rgb24': 0, 'yuv420p': WB_FX_OUT_YUV420P, 'nv12': WB_FX_OUT_NV12, 'bgr24': WB_FX_OUT_BGR24}
 
 
 class _Font(Structure):
@@ -43,7 +45,8 @@ class _Label(Structure):
 
 
 def _check_output_format(output_format):
-    # 4:2:2 is an input format only: OpenCV's RGB -> 4:2:2 arithmetic is not the I420 one the kernel restates
+    # 4:2:2 is an input format only: OpenCV's RGB -> 4:2:2 arithmetic is not the I420 one the kernel restates; RGBA /
+    # BGRA are input formats only: an encoder or cv2.imencode takes RGB24, BGR24 or 4:2:0
     if output_format not in _FX_OUT_FORMATS:
         raise ValueError('output_format must be one of %s, not %r' % (', '.join(_FX_OUT_FORMATS), output_format))
 
@@ -136,11 +139,12 @@ class EffectsEngine:
 
     def render(self, images_in, images_out, cam_ids, rows, flags, pixel_format='rgb24', output_format='rgb24'):
         """images: uint8 arrays (or device pointers with WB_FX_ON_DEVICE); rows: per frame the `Detection * 100`
-        array of a frame header (or its address).  pixel_format: layout of images_in, 'rgb24', a 4:2:0 layout
-        'yuv420p' / 'nv12' or a packed 4:2:2 layout 'yuyv422' / 'uyvy422' (converted as cv2.cvtColor does; see
-        engine.frame_shape).  output_format: layout of images_out, 'rgb24' or 'yuv420p' / 'nv12' for an encoder that
-        takes 4:2:0 (the rendered frame converted as cv2.cvtColor(COLOR_RGB2YUV_I420) does).  With either side in a YUV
-        format, images_out must be other buffers than images_in."""
+        array of a frame header (or its address).  pixel_format: layout of images_in, 'rgb24', OpenCV's 'bgr24',
+        'rgba' / 'bgra' (alpha ignored), a 4:2:0 layout 'yuv420p' / 'nv12' or a packed 4:2:2 layout 'yuyv422' /
+        'uyvy422' (converted as cv2.cvtColor does; see engine.layout_shape).  output_format: layout of images_out,
+        'rgb24', 'bgr24' for cv2.imencode (the rendered frame with R and B swapped, cv2.cvtColor(COLOR_RGB2BGR)) or
+        'yuv420p' / 'nv12' for an encoder that takes 4:2:0 (the rendered frame converted as
+        cv2.cvtColor(COLOR_RGB2YUV_I420) does).  images_out may be images_in only when both are 'rgb24' or 'bgr24'."""
         _check_output_format(output_format)
         sizes = [self._sizes.get(c) for c in cam_ids]
         check_frames(images_in, sizes, pixel_format)
@@ -267,13 +271,14 @@ class DrawEffectWithContours(DrawEffect):
 class FusedEffects(_Effect):
     """The image part of the effect chain main.py:302-312 builds for a camera, as one pass:
     with a mask   BlendEffect + DrawEffectWithContours;   without   CopyImageEffect + DrawEffect.
-    output_format 'yuv420p' / 'nv12' writes image_out as the 4:2:0 frame an encoder takes (engine.frame_shape), so the
-    output FrameBuffer holds w*h*3//2 bytes and no RGB -> 4:2:0 conversion is left to the encoder."""
+    output_format 'yuv420p' / 'nv12' writes image_out as the 4:2:0 frame an encoder takes (engine.layout_shape), so the
+    output FrameBuffer holds w*h*3//2 bytes and no RGB -> 4:2:0 conversion is left to the encoder; 'bgr24' writes the
+    BGR24 frame that cv2.imencode takes without a cv2.cvtColor of its own."""
 
     def __init__(self, camera_config, engine=None, output_format='rgb24'):
         super().__init__(engine)
         _check_output_format(output_format)
-        frame_shape(output_format, camera_config['width'], camera_config['height'])   # even sizes
+        layout_shape(output_format, camera_config['width'], camera_config['height'])   # even sizes
         self.output_format = output_format
         if 'mask' in camera_config:
             alpha, cont = _camera_tables(camera_config, True, True)
@@ -296,4 +301,4 @@ def new_rows():
 __all__ = ['EffectsEngine', 'CopyHeaderEffect', 'CopyImageEffect', 'BlendEffect', 'DrawEffect',
            'DrawEffectWithContours', 'FusedEffects', 'contour_bits', 'new_rows', 'WB_FX_BLEND', 'WB_FX_DRAW',
            'WB_FX_CONTOURS', 'WB_FX_ON_DEVICE', 'WB_FX_YUV420P', 'WB_FX_NV12', 'WB_FX_OUT_YUV420P', 'WB_FX_OUT_NV12',
-           'WB_FX_YUYV422', 'WB_FX_UYVY422']
+           'WB_FX_YUYV422', 'WB_FX_UYVY422', 'WB_FX_BGR24', 'WB_FX_RGBA', 'WB_FX_BGRA', 'WB_FX_OUT_BGR24']

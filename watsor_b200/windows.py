@@ -39,7 +39,8 @@ def grid_windows(width, height, cols, rows, overlap=0.25, full_frame=True, align
 def check_windows(windows, width, height, pixel_format='rgb24'):
     """Raises ValueError unless `windows` is a list of at most WB_MAX_WINDOWS (x, y, w, h) integer rectangles with
     w, h >= 1 inside a `width` x `height` frame, with even origins and sizes for the 4:2:0 formats and an even x and w
-    for the 4:2:2 formats (their chroma is shared by pixel pairs of a row only)."""
+    for the 4:2:2 formats (their chroma is shared by pixel pairs of a row only).  The packed RGB orders (rgb24, bgr24,
+    rgba, bgra) take any window."""
     windows = list(windows)
     if len(windows) > WB_MAX_WINDOWS:
         raise ValueError('a camera may have at most %d detection windows, not %d' % (WB_MAX_WINDOWS, len(windows)))
