@@ -127,7 +127,8 @@ int wb_register_host(wb_ctx* ctx, void* ptr, size_t bytes);
 int wb_unregister_host(wb_ctx* ctx, void* ptr);
 
 /* replaces ObjectDetector.detect (tensorflow_cpu.py:74-92 / tensorrt_gpu.py:65-91) for a batch:
- *   frames[i]   frame of camera cam_ids[i], host or device memory, packed (no row padding):
+ *   frames[i]   frame of camera cam_ids[i], host or device memory, packed (no row padding; wb_detect_planes below
+ *               takes frames whose rows are padded or whose planes are separate buffers):
  *               uint8 RGB24 HWC [h][w][3] (share.py:68-73) by default; with WB_F_YUV420P or WB_F_NV12 a
  *               4:2:0 frame [h*3/2][w]: the luma plane [h][w], then the chroma ([h/2][w/2] U, then [h/2][w/2] V
  *               for yuv420p; [h/2][w/2] interleaved (U, V) pairs for NV12).  4:2:0 needs an even w and h; the
@@ -172,6 +173,33 @@ int wb_submit(wb_ctx* ctx, int slot, int n, const uint8_t* const* frames, const 
               uint32_t flags);
 int wb_collect(wb_ctx* ctx, int slot, wb_detection* const* out, uint32_t* const* verdicts,
                float* gpu_ms);
+
+/* Frames given as planes with row pitches: hardware decoder surfaces (NV12 whose pitch, and so the start of the chroma
+ * plane, is rounded up to the decoder's alignment), ffmpeg AVFrames (data[i] / linesize[i]: yuv420p has three separate
+ * buffers), capture buffers with bytesperline > 2w, and views of part of a larger frame.  Each plane holds the rows of
+ * the packed layout above, pitch[k] bytes apart:
+ *   RGB24, BGR24, RGBA, BGRA, YUYV, UYVY   plane[0]: the h pixel rows (bpp*w or 2w bytes each)
+ *   NV12                                   plane[0]: h rows of w Y bytes; plane[1]: h/2 rows of w/2 (U, V) pairs
+ *                                          (w bytes)
+ *   yuv420p                                plane[0]: Y as for NV12; plane[1] U, plane[2] V: h/2 rows of w/2 bytes each,
+ *                                          in any order in memory, with the same pitch
+ * Planes the format does not use are NULL.  Every pitch is at least the plane's row bytes and below 2^31; bytes
+ * between the end of a row and the next row are never read. */
+typedef struct wb_frame_planes {
+  const uint8_t* plane[3];
+  int64_t pitch[3]; /* bytes between the starts of two rows of plane[k] */
+} wb_frame_planes;
+/* wb_detect / wb_submit on frames given as planes, with the same flags and wb_collect to collect wb_submit_planes.
+ * Host frames (no WB_F_FRAMES_ON_DEVICE; pageable or wb_register_host-pinned) are packed into the slot's staging
+ * buffer as they are uploaded, one cudaMemcpy2DAsync per plane.  Device frames are read in place: the kernels read the
+ * caller's planes through their pitches, without a copy.  Either way the planes must stay valid until wb_collect has
+ * returned.  A batch whose planes do not match its format (a plane missing or one too many, a pitch out of range,
+ * yuv420p U and V pitches that differ, or an odd size where 4:2:0 or 4:2:2 needs it even) is refused with a message
+ * naming the frame, the format and the value, and nothing is enqueued. */
+int wb_detect_planes(wb_ctx* ctx, int n, const wb_frame_planes* frames, const int32_t* cam_ids, uint32_t flags,
+                     wb_detection* const* out, uint32_t* const* verdicts, float* gpu_ms);
+int wb_submit_planes(wb_ctx* ctx, int slot, int n, const wb_frame_planes* frames, const int32_t* cam_ids,
+                     uint32_t flags);
 
 /* order the library's internal slot streams against a caller stream (0 = legacy default stream):
  * direction 0: every slot stream waits for the work already enqueued on `cuda_stream`;

@@ -2,7 +2,7 @@
 library has not been built -- there is no CPU fallback."""
 import ctypes
 import os
-from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_size_t,
+from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t,
                     c_uint8, c_uint32, c_uint64, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -20,6 +20,11 @@ WB_MAX_WINDOWS = 16
 class ClassFilter(Structure):
     _fields_ = [('label', c_int32), ('has_zone_list', c_int32), ('zone_bits', c_uint32),
                 ('_pad', c_int32), ('confidence', c_double), ('area', c_double)]
+
+
+class FramePlanes(Structure):
+    """wb_frame_planes: a frame's planes and the bytes between the rows of each (unused planes NULL)"""
+    _fields_ = [('plane', c_void_p * 3), ('pitch', c_int64 * 3)]
 
 
 class WatsorB200Error(RuntimeError):
@@ -73,6 +78,9 @@ def load():
                               P(c_void_p), P(c_float)]),
         'wb_submit': (c_int, [c_void_p, c_int, c_int, P(c_void_p), P(c_int32), c_uint32]),
         'wb_collect': (c_int, [c_void_p, c_int, P(c_void_p), P(c_void_p), P(c_float)]),
+        'wb_detect_planes': (c_int, [c_void_p, c_int, P(FramePlanes), P(c_int32), c_uint32, P(c_void_p),
+                                     P(c_void_p), P(c_float)]),
+        'wb_submit_planes': (c_int, [c_void_p, c_int, c_int, P(FramePlanes), P(c_int32), c_uint32]),
         'wb_stream_fence': (c_int, [c_void_p, c_uint64, c_int]),
         'wb_comm_unique_id': (c_int, [c_void_p]),
         'wb_comm_init': (c_int, [c_void_p, c_int, c_int, c_void_p]),
@@ -116,7 +124,8 @@ def load():
 EXPORTS = ['wb_abi_version', 'wb_last_error', 'wb_device_count', 'wb_create', 'wb_destroy',
            'wb_device_name', 'wb_set_stream', 'wb_model_info', 'wb_set_camera', 'wb_set_camera_windows',
            'wb_register_host',
-           'wb_unregister_host', 'wb_detect', 'wb_submit', 'wb_collect', 'wb_stream_fence', 'wb_comm_unique_id', 'wb_comm_init',
+           'wb_unregister_host', 'wb_detect', 'wb_submit', 'wb_collect', 'wb_detect_planes', 'wb_submit_planes',
+           'wb_stream_fence', 'wb_comm_unique_id', 'wb_comm_init',
            'wb_scatter_frames', 'wb_comm_destroy', 'wb_preprocess', 'wb_backbone', 'wb_backbone_frames',
            'wb_postprocess', 'wb_filter_rows', 'wb_anchors', 'wb_last_launch_count', 'wb_profile_layers',
            'wb_tracker_create', 'wb_tracker_destroy', 'wb_tracker_update', 'wb_sieve_rows', 'wb_debug_pyset_order',

@@ -10,17 +10,21 @@
 #include "yuv420.cuh"
 
 // One model image of a batch: where its pixels are and which camera it belongs to.  The image is a whole frame or a
-// detection window of one (wb_set_camera_windows); either way its rows start at `ptr`, `pitch` bytes apart.
-// Replaces the (image_shape, image_np) pair of ObjectDetector.detect (tensorflow_cpu.py:74).
+// detection window of one (wb_set_camera_windows); either way its rows start at `ptr`, `pitch` bytes apart, and its
+// chroma rows at `chroma`, `chroma_pitch` bytes apart.  The planes are the caller's device frame (read in place) or
+// the packed copy of a host frame.  Replaces the (image_shape, image_np) pair of ObjectDetector.detect
+// (tensorflow_cpu.py:74).
 struct FrameDesc {
   const uint8_t* ptr;     // device pointer to pixel (0, 0): RGB24 HWC (share.py:68-73), or its Y sample in a YUV frame
-  const uint8_t* chroma;  // YUV: the U sample of pixel (0, 0) (packed frame: ptr + w*h for 4:2:0; the U byte of the
-                          // pixel's macropixel for 4:2:2)
+  const uint8_t* chroma;  // YUV: the U sample of pixel (0, 0) (4:2:0: in the U or UV plane; 4:2:2: the U byte of the
+                          // pixel's macropixel)
+  int64_t v_off;          // YUV: bytes from a U sample to its V sample (yuv420p: V plane - U plane, either sign; NV12:
+                          // 1; 4:2:2: 2)
   int32_t w, h;
-  int32_t pitch;          // bytes between rows of the RGB24 / luma plane / macropixels (packed frame: 3w / w / 2w)
+  int32_t pitch;          // bytes between rows of the RGB / luma plane / macropixels (packed frame: bpp*w / w / 2w)
+  int32_t chroma_pitch;   // YUV: bytes between chroma rows (packed frame: w/2 yuv420p, w NV12, 2w 4:2:2)
   int32_t cam;            // -1: no camera (a window's rows are filtered after the merge, k_window_merge)
   int32_t fmt;            // WB_FMT_* (yuv420.cuh)
-  int32_t v_off;          // YUV: bytes from a U sample to its V sample (ChromaLayout::v_off of the parent frame; 2 for 4:2:2)
 };
 
 // The model images of one frame of a windowed batch, for k_window_merge: images [first, first + count) are its

@@ -64,7 +64,7 @@ __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const Ax
         raw[8 + k] = __ldg(p[k] + L.b);
       }
     };
-    // 4-byte pixels of a word-aligned frame (its pitch, 4w, always is): one 32-bit load per tap
+    // 4-byte pixels of a frame whose every row is word-aligned: one 32-bit load per tap
     auto words = [&](const RgbLayout& L) {
       const uint32_t* q0 = reinterpret_cast<const uint32_t*>(r0);
       const uint32_t* q1 = reinterpret_cast<const uint32_t*>(r1);
@@ -76,7 +76,8 @@ __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const Ax
         raw[8 + k] = (px[k] >> (8 * L.b)) & 255u;
       }
     };
-    const bool aligned = (reinterpret_cast<uintptr_t>(fd.ptr) & 3) == 0;
+    // row y starts at ptr + y * pitch: word-aligned on every row only when both are multiples of 4
+    const bool aligned = ((reinterpret_cast<uintptr_t>(fd.ptr) | (uintptr_t)fd.pitch) & 3) == 0;
     if (fd.fmt == WB_FMT_BGR24)
       bytes(rgb_layout(WB_FMT_BGR24));
     else if (fd.fmt == WB_FMT_RGBA)
@@ -95,7 +96,7 @@ __device__ __forceinline__ void resized_pixel_load(const FrameDesc& fd, const Ax
     if (fmt_422(fd.fmt))
       taps(chroma_layout_of(WB_FMT_YUYV422, fd.pitch, 2));
     else
-      taps(chroma_layout_of(fd.fmt == WB_FMT_NV12 ? WB_FMT_NV12 : WB_FMT_YUV420P, fd.pitch, (size_t)fd.v_off));
+      taps(chroma_layout_of(fd.fmt == WB_FMT_NV12 ? WB_FMT_NV12 : WB_FMT_YUV420P, fd.chroma_pitch, fd.v_off));
   }
 }
 __device__ __forceinline__ void resized_pixel_lerp(uint32_t (&raw)[12], bool yuv, float lx, float ly, float mul,

@@ -629,12 +629,29 @@ static int enqueue_kernels(wb_ctx* c, Slot& s, cudaStream_t st, int n, uint32_t 
   return 0;
 }
 
-// Copies n host frames of bytes[i] each to s.d_frames, 256-byte aligned, and points dev[i] at frame i's copy.  A buffer
-// that is too small is replaced, once the stream is done with it, by one with 25 % headroom.
-static int upload_frames(Slot& s, cudaStream_t st, int n, const uint8_t* const* frames, const size_t* bytes,
-                         const uint8_t** dev) {
+// the planes of the packed frame of format `fmt` and size w x h that starts at `base`
+static wb_frame_planes packed_planes(const uint8_t* base, int fmt, int w, int h) {
+  wb_frame_planes p{};
+  for (int k = 0; k < plane_count(fmt); ++k) {
+    p.plane[k] = base + plane_offset(fmt, w, h, k);
+    p.pitch[k] = (int64_t)plane_row_bytes(fmt, w, k);
+  }
+  return p;
+}
+
+static bool same_planes(const wb_frame_planes& a, const wb_frame_planes& b, int fmt) {
+  for (int k = 0; k < plane_count(fmt); ++k)
+    if (a.plane[k] != b.plane[k] || a.pitch[k] != b.pitch[k]) return false;
+  return true;
+}
+
+// Copies n host frames to s.d_frames, each packed into frame_bytes of its format and size (sizes[i] = (w, h)) at a
+// 256-byte aligned offset, and replaces their planes with those of the copies.  A packed frame is one copy; any other
+// is copied plane by plane, each plane's rows gathered from its pitch.  A buffer that is too small is replaced, once
+// the stream is done with it, by one with 25 % headroom.
+static int upload_frames(Slot& s, cudaStream_t st, int n, int fmt, const int2* sizes, wb_frame_planes* planes) {
   size_t total = 0;
-  for (int i = 0; i < n; ++i) total += (bytes[i] + 255) / 256 * 256;
+  for (int i = 0; i < n; ++i) total += (frame_bytes(fmt, sizes[i].x, sizes[i].y) + 255) / 256 * 256;
   if (total > s.d_frames_cap) {
     CK(cudaStreamSynchronize(st));
     s.d_frames_cap = total + total / 4;
@@ -642,9 +659,91 @@ static int upload_frames(Slot& s, cudaStream_t st, int n, const uint8_t* const* 
   }
   size_t off = 0;
   for (int i = 0; i < n; ++i) {
-    dev[i] = s.d_frames + off;
-    CK(cudaMemcpyAsync(s.d_frames + off, frames[i], bytes[i], cudaMemcpyHostToDevice, st));
-    off += (bytes[i] + 255) / 256 * 256;
+    const int w = sizes[i].x, h = sizes[i].y;
+    const wb_frame_planes& src = planes[i];
+    const wb_frame_planes dst = packed_planes(s.d_frames + off, fmt, w, h);
+    if (same_planes(src, packed_planes(src.plane[0], fmt, w, h), fmt)) {
+      CK(cudaMemcpyAsync(s.d_frames + off, src.plane[0], frame_bytes(fmt, w, h), cudaMemcpyHostToDevice, st));
+    } else {
+      for (int k = 0; k < plane_count(fmt); ++k)
+        CK(cudaMemcpy2DAsync(const_cast<uint8_t*>(dst.plane[k]), (size_t)dst.pitch[k], src.plane[k],
+                             (size_t)src.pitch[k], (size_t)dst.pitch[k], plane_rows(h, k), cudaMemcpyHostToDevice, st));
+    }
+    planes[i] = dst;
+    off += (frame_bytes(fmt, w, h) + 255) / 256 * 256;
+  }
+  return 0;
+}
+
+// The descriptor of the window (x, y, w, h) = wd of a frame given as device planes (NULL planes: a descriptor without
+// pixels, for the post stage alone).  The window's rows are the frame's, read through the planes' own pitches.
+static FrameDesc frame_desc(const wb_frame_planes& p, int fmt, int4 wd, int cam) {
+  FrameDesc d{};
+  d.w = wd.z;
+  d.h = wd.w;
+  d.cam = cam;
+  d.fmt = fmt;
+  d.pitch = (int32_t)p.pitch[0];
+  if (p.plane[0] == nullptr) return d;
+  const uint8_t* row = p.plane[0] + wd.y * p.pitch[0];  // the window's first row, of pixels or macropixels
+  if (fmt_rgb(fmt)) {
+    d.ptr = row + (size_t)wd.x * rgb_layout(fmt).bpp;
+  } else if (fmt_422(fmt)) {
+    // macropixels Y0 U Y1 V (YUYV) or U Y0 V Y1 (UYVY), V two bytes after U
+    d.ptr = row + luma_origin(fmt) + (size_t)wd.x * 2;
+    d.chroma = row + (fmt == WB_FMT_YUYV422 ? 1 : 0) + (size_t)(wd.x >> 1) * 4;
+    d.chroma_pitch = d.pitch;
+    d.v_off = 2;
+  } else {
+    const bool nv12 = fmt == WB_FMT_NV12;
+    d.ptr = row + wd.x;
+    d.chroma = p.plane[1] + (wd.y >> 1) * p.pitch[1] + (size_t)(wd.x >> 1) * (nv12 ? 2 : 1);
+    d.chroma_pitch = (int32_t)p.pitch[1];
+    d.v_off = nv12 ? 1 : (int64_t)(reinterpret_cast<intptr_t>(p.plane[2]) - reinterpret_cast<intptr_t>(p.plane[1]));
+  }
+  return d;
+}
+
+// Refuses planes that do not match frame i's format and width: a used plane missing or an unused one given, a pitch
+// below the plane's row bytes or at 2^31 or more (FrameDesc holds pitches as int32), yuv420p U and V pitches that
+// differ (one chroma pitch serves both).
+static int check_planes(int i, const wb_frame_planes& p, int fmt, int w) {
+  const std::string at = "frame " + std::to_string(i) + " (" + fmt_name(fmt) + "): ";
+  const int np = plane_count(fmt);
+  for (int k = 0; k < 3; ++k) {
+    const std::string pk = "plane[" + std::to_string(k) + "]";
+    if (k >= np) {
+      REQUIRE(p.plane[k] == nullptr, at + fmt_name(fmt) + " has " + std::to_string(np) +
+                                         (np == 1 ? " plane" : " planes") + ", but " + pk + " is given");
+      continue;
+    }
+    REQUIRE(p.plane[k] != nullptr, at + pk + " is NULL");
+    const int64_t row = (int64_t)plane_row_bytes(fmt, w, k);
+    const std::string pitch = "pitch[" + std::to_string(k) + "] = " + std::to_string(p.pitch[k]);
+    REQUIRE(p.pitch[k] >= row, at + pitch + " is below the plane's row bytes (" + std::to_string(row) + ")");
+    REQUIRE(p.pitch[k] < ((int64_t)1 << 31), at + pitch + " is 2^31 or more");
+  }
+  REQUIRE(fmt != WB_FMT_YUV420P || p.pitch[1] == p.pitch[2],
+          at + "the U and V planes need the same pitch, not pitch[1] = " + std::to_string(p.pitch[1]) +
+              " and pitch[2] = " + std::to_string(p.pitch[2]));
+  return 0;
+}
+
+static int require_camera(wb_ctx* c, int cam) {
+  REQUIRE(cam >= 0 && cam < WB_MAX_CAMERAS && c->h_cams[cam].width > 0,
+          "cam_id " + std::to_string(cam) + " has not been configured with wb_set_camera");
+  return 0;
+}
+
+// the planes of n packed frames (wb_detect / wb_submit, wb_backbone_frames, wb_profile_layers), sized by their cameras
+static int packed_frames(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t* cam_ids, int fmt,
+                         std::vector<wb_frame_planes>& planes) {
+  planes.resize(n);
+  for (int i = 0; i < n; ++i) {
+    if (int rc = require_camera(c, cam_ids[i])) return rc;
+    REQUIRE(frames[i] != nullptr, "NULL frame pointer");
+    const CameraCfg& cc = c->h_cams[cam_ids[i]];
+    planes[i] = packed_planes(frames[i], fmt, cc.width, cc.height);
   }
   return 0;
 }
@@ -661,34 +760,35 @@ static const FormatFlag kFrameFormats[] = {{WB_F_YUV420P, WB_FMT_YUV420P, "WB_F_
 // One descriptor per model image.  With use_windows and at least one camera of the batch having detection windows, the
 // batch is windowed: every window of a frame is one image (a camera without windows: one full-frame window, camera
 // -1), and s.h_win / s.d_win describe the frames for k_window_merge.  Otherwise an image is a frame, as always.  A host
-// frame is copied to the device once, whatever its window count; the windows point into that copy (or into the
-// caller's device frame).
-static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, const int32_t* cam_ids,
+// frame is copied to the device once, packed, whatever its window count; the windows point into that copy (or into the
+// caller's device planes).  frames == NULL: descriptors without pixels (wb_postprocess).  Every check comes before the
+// first copy, so a refused batch enqueues nothing.
+static int fill_desc(wb_ctx* c, Slot& s, int n, const wb_frame_planes* frames, const int32_t* cam_ids,
                      bool on_device, int fmt, cudaStream_t st, bool use_windows, int* n_images_out) {
-  std::vector<size_t> bytes(n);
+  std::vector<int2> sizes(n);
   bool windowed = false;
   int n_images = 0;
   for (int i = 0; i < n; ++i) {
     int cam = cam_ids[i];
-    REQUIRE(cam >= 0 && cam < WB_MAX_CAMERAS && c->h_cams[cam].width > 0,
-            "cam_id " + std::to_string(cam) + " has not been configured with wb_set_camera");
-    REQUIRE(frames == nullptr || frames[i] != nullptr, "NULL frame pointer");
+    if (int rc = require_camera(c, cam)) return rc;
     const CameraCfg& cc = c->h_cams[cam];
     // 4:2:0 chroma covers 2x2 pixels, 4:2:2 chroma a pixel pair of one row
     const bool yuv420 = fmt == WB_FMT_YUV420P || fmt == WB_FMT_NV12;
-    const std::string size = "cam_id " + std::to_string(cam) + " is " + std::to_string(cc.width) + "x" +
-                             std::to_string(cc.height);
+    const std::string size = "frame " + std::to_string(i) + " (" + fmt_name(fmt) + "): cam_id " + std::to_string(cam) +
+                             " is " + std::to_string(cc.width) + "x" + std::to_string(cc.height);
     REQUIRE(!yuv420 || (cc.width % 2 == 0 && cc.height % 2 == 0), size + ": 4:2:0 frames need an even width and height");
     REQUIRE(!fmt_422(fmt) || cc.width % 2 == 0, size + ": 4:2:2 frames need an even width");
-    bytes[i] = frame_bytes(fmt, cc.width, cc.height);
+    if (frames != nullptr)
+      if (int rc = check_planes(i, frames[i], fmt, cc.width)) return rc;
+    sizes[i] = make_int2(cc.width, cc.height);
     const int nw = use_windows ? (int)c->cam_windows[cam].size() : 0;
     windowed |= nw > 0;
     n_images += std::max(nw, 1);
     for (int k = 0; k < nw; ++k) {
       const int4 wd = c->cam_windows[cam][k];
-      const std::string win = "cam_id " + std::to_string(cam) + " window " + std::to_string(k) + " (" +
-                              std::to_string(wd.x) + ", " + std::to_string(wd.y) + ", " + std::to_string(wd.z) + ", " +
-                              std::to_string(wd.w) + ")";
+      const std::string win = "frame " + std::to_string(i) + " (" + fmt_name(fmt) + "): cam_id " + std::to_string(cam) +
+                              " window " + std::to_string(k) + " (" + std::to_string(wd.x) + ", " +
+                              std::to_string(wd.y) + ", " + std::to_string(wd.z) + ", " + std::to_string(wd.w) + ")";
       REQUIRE(!yuv420 || (wd.x % 2 == 0 && wd.y % 2 == 0 && wd.z % 2 == 0 && wd.w % 2 == 0),
               win + ": 4:2:0 frames need an even window origin, width and height");
       REQUIRE(!fmt_422(fmt) || (wd.x % 2 == 0 && wd.z % 2 == 0), win + ": 4:2:2 frames need an even window x and width");
@@ -697,21 +797,16 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
   REQUIRE(n_images <= c->max_batch, "the batch's detection windows add up to " + std::to_string(n_images) +
                                         " model images, more than max_batch (" + std::to_string(c->max_batch) + ")");
   if (!windowed) n_images = n;
-  std::vector<const uint8_t*> dev(n, nullptr);  // each frame on the device
-  if (frames != nullptr && on_device) {
+  std::vector<wb_frame_planes> dev(n, wb_frame_planes{});  // each frame's planes on the device
+  if (frames != nullptr) {
     dev.assign(frames, frames + n);
-  } else if (frames != nullptr) {
-    if (int rc = upload_frames(s, st, n, frames, bytes.data(), dev.data())) return rc;
+    if (!on_device)
+      if (int rc = upload_frames(s, st, n, fmt, sizes.data(), dev.data())) return rc;
   }
   int img = 0;
   for (int i = 0; i < n; ++i) {
     const int cam = cam_ids[i];
     const CameraCfg& cc = c->h_cams[cam];
-    const uint8_t* base = dev[i];
-    const ChromaLayout cl = chroma_layout(fmt, cc.width, cc.height);
-    // bytes per pixel of the packed RGB frame / luma plane / macropixels
-    const int bpp = fmt_rgb(fmt) ? rgb_layout(fmt).bpp : cl.luma_step;
-    const size_t luma0 = fmt_rgb(fmt) ? 0 : luma_origin(fmt);
     const std::vector<int4>& wins = c->cam_windows[cam];
     const int nw = windowed ? std::max((int)wins.size(), 1) : 1;
     if (windowed) {
@@ -724,22 +819,11 @@ static int fill_desc(wb_ctx* c, Slot& s, int n, const uint8_t* const* frames, co
     }
     for (int k = 0; k < nw; ++k) {
       const int4 wd = (windowed && !wins.empty()) ? wins[k] : make_int4(0, 0, cc.width, cc.height);
-      FrameDesc d;
-      d.ptr = base ? base + luma0 + ((size_t)wd.y * cc.width + wd.x) * bpp : nullptr;
-      d.chroma = base ? base + chroma_origin(fmt, cc.width, cc.height) + (size_t)(wd.y >> cl.row_shift) * cl.row +
-                            (size_t)(wd.x >> 1) * cl.step
-                      : nullptr;
-      d.w = wd.z;
-      d.h = wd.w;
-      d.pitch = cc.width * bpp;
-      d.cam = windowed ? -1 : cam;
-      d.fmt = fmt;
-      d.v_off = (int32_t)cl.v_off;
       if (windowed) {
         s.h_win[i].x[k] = wd.x;
         s.h_win[i].y[k] = wd.y;
       }
-      s.h_desc[img++] = d;
+      s.h_desc[img++] = frame_desc(dev[i], fmt, wd, windowed ? -1 : cam);
     }
   }
   CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n_images, cudaMemcpyHostToDevice, st));
@@ -766,10 +850,10 @@ struct StageHook {
   }
 };
 
-extern "C" {
-
-int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const int32_t* cam_ids, uint32_t flags) {
-  REQUIRE(c && frames && cam_ids, "NULL argument");
+// wb_submit (packed frames) and wb_submit_planes: exactly one of `packed` and `planes` is given
+static int submit(wb_ctx* c, int slot, int n, const uint8_t* const* packed, const wb_frame_planes* planes,
+                  const int32_t* cam_ids, uint32_t flags) {
+  REQUIRE(c && (packed || planes) && cam_ids, "NULL argument");
   REQUIRE(slot >= 0 && slot < WB_SLOTS, "slot out of range");
   REQUIRE(n >= 1 && n <= c->max_batch, "batch size out of range (1..max_batch)");
   std::lock_guard<std::mutex> lock(c->mu);
@@ -780,9 +864,14 @@ int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const in
   std::string err;
   const int fmt = pixel_format(flags, kFrameFormats, err);
   REQUIRE(fmt >= 0, err);
+  std::vector<wb_frame_planes> packed_as_planes;
+  if (packed) {
+    if (int rc = packed_frames(c, n, packed, cam_ids, fmt, packed_as_planes)) return rc;
+    planes = packed_as_planes.data();
+  }
   CK(cudaEventRecord(s.ev0, st));
   int n_images = n;
-  if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &n_images))
+  if (int rc = fill_desc(c, s, n, planes, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &n_images))
     return rc;
   if (int rc = enqueue_kernels(c, s, st, n_images, flags, n, s.windowed)) return rc;
   if (!(flags & WB_F_OUT_ON_DEVICE)) {
@@ -797,6 +886,17 @@ int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const in
   s.busy = true;
   c->last_launches = s.launches;
   return 0;
+}
+
+extern "C" {
+
+int wb_submit(wb_ctx* c, int slot, int n, const uint8_t* const* frames, const int32_t* cam_ids, uint32_t flags) {
+  return submit(c, slot, n, frames, nullptr, cam_ids, flags);
+}
+
+int wb_submit_planes(wb_ctx* c, int slot, int n, const wb_frame_planes* frames, const int32_t* cam_ids,
+                     uint32_t flags) {
+  return submit(c, slot, n, nullptr, frames, cam_ids, flags);
 }
 
 int wb_collect(wb_ctx* c, int slot, wb_detection* const* out, uint32_t* const* verdicts, float* gpu_ms) {
@@ -860,6 +960,12 @@ int wb_detect(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t* cam
   return wb_collect(c, 0, out, verdicts, gpu_ms);
 }
 
+int wb_detect_planes(wb_ctx* c, int n, const wb_frame_planes* frames, const int32_t* cam_ids, uint32_t flags,
+                     wb_detection* const* out, uint32_t* const* verdicts, float* gpu_ms) {
+  if (int rc = wb_submit_planes(c, 0, n, frames, cam_ids, flags)) return rc;
+  return wb_collect(c, 0, out, verdicts, gpu_ms);
+}
+
 // ---------------------------------------------------------------------------------------------------
 int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t* widths, const int32_t* heights,
                   float* out) {
@@ -868,13 +974,15 @@ int wb_preprocess(wb_ctx* c, int n, const uint8_t* const* frames, const int32_t*
   if (h.rc) return h.rc;
   Slot& s = h.s;
   cudaStream_t st = h.st;
-  std::vector<size_t> bytes(n);
-  for (int i = 0; i < n; ++i) bytes[i] = (size_t)widths[i] * heights[i] * 3;
-  std::vector<const uint8_t*> dev(n);
-  if (int rc = upload_frames(s, st, n, frames, bytes.data(), dev.data())) return rc;
+  std::vector<int2> sizes(n);
+  std::vector<wb_frame_planes> planes(n);
+  for (int i = 0; i < n; ++i) {
+    sizes[i] = make_int2(widths[i], heights[i]);
+    planes[i] = packed_planes(frames[i], WB_FMT_RGB24, widths[i], heights[i]);
+  }
+  if (int rc = upload_frames(s, st, n, WB_FMT_RGB24, sizes.data(), planes.data())) return rc;
   for (int i = 0; i < n; ++i)
-    s.h_desc[i] = FrameDesc{dev[i], dev[i] + (size_t)widths[i] * heights[i], widths[i], heights[i], widths[i] * 3, -1,
-                            WB_FMT_RGB24, 0};
+    s.h_desc[i] = frame_desc(planes[i], WB_FMT_RGB24, make_int4(0, 0, widths[i], heights[i]), -1);
   CK(cudaMemcpyAsync(s.d_desc, s.h_desc, sizeof(FrameDesc) * n, cudaMemcpyHostToDevice, st));
   LaunchCtx lc{st, &s.launches};
   launch_preprocess_f32(lc, s.d_desc, n, c->d_pre, c->hdr.input_h, c->hdr.input_w, c->hdr.pre_mul, c->hdr.pre_sub);
@@ -962,8 +1070,11 @@ int wb_backbone_frames(wb_ctx* c, int n, const uint8_t* const* frames, const int
   std::string err;
   const int fmt = pixel_format(flags, kFrameFormats, err);
   REQUIRE(fmt >= 0, err);
+  std::vector<wb_frame_planes> planes;
+  if (int rc = packed_frames(c, n, frames, cam_ids, fmt, planes)) return rc;
   int ni = n;
-  if (int rc = fill_desc(c, s, n, frames, cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &ni)) return rc;
+  if (int rc = fill_desc(c, s, n, planes.data(), cam_ids, (flags & WB_F_FRAMES_ON_DEVICE) != 0, fmt, st, true, &ni))
+    return rc;
   if (stop_layer >= 0) {
     s.launches = 0;
     if (int rc = run_program(c, s, st, ni, nullptr, 0, stop_layer)) return rc;
@@ -1044,7 +1155,9 @@ int wb_profile_layers(wb_ctx* c, int n, const uint8_t* const* device_frames, con
   if (h.rc) return h.rc;
   Slot& s = h.s;
   cudaStream_t st = h.st;
-  if (int rc = fill_desc(c, s, n, device_frames, cam_ids, true, WB_FMT_RGB24, st, false, nullptr)) return rc;
+  std::vector<wb_frame_planes> planes;
+  if (int rc = packed_frames(c, n, device_frames, cam_ids, WB_FMT_RGB24, planes)) return rc;
+  if (int rc = fill_desc(c, s, n, planes.data(), cam_ids, true, WB_FMT_RGB24, st, false, nullptr)) return rc;
   const int nl = (int)c->layers.size();
   REQUIRE(max_launches >= nl + 1, "max_launches too small");
   std::vector<Event> ev(nl + 2);  // entry i is timed from ev[i] to ev[i + 1]

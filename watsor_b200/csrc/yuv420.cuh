@@ -59,20 +59,20 @@ struct ChromaLayout {
   int step;       // bytes between horizontally adjacent U samples
   int row;        // bytes between chroma rows
   int row_shift;  // luma row y has chroma row y >> row_shift: 1 (4:2:0, one per two luma rows), 0 (4:2:2, one per row)
-  size_t v_off;   // V sample = U sample + v_off
+  ptrdiff_t v_off;  // V sample = U sample + v_off
 };
 
-// the layout of a YUV frame, or of a window of one, whose luma rows are `pitch` bytes apart; v_off is only read for
-// yuv420p, where it is the parent frame's (w/2) * (h/2)
-__host__ __device__ __forceinline__ ChromaLayout chroma_layout_of(int fmt, int pitch, size_t v_off) {
-  if (fmt_422(fmt)) return ChromaLayout{2, 4, pitch, 0, 2};
-  if (fmt == WB_FMT_NV12) return ChromaLayout{1, 2, pitch, 1, 1};
-  return ChromaLayout{1, 1, pitch / 2, 1, v_off};
+// the layout of a YUV frame, or of a window of one, whose chroma rows are `row` bytes apart (4:2:2: the macropixel
+// rows); v_off is only read for yuv420p, where it is the distance from the U plane to the V plane, of either sign
+__host__ __device__ __forceinline__ ChromaLayout chroma_layout_of(int fmt, int row, ptrdiff_t v_off) {
+  if (fmt_422(fmt)) return ChromaLayout{2, 4, row, 0, 2};
+  if (fmt == WB_FMT_NV12) return ChromaLayout{1, 2, row, 1, 1};
+  return ChromaLayout{1, 1, row, 1, v_off};
 }
 
 // the layout of a packed w x h frame
 __host__ __device__ __forceinline__ ChromaLayout chroma_layout(int fmt, int w, int h) {
-  return chroma_layout_of(fmt, fmt_422(fmt) ? 2 * w : w, (size_t)(w / 2) * (h / 2));
+  return chroma_layout_of(fmt, fmt_422(fmt) ? 2 * w : fmt == WB_FMT_NV12 ? w : w / 2, (ptrdiff_t)(w / 2) * (h / 2));
 }
 
 // byte offsets, from the first byte of a packed w x h frame, of the Y and the U sample of pixel (0, 0)
@@ -84,6 +84,23 @@ __host__ __device__ __forceinline__ size_t chroma_origin(int fmt, int w, int h) 
 // bytes of one packed frame
 __host__ __device__ __forceinline__ size_t frame_bytes(int fmt, int w, int h) {
   return fmt_rgb(fmt) ? (size_t)w * h * rgb_layout(fmt).bpp : fmt_422(fmt) ? (size_t)w * h * 2 : (size_t)w * h * 3 / 2;
+}
+
+// A frame as planes (wb_frame_planes): the RGB formats and 4:2:2 have one plane, the pixel rows; NV12 two, Y and the
+// interleaved UV pairs; yuv420p three, Y, U and V.  A packed frame is its planes stored back to back, each with rows of
+// plane_row_bytes, so plane k starts plane_offset(k) bytes after plane 0.
+__host__ __device__ __forceinline__ int plane_count(int fmt) {
+  return fmt == WB_FMT_YUV420P ? 3 : fmt == WB_FMT_NV12 ? 2 : 1;
+}
+__host__ __device__ __forceinline__ int plane_rows(int h, int k) { return k > 0 ? h / 2 : h; }
+__host__ __device__ __forceinline__ size_t plane_row_bytes(int fmt, int w, int k) {
+  return fmt_rgb(fmt) ? (size_t)w * rgb_layout(fmt).bpp : fmt_422(fmt) ? (size_t)w * 2
+         : k == 0 || fmt == WB_FMT_NV12 ? (size_t)w : (size_t)(w / 2);
+}
+__host__ __device__ __forceinline__ size_t plane_offset(int fmt, int w, int h, int k) {
+  size_t off = 0;
+  for (int j = 0; j < k; ++j) off += plane_row_bytes(fmt, w, j) * plane_rows(h, j);
+  return off;
 }
 
 // address of the U sample of pixel (x, y) given that of pixel (0, 0); the V sample is at + v_off.  A window of a frame

@@ -113,12 +113,16 @@ class B200ObjectDetector(object):
         the 4-byte 'rgba' / 'bgra' (H, W, 4) of GPU pipelines (alpha ignored); the 4:2:0 layouts decoders emit,
         'yuv420p' / 'nv12' (H*3//2, W); or the packed 4:2:2 layouts of webcams and capture cards, 'yuyv422' /
         'uyvy422' (H, W, 2).  All are converted on the GPU exactly as cv2.cvtColor converts them to RGB24.  One format
-        per batch."""
+        per batch.  A frame may also be a tuple of its planes (engine.layout_planes) with row pitches of their own:
+        arrays or tensors whose first dimension counts rows (an AVFrame's data[i] viewed with linesize[i], a crop of a
+        larger frame) or, with frames_on_device, (device address, pitch) pairs such as a decoder surface's.  Device
+        planes are read in place; host planes are packed as they are uploaded."""
         flags = (_lib.WB_F_FUSE_FILTERS if fuse_filters else 0) | \
                 (_lib.WB_F_FRAMES_ON_DEVICE if frames_on_device else 0)
         return self.engine.detect(frames, cam_ids, detections, verdicts, flags, pixel_format)
 
     def submit(self, slot, frames, cam_ids, fuse_filters=True, frames_on_device=False, pixel_format='rgb24'):
+        """detect_batch's frames (planes too), enqueued on `slot`; they must stay valid until `collect`"""
         flags = (_lib.WB_F_FUSE_FILTERS if fuse_filters else 0) | \
                 (_lib.WB_F_FRAMES_ON_DEVICE if frames_on_device else 0)
         self.engine.submit(slot, frames, cam_ids, flags, pixel_format)

@@ -57,6 +57,66 @@ def layout_shape(pixel_format, width, height):
     return (height * 3 // 2, width)
 
 
+def layout_planes(pixel_format, width, height):
+    """(rows, row bytes) of each plane of a `width` x `height` frame in `pixel_format`, in the order wb_frame_planes
+    takes them (include/watsor_b200.h): one plane for the RGB byte orders and the packed 4:2:2 formats, the pixel rows;
+    two for nv12, Y and the interleaved (U, V) pairs; three for yuv420p, Y, U and V.  The sizes layout_shape refuses
+    are refused here too."""
+    layout_shape(pixel_format, width, height)
+    if pixel_format in _BYTES_PER_PIXEL:
+        return ((height, width * _BYTES_PER_PIXEL[pixel_format]),)
+    if pixel_format in ('yuyv422', 'uyvy422'):
+        return ((height, width * 2),)
+    if pixel_format == 'nv12':
+        return ((height, width), (height // 2, width))
+    return ((height, width), (height // 2, width // 2), (height // 2, width // 2))
+
+
+def plane_address(plane, rows, row_bytes, on_device, where):
+    """(address, pitch) of one plane of a frame given as planes.  `plane` is a uint8 numpy array or torch tensor whose
+    first dimension counts the plane's `rows` and whose other dimensions hold one row's `row_bytes` densely (a view
+    such as big[y0:y1, x0:x1] qualifies): the pitch is the first dimension's stride.  Device planes
+    (`on_device`) are CUDA tensors or (address, pitch) pairs from any other library, which the C library checks.
+    rows None: a camera this engine does not know, whose size the library checks.  Raises ValueError naming `where`."""
+    if isinstance(plane, tuple):
+        if not on_device:
+            raise ValueError('%s: an (address, pitch) pair is a device plane; pass frames_on_device=True' % where)
+        if len(plane) != 2:
+            raise ValueError('%s: a device plane is an (address, pitch) pair, not %d values' % (where, len(plane)))
+        return int(plane[0]), int(plane[1])
+    if isinstance(plane, np.ndarray):
+        if on_device:
+            raise ValueError('%s: a numpy array is host memory, but frames_on_device is set' % where)
+        dtype_ok, shape, strides, addr = plane.dtype == np.uint8, plane.shape, plane.strides, plane.ctypes.data
+    elif type(plane).__module__.split('.')[0] == 'torch':
+        import torch
+        if plane.is_cuda != bool(on_device):
+            raise ValueError('%s: a %s tensor, but frames_on_device is %s' % (
+                where, 'CUDA' if plane.is_cuda else 'CPU', bool(on_device)))
+        dtype_ok, shape, strides = plane.dtype == torch.uint8, tuple(plane.shape), plane.stride()
+        addr = plane.data_ptr()
+    else:
+        raise ValueError('%s: a plane is a uint8 numpy array or torch tensor%s, not %s' % (
+            where, ' or an (address, pitch) pair' if on_device else '', type(plane).__name__))
+    if not dtype_ok or len(shape) < 1:
+        raise ValueError('%s: a plane is a uint8 array of at least one dimension, not %s of shape %s' % (
+            where, getattr(plane, 'dtype', '?'), shape))
+    dense, step = True, 1
+    for n, st in reversed(list(zip(shape[1:], strides[1:]))):
+        dense &= n == 1 or st == step
+        step *= n
+    if not dense:
+        raise ValueError('%s: the bytes of a row must be dense (strides %s for shape %s)' % (where, strides, shape))
+    if rows is not None and (shape[0] != rows or step != row_bytes):
+        raise ValueError('%s: %d rows of %d bytes expected, not %d rows of %d bytes (shape %s)' % (
+            where, rows, row_bytes, shape[0], step, shape))
+    pitch = strides[0] if shape[0] > 1 or strides[0] >= step else step    # numpy may give one row any stride
+    if pitch < step:
+        raise ValueError('%s: the row pitch %d is below the row bytes %d (rows overlap or run bottom-up)' % (
+            where, pitch, step))
+    return addr, pitch
+
+
 def frame_shape(pixel_format, width, height):
     """layout_shape for the RGB24 and YUV layouts of PIXEL_FORMATS, the names this function has always taken; it
     refuses the other RGB byte orders (bgr24, rgba, bgra) as it always has, and layout_shape gives their shapes."""
@@ -192,10 +252,40 @@ class Engine:
         check(self.lib.wb_unregister_host(self._ctx, address))
 
     # ------------------------------------------------------------------ hot path
-    def _io(self, frames, cam_ids, out, verdicts):
+    def _frame_planes(self, frames, cam_ids, pixel_format, on_device):
+        """wb_frame_planes of a batch with at least one frame given as a tuple of planes (see plane_address); the
+        batch's packed frames become the planes at their packed offsets"""
+        arr = (_lib.FramePlanes * len(frames))()
+        for i, (frame, cam) in enumerate(zip(frames, cam_ids)):
+            size = self.cameras.get(cam)
+            layout = layout_planes(pixel_format, *size) if size is not None else None
+            if isinstance(frame, tuple):
+                if layout is not None and len(frame) != len(layout):
+                    raise ValueError('frame %d: a %s frame has %d plane%s, not %d' % (
+                        i, pixel_format, len(layout), 's' if len(layout) > 1 else '', len(frame)))
+                for k, plane in enumerate(frame[:3]):
+                    rows, row_bytes = layout[k] if layout is not None else (None, None)
+                    where = 'frame %d (%s) plane %d' % (i, pixel_format, k)
+                    arr[i].plane[k], arr[i].pitch[k] = plane_address(plane, rows, row_bytes, on_device, where)
+                continue
+            if isinstance(frame, np.ndarray) and on_device:
+                raise ValueError('frame %d: a numpy array is host memory, but frames_on_device is set' % i)
+            addr = _addr(frame)
+            offset = 0
+            for k, (rows, row_bytes) in enumerate(layout or ((0, 0),)):
+                arr[i].plane[k], arr[i].pitch[k] = addr + offset, row_bytes
+                offset += rows * row_bytes
+        return arr
+
+    def _io(self, frames, cam_ids, out, verdicts, pixel_format='rgb24', flags=0):
+        """ctypes arguments of a batch; fp is a wb_frame_planes array when a frame is a tuple of planes, else the
+        frames' addresses"""
         n = len(frames)
         assert n == len(cam_ids)
-        fp = _ptr_array([_addr(f) for f in frames])
+        if any(isinstance(f, tuple) for f in frames):
+            fp = self._frame_planes(frames, cam_ids, pixel_format, flags & _lib.WB_F_FRAMES_ON_DEVICE)
+        else:
+            fp = _ptr_array([_addr(f) for f in frames])
         cams = (c_int32 * n)(*cam_ids)
         op = _ptr_array([_addr(o) for o in out]) if out is not None else None
         vp = _ptr_array([_addr(v) for v in verdicts]) if verdicts is not None else None
@@ -211,18 +301,24 @@ class Engine:
     def detect(self, frames, cam_ids, out, verdicts=None, flags=0, pixel_format='rgb24'):
         """frames: host uint8 arrays (or device pointers with WB_F_FRAMES_ON_DEVICE) in `pixel_format`
         (a name of FRAME_FORMATS: 'rgb24', 'bgr24', 'rgba', 'bgra', 'yuv420p', 'nv12', 'yuyv422' or 'uyvy422', see
-        layout_shape); out: per frame a `Detection*100` ctypes array / address.
+        layout_shape); out: per frame a `Detection*100` ctypes array / address.  A frame may also be a tuple of its
+        planes (layout_planes), each an array or tensor with row padding of its own or an (address, pitch) pair on
+        the device (plane_address): decoder surfaces and ffmpeg frames, read without packing them first.
         Returns device ms."""
         flags |= self._format_flags(frames, cam_ids, pixel_format)
-        n, fp, cams, op, vp = self._io(frames, cam_ids, out, verdicts)
+        n, fp, cams, op, vp = self._io(frames, cam_ids, out, verdicts, pixel_format, flags)
         ms = c_float(0)
-        check(self.lib.wb_detect(self._ctx, n, fp, cams, flags, op, vp, byref(ms)))
+        fn = self.lib.wb_detect_planes if fp._type_ is _lib.FramePlanes else self.lib.wb_detect
+        check(fn(self._ctx, n, fp, cams, flags, op, vp, byref(ms)))
         return ms.value
 
     def submit(self, slot, frames, cam_ids, flags=0, pixel_format='rgb24'):
+        """`detect`'s frames, enqueued on `slot`; `collect` returns the results.  The frames, and every plane of a
+        frame given as planes, must stay valid until then."""
         flags |= self._format_flags(frames, cam_ids, pixel_format)
-        n, fp, cams, _, _ = self._io(frames, cam_ids, None, None)
-        check(self.lib.wb_submit(self._ctx, slot, n, fp, cams, flags))
+        n, fp, cams, _, _ = self._io(frames, cam_ids, None, None, pixel_format, flags)
+        fn = self.lib.wb_submit_planes if fp._type_ is _lib.FramePlanes else self.lib.wb_submit
+        check(fn(self._ctx, slot, n, fp, cams, flags))
 
     def collect(self, slot, out=None, verdicts=None):
         op = _ptr_array([_addr(o) for o in out]) if out is not None else None
